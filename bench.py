@@ -1,11 +1,11 @@
 #!/usr/bin/env python
-"""bench.py — POST label throughput (labels/s) of the B200 engine, per the driver's contract.
+"""bench.py — POST label throughput (labels/s) of the GPU engine on one H100 (or N with torchrun).
 
-Workload (BASELINE.json configs[1]): 4-SU init, scrypt N = 8192, r = p = 1, single B200, labels
+Workload (BASELINE.json configs[1]): 4-SU init, scrypt N = 8192, r = p = 1, single H100, labels
 discarded ("/dev/null").  One *step* = one batch of `--batch` consecutive labels of the 2^34-label
-index space (default: 72 layers of resident scratchpads ~ 5.5 M labels ~ 3 s, so that the driver's 20 steps sample
-~10^8 labels / a minute of steady state per arm; the reference's default ComputeBatchSize is 2^20), exactly what one `initialize(start, end)`
-call of the reference's initializer does per ComputeBatchSize batch (activation/post.go:295).
+index space (default: DEFAULT_BATCH, a fixed count so that the same arguments always compute the same labels; 64 layers
+of an 80 GB H100's resident scratchpads, ~2 s per step; the reference's default ComputeBatchSize is 2^20), exactly what
+one `initialize(start, end)` call of the reference's initializer does per ComputeBatchSize batch (activation/post.go:295).
 
   value      labels/s with the output resident in HBM (b200post_labels_range_dev), device-timed
   e2e        labels/s through the host-buffer C-ABI call (b200post_labels_range): commitment H2D and
@@ -13,6 +13,9 @@ call of the reference's initializer does per ComputeBatchSize batch (activation/
   roofline   the ROMix kernel against the measured HBM copy bandwidth; algorithmic bytes =
              2*128*N + 16 = 2 097 168 B/label (SURVEY.md §8d)
   cpu_baseline  the oracle port on this box's host cores (bounded sample)
+
+`--dump-outputs DIR` writes what the last timed step returned (a seeded sample of its labels, their indices and the
+step's VRF candidate) as float32/float64 .npy files, so that two builds can be compared output for output.
 
 N > 1 (torchrun): one process per GPU, contiguous index shards, no data-path collective; the only
 exchange is an NCCL all-gather of one 48-byte VRF candidate per rank per step (SURVEY.md §8e).
@@ -39,8 +42,11 @@ N_SCRYPT = 8192
 BYTES_PER_LABEL = 2 * 128 * N_SCRYPT + 16          # algorithmic HBM bytes per label (SURVEY.md §8d)
 NUM_LABELS_4SU = 4 * 2**32
 METRIC = "POST labels/sec (scrypt N=8192 init)"
-ALU_OPS_PER_BLOCKMIX = 553                         # alu-pipe SASS instructions per BlockMix of the shipped kernel (profiles/)
-HBM_FALLBACK_GBS = 6650.0                          # /opt/skills/guides/B200_PROFILING.md fallback
+ALU_OPS_PER_BLOCKMIX = 566                         # alu-pipe SASS instructions (LOP3/SHF/LEA) per BlockMix in the sm_90a main loop of romix_pipe_kernel
+NOMINAL_SM_HZ = 1.98e9                             # H100 SXM maximum SM clock, used when nvidia-smi gives no sample
+HBM_FALLBACK_GBS = 3350.0                          # H100 SXM data sheet (HBM3)
+DEFAULT_BATCH = 64 * 132 * 256                     # labels per step: 64 layers of an 80 GB H100 at N = 8192 (132 SMs x 256 slots)
+DUMP_ROWS = 1 << 18                                # labels sampled into --dump-outputs (16 MiB as float32)
 
 
 def measured_peaks():
@@ -50,7 +56,7 @@ def measured_peaks():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:  # noqa: BLE001
             pass
-    return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
+    return HBM_FALLBACK_GBS, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
@@ -159,7 +165,7 @@ def _valid_proofs(b2, vf, pr, provider: int, n_identities: int, k2: int, labels_
 
 
 def bench_verify(b2, provider: int, orc=None, n_proofs: int = 10000, k2: int = 37) -> dict:
-    """BASELINE.json configs[2]: PostVerifier batch, 10 000 proofs x K2 = 37 indices, N = 8192, one B200.
+    """BASELINE.json configs[2]: PostVerifier batch, 10 000 proofs x K2 = 37 indices, N = 8192, one GPU.
     MIXED batch: half the proofs are VALID (real proofs of small POSTs initialised and proven on this GPU, repeated),
     half have one index bumped (systest/tests/distributed_post_verification_test.go:254-256) and are rejected at a known
     position.  Timed end to end through b200post_verify_batch with host buffers: index unpack + key derivation (host),
@@ -254,6 +260,22 @@ def bench_verify(b2, provider: int, orc=None, n_proofs: int = 10000, k2: int = 3
     return res
 
 
+def dump_outputs(out_dir: Path, d_out, first_index: int, vrf) -> None:
+    """The last timed step's outputs: DUMP_ROWS of its labels (rows chosen by a fixed seed), their label indices and the
+    VRF candidate of the step (index -1 and label32 all 255 when the step had none)."""
+    import numpy as np
+    import torch
+    out_dir.mkdir(parents=True, exist_ok=True)
+    n = d_out.shape[0]
+    rows = np.sort(np.random.default_rng(0).choice(n, size=min(n, DUMP_ROWS), replace=False))
+    labels = d_out[torch.from_numpy(rows).to(d_out.device)].cpu().numpy()
+    np.save(out_dir / "labels.npy", labels.astype(np.float32))
+    np.save(out_dir / "label_index.npy", (first_index + rows).astype(np.float64))
+    index, label32 = vrf if vrf is not None else (-1, b"\xff" * 32)
+    np.save(out_dir / "vrf_index.npy", np.array([index], dtype=np.float64))
+    np.save(out_dir / "vrf_label32.npy", np.frombuffer(label32, dtype=np.uint8).astype(np.float32))
+
+
 def _timed(fn) -> float:
     t0 = time.perf_counter()
     fn()
@@ -336,10 +358,11 @@ def main() -> None:
     ap.add_argument("--steps", type=int, default=8)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
-    ap.add_argument("--batch", type=int, default=0, help="labels per step per GPU (0 = 72 layers of resident scratchpads ~ 5.5 M labels ~ 3 s: 20 steps sample ~ 10^8 labels / 60 s of steady state, SURVEY.md §8d cfg2)")
+    ap.add_argument("--batch", type=int, default=DEFAULT_BATCH, help="labels per step per GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-verify", action="store_true", help="skip the configs[2] verify-batch measurement")
     ap.add_argument("--no-k2pow", action="store_true", help="skip the configs[4] k2pow (RandomX) measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write rank 0's outputs of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -377,7 +400,7 @@ def main() -> None:
 
     wave = b2.wave_slots(N_SCRYPT, provider=local_rank)                    # resident scratchpads per wave
     tpb = b2.get_option("tpb")
-    batch = args.batch or 72 * wave
+    batch = args.batch
     d_out = torch.empty((batch, 16), dtype=torch.uint8, device=dev)        # labels stay in HBM for `value`
     h_out = np.empty((batch, 16), dtype=np.uint8)                          # host sink for `e2e`
 
@@ -419,11 +442,13 @@ def main() -> None:
         return el, bracket_ms, calls_ms
 
     debug = bool(os.environ.get("B200POST_BENCH_DEBUG"))
+    last = {}                                       # what the most recent device-resident step returned
 
     def step_dev(s: int):
         t_a = time.perf_counter()
         vrf = b2.labels_range_dev(commitment, N_SCRYPT, shard_start(s), batch, d_out.data_ptr(), provider=local_rank,
                                   vrf_difficulty_=diff)
+        last.update(step=s, vrf=vrf)
         t_b = time.perf_counter()
         exchange(vrf)
         if debug:
@@ -451,6 +476,8 @@ def main() -> None:
     clocks = sampler.stop() if rank == 0 else None
     launches = b2.launch_count() - launches0
     romix_ms, romix_k, romix_labels = b2.romix_time(provider=local_rank, reset=True)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), d_out, shard_start(last["step"]), last["vrf"])
 
     # ---- end-to-end arm (host buffers through the reference-facing C-ABI call)
     for w in range(2):
@@ -467,16 +494,6 @@ def main() -> None:
     labels_per_launch = romix_labels / max(romix_k, 1)     # label-equivalents per ROMix launch (engine-counted)
     romix_avg_ms = romix_ms / max(romix_k, 1)
     achieved = labels_per_launch * BYTES_PER_LABEL / (romix_avg_ms / 1e3) / 1e9 if romix_avg_ms > 0 else 0.0
-    # dram__bytes of one launch comes from an `ncu --set full` capture (a number measured under ncu is never a bench value,
-    # so it cannot be taken live here); the file records which build it was captured on
-    traffic, traffic_src = None, None
-    tfile = ROOT / "profiles" / "romix_dram_bytes_per_launch.json"
-    if tfile.exists():
-        try:
-            tj = json.loads(tfile.read_text())
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("captured_on", "build not recorded in the file")
-        except Exception:  # noqa: BLE001
-            traffic = None
 
     verify_extra = None
     k2pow_extra = None
@@ -515,7 +532,7 @@ def main() -> None:
             "config": {"workload": "4-SU POST init (2^34 labels/GPU), scrypt-jane (ChaCha20/8 + Keccak-512) N=8192 r=1 p=1, labels discarded (/dev/null sink)",
                        "labels_per_step_per_gpu": batch, "wave_slots": wave, "provider": prov["model"],
                        "romix_variant": b2.get_option("romix_variant"), "rotate_mask": b2.get_option("rotate_mask"),
-                       "tpb": tpb, "l2": "working set = wave_slots x 1 MiB scratch >> 126 MB L2; every step uses fresh indices",
+                       "tpb": tpb, "l2": "working set = wave_slots x 2 MiB scratch >> 50 MB L2; every step uses fresh indices",
                        "parallelism": f"index-range shards x{world}, NCCL all-gather of one 48-B VRF record per step" if world > 1 else "single GPU",
                        "timer": "two CUDA events on the engine's launching stream bracketing the K steps (barrier + synchronize on both sides), max over ranks",
                        "value_from_call_times_only": total_labels / (calls_ms / 1e3) if calls_ms > 0 else None,
@@ -523,13 +540,13 @@ def main() -> None:
             "e2e": {"value": e2e_value, "unit": "labels/s", "h2d_bytes_per_step": 32 + 32, "d2h_bytes_per_step": batch * 16 + 48},
             "gpu_launches": int(launches),
             "roofline": {"bound": "hbm", "kernel": "romix_pipe_kernel" if b2.get_option("romix_variant") == 4 else "romix_kernel", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak if peak else None, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
-                         # integer roofline of the label function: 2N BlockMix x 553 alu-pipe instructions (512 XOR/rotate
-                         # of two ChaCha20/8 cores + 41 XOR/address, counted in the SASS) = 9.06 M per label, at the
-                         # measured 64 ops/clk/SM (profiles/r01_alubench.log) and the maximum SM clock
-                         "int_roofline_labels_per_s": prov["sm_count"] * 64 * (clocks["sm_mhz"] * 1e6 if clocks and clocks.get("sm_mhz") else 1.965e9) / (16384 * ALU_OPS_PER_BLOCKMIX),
-                         "int_roofline_at_max_clock_labels_per_s": prov["sm_count"] * 64 * (clocks["sm_max_mhz"] * 1e6 if clocks and clocks.get("sm_max_mhz") else 1.965e9) / (16384 * ALU_OPS_PER_BLOCKMIX),
-                         "int_roofline_clock": "median SM clock sampled during the timed region" if clocks and clocks.get("sm_mhz") else "nominal 1.965 GHz (no nvidia-smi sample)",
+                         "frac": achieved / peak if peak else None, "peak_source": peak_src,
+                         # integer roofline of the label function: 2N BlockMix x ALU_OPS_PER_BLOCKMIX alu-pipe instructions
+                         # (XOR/rotate of two ChaCha20/8 cores + XOR/address, counted in the SASS) per label, at the
+                         # 64 INT32 logic/shift results per clock per SM of compute capability 9.0 and the SM clock
+                         "int_roofline_labels_per_s": prov["sm_count"] * 64 * (clocks["sm_mhz"] * 1e6 if clocks and clocks.get("sm_mhz") else NOMINAL_SM_HZ) / (16384 * ALU_OPS_PER_BLOCKMIX),
+                         "int_roofline_at_max_clock_labels_per_s": prov["sm_count"] * 64 * (clocks["sm_max_mhz"] * 1e6 if clocks and clocks.get("sm_max_mhz") else NOMINAL_SM_HZ) / (16384 * ALU_OPS_PER_BLOCKMIX),
+                         "int_roofline_clock": "median SM clock sampled during the timed region" if clocks and clocks.get("sm_mhz") else "nominal 1.98 GHz (no nvidia-smi sample)",
                          "alu_ceiling_labels_per_s": alu_probe,
                          "frac_of_alu_ceiling": (labels_per_launch / (romix_avg_ms / 1e3) / alu_probe) if alu_probe and romix_avg_ms > 0 else None,
                          "bytes_per_label": BYTES_PER_LABEL, "labels_per_launch": labels_per_launch,

@@ -1,6 +1,6 @@
-"""go-spacemesh_b200 — B200-native POST label engine (host bindings over the C ABI).
+"""go-spacemesh_b200 — GPU-native POST label engine (host bindings over the C ABI).
 
-The product is ``libb200post.so`` (hand-written sm_100a CUDA + a C++ host runtime, built from
+The product is ``libb200post.so`` (hand-written sm_90a CUDA + a C++ host runtime, built from
 ``csrc/``); this module is the thin ctypes layer the tests, ``bench.py`` and ``__graft_entry__`` use,
 named after the reference interfaces it stands behind (activation/post.go, post_verifier.go).
 
@@ -49,7 +49,7 @@ class VrfNonce(ctypes.Structure):
 
 
 def build(verbose: bool = False) -> Path:
-    """Compile libb200post.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+    """Compile libb200post.so in-tree with nvcc for sm_90a (cross-compiles without a GPU)."""
     cmd = ["make", "-C", str(_HERE / "csrc"), "-j4"]
     res = subprocess.run(cmd, capture_output=not verbose, text=True)
     if res.returncode != 0:

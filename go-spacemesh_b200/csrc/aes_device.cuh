@@ -1,4 +1,4 @@
-// aes_device.cuh — AES-128 single-block encryption for sm_100a kernels (FIPS-197, T-table form).
+// aes_device.cuh — AES-128 single-block encryption for sm_90a kernels (FIPS-197, T-table form).
 //
 // Used by the verify epilogue and the proving scan: one 16-byte label is encrypted under a per-proof key and
 // ciphertext bytes are compared with the proving difficulty (ASSUMED post-rs Prover8_56 scheme, see

@@ -1,7 +1,7 @@
 // engine.cu — layer scheduler for the POST label kernels (see engine.h).
 //
 // Mirrors what the reference's initializer does around libpost's `initialize()` (activation/post.go:295:
-// batches of ComputeBatchSize labels, cancellable, progress observable) but sized for a B200.  A *layer*
+// batches of ComputeBatchSize labels, cancellable, progress observable) but sized for the GPU.  A *layer*
 // is one label per resident slot (threads x SMs that fit the registers and the HBM scratch).  With the
 // pipelined ROMix kernel the stream carries, for layer m:
 //     K1(m)  ->  K2p{ mix layer m-1 | fill layer m }  ->  K3(m-1)        (and on the copy stream: D2H(m-1))
@@ -102,22 +102,37 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
         CU_TRY(cudaMalloc(&d_running_, sizeof(VrfCandidate)));
         CU_TRY(cudaMallocHost(&h_running_, sizeof(VrfCandidate)));
     }
-    variant_ = variant; mw_ = mw; tpb_ = tpb; dr_unroll_ = dr;
-    int ctas = romix_max_ctas_per_sm(variant, mw, tpb, dr);
-    if (ctas <= 0) { set_error("romix kernel cannot be resident (unsupported variant / mask / tpb combination)"); return B200POST_ERR_INVALID_ARGUMENT; }
-    const int64_t want_ctas = o.ctas_per_sm.load();
-    if (want_ctas > 0) ctas = std::min<int>(ctas, (int)want_ctas);
-
     const size_t pads = variant == ROMIX_PIPELINED ? 2 : 1;   // scratchpads per slot
     const size_t per_slot = 128 * (size_t)N * pads;
     size_t free_b = 0, total_b = 0;
     CU_TRY(cudaMemGetInfo(&free_b, &total_b));
-    size_t budget = (size_t)((double)(free_b + v_bytes_) * 0.95);   // 0.95: one layer (148 GiB at defaults) still fits after the k2pow engine (dataset 2 GiB + a batch of scratchpads, ~16 GiB) has allocated first
+    size_t budget = (size_t)((double)(free_b + v_bytes_) * 0.95);   // 0.95: headroom for the k2pow engine's dataset and scratchpads (~14 GiB) when it allocates after this one
     const int64_t cap_mib = o.max_scratch_mib.load();
     if (cap_mib > 0) budget = std::min(budget, (size_t)cap_mib << 20);
-    const size_t per_cta_layer = per_slot * (size_t)tpb * (size_t)prop_.multiProcessorCount;
-    while (ctas > 1 && per_cta_layer * (size_t)ctas > budget) ctas--;
-    uint64_t wave = (uint64_t)prop_.multiProcessorCount * (uint64_t)ctas * (uint64_t)tpb;
+    const size_t sms = (size_t)prop_.multiProcessorCount;
+    const int64_t want_ctas = o.ctas_per_sm.load();
+    // resident CTAs per SM of `t` threads: the occupancy limit, the option, then what the HBM budget holds
+    auto ctas_for = [&](int t) {
+        int c = romix_max_ctas_per_sm(variant, mw, t, dr);
+        if (want_ctas > 0) c = std::min<int>(c, (int)want_ctas);
+        while (c > 0 && per_slot * (size_t)t * sms * (size_t)c > budget) c--;
+        return c;
+    };
+    if (romix_max_ctas_per_sm(variant, mw, tpb, dr) <= 0) { set_error("romix kernel cannot be resident (unsupported variant / mask / tpb combination)"); return B200POST_ERR_INVALID_ARGUMENT; }
+    int ctas = ctas_for(tpb);
+    // HBM, not the register file, bounds the pipelined layer when it cannot give every SM one CTA of `tpb` slots: an
+    // 80 GB H100 holds ~36 k slots at N = 8192, while 132 SMs x 512 threads would take 67 k, and a 512-thread grid of
+    // 36 k slots leaves half of the SMs idle.  Smaller CTAs (down to 64 threads) then spread the layer over every SM;
+    // the size that puts the most slots on the device wins.
+    if (variant == ROMIX_PIPELINED) {
+        for (int t = tpb / 2; t >= 64; t /= 2) {
+            const int c = ctas_for(t);
+            if ((uint64_t)c * t > (uint64_t)ctas * tpb) { ctas = c; tpb = t; }
+        }
+    }
+    if (ctas == 0) ctas = 1;   // not even one CTA per SM fits: the layer shrinks below
+    variant_ = variant; mw_ = mw; tpb_ = tpb; dr_unroll_ = dr;
+    uint64_t wave = (uint64_t)sms * (uint64_t)ctas * (uint64_t)tpb;
     if (per_slot * wave > budget) {
         // not even one CTA per SM: shrink to what fits, in whole warps (the kernels take any multiple of 32)
         wave = budget / per_slot / 32 * 32;

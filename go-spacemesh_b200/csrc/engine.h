@@ -1,4 +1,4 @@
-// engine.h — host runtime of the B200 POST label engine: per-device scratch, layer scheduling,
+// engine.h — host runtime of the POST label engine: per-device scratch, layer scheduling,
 // double-buffered staging.  C++ because the reference's host side for this path is compiled code
 // (Go: activation/post.go PostSetupManager, activation/post_verifier.go); the Go toolchain is absent
 // in this image (INTEGRATION.md shows the cgo binding that sits on top of the C ABI).
@@ -18,7 +18,7 @@ namespace b200post {
 struct Options {
     std::atomic<int64_t> romix_variant{ROMIX_PIPELINED};
     std::atomic<int64_t> rotate_mask{0};
-    std::atomic<int64_t> tpb{512};             // pipelined default: one 16-warp CTA per SM (measured best)
+    std::atomic<int64_t> tpb{512};             // CTA size; the pipelined kernel takes smaller CTAs when HBM cannot give every SM one of this size
     std::atomic<int64_t> dr_unroll{4};         // pipelined kernel: ChaCha double-rounds unrolled (4) or rolled (1)
     std::atomic<int64_t> ctas_per_sm{0};       // 0 = occupancy maximum
     std::atomic<int64_t> max_scratch_mib{0};   // 0 = 95 % of free HBM

@@ -1,4 +1,4 @@
-// label_kernels.cu — hand-written sm_100a kernels for the POST label path (see label_kernels.cuh).
+// label_kernels.cu — hand-written sm_90a kernels for the POST label path (see label_kernels.cuh).
 #include "label_kernels.cuh"
 
 namespace b200post {
@@ -9,7 +9,7 @@ namespace b200post {
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
 // Scratchpad accesses are streaming (.cs = evict-first): V is written once and read about once, and a
-// wave's scratch (tens of GiB) never fits the 126 MB L2.  (Default and .cg policies measured the same.)
+// wave's scratch (tens of GiB) never fits the 50 MB L2.  (Default and .cg policies measured the same.)
 __device__ __forceinline__ uint4 ld_stream(const uint4 *p) {
     uint4 v;
     asm volatile("ld.global.cs.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
@@ -240,9 +240,9 @@ __global__ void __launch_bounds__(TPB) romix_kernel(const RomixParams p) {
 // each — so its latency floor on this clock is ~7 ms however many lanes are thrown at it (splitting a core over four
 // lanes leaves the chain as long and adds shuffles: a single lane already issues the four independent quarter rounds
 // back to back).  What CAN be removed is everything the throughput kernel adds for a full wave: here a label gets a
-// lane, labels are spread over as many WARPS as there are scheduler slots (148 x 4) so that every label's warp issues
-// every cycle, and the scratchpad rows (n MiB in total) stay in the 126 MB L2, so the dependent phase-2 read is an L2
-// hit.  Slot s is handled by lane s / W of warp s % W (W = warps launched); V is private scratch, label-major here:
+// lane, labels are spread over as many WARPS as there are scheduler slots (SMs x 4) so that every label's warp issues
+// every cycle, and for a proof's K2 = 37 labels the scratchpad rows (n MiB in total) stay in the 50 MB L2, so the
+// dependent phase-2 read is an L2 hit.  Slot s is handled by lane s / W of warp s % W (W = warps launched); V is private scratch, label-major here:
 // row j of slot s at V + (s * N + j) * 8 uint4 (n x 128*N bytes in total, whatever W is).
 // =================================================================================================
 __device__ __forceinline__ uint4 ld_l2(const uint4 *p) {

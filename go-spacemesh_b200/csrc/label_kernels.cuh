@@ -1,4 +1,4 @@
-// label_kernels.cuh — sm_100a kernels of the POST label path and their launch table.
+// label_kernels.cuh — sm_90a kernels of the POST label path and their launch table.
 //
 // One label = one thread ("slot").  A *wave* is the set of slots resident on the GPU at once; every
 // slot owns a private 128*N-byte ROMix scratchpad in HBM for the lifetime of the wave.

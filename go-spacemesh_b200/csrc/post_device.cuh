@@ -1,4 +1,4 @@
-// post_device.cuh — per-thread arithmetic of the POST label function for sm_100a.
+// post_device.cuh — per-thread arithmetic of the POST label function for sm_90a.
 //
 // label32(i) = scrypt_jane(P = commitment[32] || LE64(i) || 0^32, S = "", N, r = 1, p = 1, dkLen = 32)
 // where scrypt_jane is scrypt's structure (PBKDF2 -> ROMix -> PBKDF2, RFC 7914 §6) with ChaCha20/8 as the

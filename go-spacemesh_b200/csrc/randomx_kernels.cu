@@ -1,4 +1,4 @@
-// randomx_kernels.cu — RandomX (k2pow) on sm_100a.  go-spacemesh reaches this function only through an RPC to the
+// randomx_kernels.cu — RandomX (k2pow) on sm_90a.  go-spacemesh reaches this function only through an RPC to the
 // external post-service (activation/nipost.go:171) and through libpost's verifier (activation/post_verifier.go:159);
 // the arithmetic is tevador/RandomX v1.1.x (doc/specs.md), restated here for the GPU:
 //
@@ -16,8 +16,8 @@
 //   chain seed   Blake2b-512 of the register file;  finalize: AesHash1R over the scratchpad + Blake2b-256.
 //
 // Throughput is bounded by dependent scratchpad accesses (one 8-byte access per ~5 instructions, each a random HBM
-// sector) and by SIMT divergence across VMs — RandomX is built to be that — so the lever a B200 offers is capacity:
-// tens of thousands of 2 MiB scratchpads resident in 180 GB of HBM and the full 2080 MiB dataset next to them.
+// sector) and by SIMT divergence across VMs — RandomX is built to be that — so the lever the GPU offers is capacity:
+// thousands of 2 MiB scratchpads resident in 80 GB of HBM and the full 2080 MiB dataset next to them.
 #include "randomx_kernels.cuh"
 
 #include <cstring>
@@ -409,11 +409,10 @@ __device__ __forceinline__ double u2d(u64 v) { return __longlong_as_double((long
 
 // ---------------------------------------------------------------------------------------------- the VM: one WARP per VM
 // All 32 lanes run the same VM, so the interpreter never diverges: a step costs its own latency, not the worst latency
-// among 32 unrelated programs, and a hash takes ~1 s instead of ~9 s (the verifier's pow check needs that) in 1/8 of
-// the memory.  Measured alternatives (profiles/r02_k2pow_variants.md): one THREAD per VM (register files in shared
-// memory, switch diverging over 32 programs) 4.2 kH/s at 256 VMs/SM = 74 GB of scratchpads and 9 s per batch, flat
-// beyond that; a first warp-per-VM kernel with the register file spread over the lanes (operands by shuffle) issued
-// 59 SASS instructions per VM instruction and stopped at 3.3 kH/s.  This kernel: the register file lives in shared
+// among 32 unrelated programs, so a hash finishes soon enough for the verifier's pow check, in 1/8 of the memory.
+// Rejected alternatives: one THREAD per VM (register files in shared memory, switch diverging over 32 programs, 8x the
+// scratchpads per SM and a batch as slow as its slowest program); a first warp-per-VM kernel with the register file
+// spread over the lanes (operands by shuffle, over twice the SASS instructions per VM instruction).  This kernel: the register file lives in shared
 // memory (one LDS.64 per operand instead of two shuffles and a convergence check), slot fields of the instruction
 // word are byte offsets, opcodes are dense with one opcode per (operation, operand kind) so a handler touches only
 // what it needs, and every lane executes the whole instruction redundantly (both halves of an FP register too): no
@@ -421,7 +420,6 @@ __device__ __forceinline__ double u2d(u64 v) { return __longlong_as_double((long
 // scratchpad / dataset lines around it.  The dispatch is a jump table indexed by opcode | rounding mode, both operands
 // are requested before the branch and lane 0 interprets alone; 25 SASS instructions per VM instruction and 23 KB of code — the 32 KB instruction
 // cache is a hard budget for an interpreter: a 58 KB build with 30 % fewer instructions per step was slower.
-// 6.6 kH/s (profiles/r02_rx_execute_v3_ncu.md, r02_k2pow_variants.md).
 __device__ __forceinline__ uint8_t *sp_byte(uint8_t *cold, uint8_t *hot, u32 addr) { return (addr < kScratchpadL1 ? hot : cold) + addr; }
 
 // Per-warp shared state of the VM kernel.  The interpreter addresses it with explicit 32-bit shared-window addresses

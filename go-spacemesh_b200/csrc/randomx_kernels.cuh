@@ -1,4 +1,4 @@
-// randomx_kernels.cuh — launch interface of the sm_100a RandomX kernels (k2pow).  See randomx_kernels.cu.
+// randomx_kernels.cuh — launch interface of the sm_90a RandomX kernels (k2pow).  See randomx_kernels.cu.
 #pragma once
 #include <cuda_runtime.h>
 

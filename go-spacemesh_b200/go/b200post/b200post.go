@@ -71,7 +71,7 @@ func statusErr(rc C.int, msg string) error {
 	}
 }
 
-// Providers lists the B200s — drop-in for initialization.OpenCLProviders().
+// Providers lists the GPUs — drop-in for initialization.OpenCLProviders().
 func Providers() ([]Provider, error) {
 	n := int(C.b200post_providers(nil, 0))
 	if n == 0 {

@@ -57,7 +57,7 @@ type SetupOpts struct { // PostSetupOpts (activation/post.go:53-61)
 	DataDir          string
 	NumUnits         uint32
 	MaxFileSize      uint64
-	ProviderID       *uint32 // nil = not specified; use AllProviders for every B200 of the box
+	ProviderID       *uint32 // nil = not specified; use AllProviders for every GPU of the box
 	ScryptN          uint64
 	ComputeBatchSize uint64
 }
@@ -209,7 +209,7 @@ func NewVerifierWith(provider uint32, o VerifierOptions) (*Verifier, error) {
 	return v, nil
 }
 
-// NewVerifierOn builds one verifier over several B200s: a worker per device drains the same queue.
+// NewVerifierOn builds one verifier over several GPUs: a worker per device drains the same queue.
 func NewVerifierOn(providers []uint32) (*Verifier, error) {
 	if len(providers) == 0 {
 		return nil, errors.New("b200post: no providers")

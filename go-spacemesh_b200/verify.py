@@ -251,7 +251,7 @@ class PreparedBatch:
         return list(self.st[:self.n]), list(self.bad[:self.n])
 
     def run_multi(self, providers: list[int], pow="builtin"):
-        """The batch split over several B200s (contiguous runs of proofs, one host thread per device)."""
+        """The batch split over several GPUs (contiguous runs of proofs, one host thread per device)."""
         ids = (ctypes.c_uint32 * len(providers))(*providers)
         opts, _cb = _verifier_opts(pow)
         rc = _bind().b200post_verify_batch_multi(ids, len(providers), self.n, self.cps, self.cms, ctypes.byref(self.cq),

@@ -1,5 +1,5 @@
 /*
- * b200post.h — C ABI of the B200-native POST label engine (libb200post.so).
+ * b200post.h — C ABI of the GPU-native POST label engine (libb200post.so).
  *
  * This is the drop-in boundary for go-spacemesh's POST hot path.  Every entry point is blocking,
  * thread-safe, takes plain pointers and sizes, never hands ownership of memory across the boundary and
@@ -12,7 +12,7 @@
  *                                   (PostSetupProvider{ID, Model, DeviceType}, activation/post.go:24)
  *   b200post_labels_range        -> (*initialization.Initializer).Initialize activation/post.go:295
  *                                   = libpost `initialize(init, start, end, out, &nonce)` per ComputeBatchSize batch
- *   b200post_labels_range_multi  -> same, index range sharded over several B200s (SURVEY.md §8e)
+ *   b200post_labels_range_multi  -> same, index range sharded over several GPUs (SURVEY.md §8e)
  *   b200post_labels_gather       -> the label recomputation inside verifying.ProofVerifier.Verify
  *                                   activation/post_verifier.go:159 (K2 / K3 / one selected index per proof)
  *   b200post_verify_vrf_nonce    -> verifying.VerifyVRFNonce                 activation/validation.go:261-282
@@ -53,7 +53,7 @@ enum {
 typedef struct b200post_provider {
     uint32_t id;            /* CUDA device ordinal                                  */
     uint32_t device_class;  /* B200POST_DEVICE_CLASS_GPU                            */
-    char model[64];         /* e.g. "NVIDIA B200"                                   */
+    char model[64];         /* e.g. "NVIDIA H100 80GB HBM3"                        */
     uint64_t hbm_bytes;     /* total device memory                                  */
     uint32_t sm_count;
     uint32_t cc_major, cc_minor;

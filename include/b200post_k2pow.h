@@ -1,5 +1,5 @@
 /*
- * b200post_k2pow.h — k2pow (RandomX proof of work) on the B200 (part of libb200post.so).
+ * b200post_k2pow.h — k2pow (RandomX proof of work) on the GPU (part of libb200post.so).
  *
  * What it replaces in the reference (paths relative to spacemeshos/go-spacemesh):
  *   b200post_k2pow_search   -> the k2pow nonce search the external post-service runs before the proving scan, asked for
@@ -17,7 +17,7 @@
  * no k2pow fixture exists in the reference tree).
  *
  * "Fast mode" only: the 2080 MiB dataset is built on the device (once per key and device, ~1 s) and stays in HBM; the
- * reference's light/fast distinction (RandomXMode) is a CPU memory trade-off that a 180 GB device does not need.
+ * reference's light/fast distinction (RandomXMode) is a CPU memory trade-off that an 80 GB device does not need.
  * No CPU fallback: without a CUDA device every call returns B200POST_ERR_NO_DEVICE.
  */
 #ifndef B200POST_K2POW_H
@@ -85,8 +85,8 @@ int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uin
  * and of its VM kernel alone (the dominant kernel).  Any pointer may be NULL. */
 int b200post_randomx_last_timing(uint32_t provider, double *total_ms, double *vm_kernel_ms, uint64_t *hashes, uint64_t *vm_launches);
 
-/* VMs (hashes) one device batch holds under the current options ("rx_vm_mode", default 1 = 48 VMs per SM: 7 104 on a
- * 148-SM B200; "rx_vms_per_sm" overrides the count; shrunk to what fits in free HBM at 2 MiB + 16 KiB per VM). */
+/* VMs (hashes) one device batch holds under the current options ("rx_vm_mode", default 1 = 48 VMs per SM: 6 336 on a
+ * 132-SM H100; "rx_vms_per_sm" overrides the count; shrunk to what fits in free HBM at 2 MiB + 16 KiB per VM). */
 int b200post_randomx_batch_size(uint32_t provider, uint64_t *vms);
 
 #ifdef __cplusplus

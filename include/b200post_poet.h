@@ -1,5 +1,5 @@
 /*
- * b200post_poet.h — PoET registration proof-of-work nonce search on the B200 (SURVEY.md §8f.4).
+ * b200post_poet.h — PoET registration proof-of-work nonce search on the GPU (SURVEY.md §8f.4).
  *
  * Stands in for `shared.FindSubmitPowNonce(ctx, powChallenge, poetChallenge, nodeID, difficulty)` of the
  * un-vendored github.com/spacemeshos/poet v0.10.4 (go.mod:47), called at activation/poet.go:529-535 when a PoET

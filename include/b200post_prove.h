@@ -1,5 +1,5 @@
 /*
- * b200post_prove.h — POST proof generation scan on the B200 (part of libb200post.so).  SURVEY.md §8f.3.
+ * b200post_prove.h — POST proof generation scan on the GPU (part of libb200post.so).  SURVEY.md §8f.3.
  *
  * What it stands in for: the AES scan half of `PostClient.Proof` (activation/interface.go:204-207), which in
  * the reference is one blocking RPC (activation/nipost.go:171, api/grpcserver/post_client.go:69-143) into the

@@ -1,5 +1,5 @@
 /*
- * b200post_setup.h — POST data initialisation sessions on the B200 label engine (part of libb200post.so).
+ * b200post_setup.h — POST data initialisation sessions on the GPU label engine (part of libb200post.so).
  *
  * Host-side mirror, behind a C ABI, of what go-spacemesh drives for POST setup:
  *   activation.PostSetupManager   PrepareInitializer / StartSession / Status / Reset   activation/post.go:245-449
@@ -48,7 +48,7 @@ enum {                                       /* PostSetupState, activation/post.
 };
 
 #define B200POST_PROVIDER_UNSET (-1)         /* PostSetupOpts.ProviderID == nil                                */
-#define B200POST_PROVIDER_ALL (-2)           /* extension: shard every batch over all B200s of the box         */
+#define B200POST_PROVIDER_ALL (-2)           /* extension: shard every batch over all GPUs of the box         */
 
 typedef struct b200post_post_config {        /* PostConfig, activation/post.go:27-38 */
     uint32_t min_num_units, max_num_units;

@@ -1,5 +1,5 @@
 /*
- * b200post_verify.h — batched POST proof verification on the B200 label engine (part of libb200post.so).
+ * b200post_verify.h — batched POST proof verification on the GPU label engine (part of libb200post.so).
  *
  * Replaces, for the label-recomputation-heavy part, what go-spacemesh reaches through
  *   activation.PostVerifier            activation/interface.go:26-29

@@ -4,7 +4,7 @@
  * stand in for `-lpost` on that path (link mechanics: Makefile-libs.Inc:5-6,59-69 in the reference;
  * call sites: activation/post.go:295,355-361, activation/post_supervisor.go:106,121).
  *
- * `post.h` is NOT present under /root/reference (it is fetched at build time, Makefile-libs.Inc:78-94),
+ * `post.h` is NOT present in the go-spacemesh tree (it is fetched at build time, Makefile-libs.Inc:78-94),
  * so these declarations are a restatement of the published header and are marked "unpinned" in
  * DESIGN.md: a maintainer must diff them against the real post.h before linking.
  *

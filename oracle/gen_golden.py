@@ -12,7 +12,7 @@ Inputs mirror the reference's own deterministic test inputs where it has any:
     LabelsPerUnit = 128 (:48), default scrypt N = 8192;
   * activation/post_test.go:354-357 — Scrypt.N = 2, 1024 labels (BASELINE.json configs[0]).
 
-Run in the build container:  python oracle/gen_golden.py        (~2 min; reads /root/reference for the fixture)
+Run:  GO_SPACEMESH_DIR=<go-spacemesh checkout> python oracle/gen_golden.py        (~2 min; the fixture is read from there)
 """
 import hashlib
 import json
@@ -67,7 +67,7 @@ def main():
 
     # ---- real identities from the reference's checkpoint fixture: the pin of the label function
     import base64
-    ref = "/root/reference/checkpoint/checkpointdata.json"
+    ref = os.path.join(os.environ.get("GO_SPACEMESH_DIR", ""), "checkpoint", "checkpointdata.json")
     if os.path.exists(ref):
         seen = {}
         for a in json.load(open(ref))["data"]["atxs"]:

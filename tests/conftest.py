@@ -13,7 +13,7 @@ GOLDEN = ROOT / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with `pytest -m gpu` under gpurun)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with `pytest -m gpu`)")
 
 
 @pytest.fixture(scope="session")

@@ -16,7 +16,7 @@ def k2(b2, gpu_ready):
 
 
 def test_randomx_known_answers_on_gpu(k2):
-    """RandomX src/tests/tests.cpp vectors, computed by the sm_100a kernels (dataset, AES generators, VM, Blake2b)."""
+    """RandomX src/tests/tests.cpp vectors, computed by the sm_90a kernels (dataset, AES generators, VM, Blake2b)."""
     assert k2.randomx_hash(b"test key 000", [b"This is a test"])[0].hex() == \
         "639183aae1bf4c9a35884cb46b09cad9175f04efd7684e7262a0ac1c2f0b4e3f"
     assert k2.randomx_hash(b"test key 000", [b"Lorem ipsum dolor sit amet"])[0].hex() == \

@@ -1,6 +1,6 @@
 """The C library's own NCCL exchange (b200post_vrf_comm_*): two PROCESSES, one GPU each, each initialises its shard and
 the ranks min-reduce the VRF candidate — BASELINE.json configs[3]'s shape at world 2, with no torch in the loop.
-Needs two GPUs (skipped otherwise; the driver's single-GPU test box skips it, tools/ + profiles/ hold a 2-GPU run)."""
+Needs two GPUs (skipped on a single-GPU machine)."""
 import ctypes
 import multiprocessing as mp
 import sys

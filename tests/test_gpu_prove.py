@@ -1,5 +1,5 @@
 """GPU tier: init -> prove -> verify, the reference's e2e shape (activation/e2e/nipost_test.go:151-231: setup
-session, PostClient.Proof, real verifier) run entirely on the B200 engine, plus parity of the proving scan with
+session, PostClient.Proof, real verifier) run entirely on the GPU engine, plus parity of the proving scan with
 the oracle's restatement."""
 import importlib
 

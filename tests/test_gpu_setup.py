@@ -180,7 +180,7 @@ def test_all_providers_extension(su, orc, tmp_path):
 
 
 def test_postcli_compatible_cli(b2, orc, tmp_path):
-    """systest/cluster/nodes.go:990-999 flag set, with a B200 provider instead of the CPU one."""
+    """systest/cluster/nodes.go:990-999 flag set, with a GPU provider instead of the CPU one."""
     import subprocess
     cli = Path(b2.LIB_PATH).parent / "b200postcli"
     if not cli.exists():

@@ -3,7 +3,7 @@
 //   mode 3: the Salsa mix — add, rotate, xor per step (8 independent chains per thread)
 // Prints thread-instructions per clock per SM; the alu pipe (SHF, LOP3) tops out at 64, which is the ceiling
 // the ROMix kernel runs into (DESIGN.md §4).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/alubench tools/alubench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/alubench tools/alubench.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>

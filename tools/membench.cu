@@ -1,8 +1,8 @@
-// tools/membench.cu — dev probe: what HBM delivers for the two ROMix access patterns on this B200.
+// tools/membench.cu — dev probe: what HBM delivers for the two ROMix access patterns on this GPU.
 //   (a) random 128-byte row reads (one row per 8-lane group, 16 B per lane) over a large buffer,
 //       with `depth` independent rows in flight per group;
 //   (b) streaming 128-bit writes; (c) both at once (half the CTAs each).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/membench tools/membench.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/membench tools/membench.cu
 #include <cuda_runtime.h>
 #include <cstdint>
 #include <cstdio>

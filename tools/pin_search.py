@@ -1,7 +1,7 @@
 """Search for the label-function conventions that make the real VRF nonces of the reference's checkpoint fixture
 (checkpoint/checkpointdata.json: 42 identities of a LabelsPerUnit=1024 network) valid.  A VRF nonce is the index
 of a label whose 32-byte scrypt output is below 2^256/numLabels, so the right function shows >= 15 leading zero
-bits for every identity; a wrong one shows ~1.  Run in the build container only (reads /root/reference)."""
+bits for every identity; a wrong one shows ~1.  Reads the fixture from the go-spacemesh checkout at $GO_SPACEMESH_DIR."""
 import base64, hashlib, hmac, json, struct, sys
 import numpy as np
 import blake3
@@ -108,7 +108,8 @@ def lz(b):
 if __name__ == "__main__":
     np.seterr(over="ignore")
     assert scrypt_batch([b"pw"], [b"salt"], 16, salsa8, "sha256") == [hashlib.scrypt(b"pw", salt=b"salt", n=16, r=1, p=1, dklen=32)]
-    d = json.load(open("/root/reference/checkpoint/checkpointdata.json"))
+    import os
+    d = json.load(open(os.path.join(os.environ["GO_SPACEMESH_DIR"], "checkpoint", "checkpointdata.json")))
     ids = {}
     for a in d["data"]["atxs"]:
         ids[(a["publicKey"], a["commitmentAtx"], a["vrfNonce"], a["numUnits"])] = a
