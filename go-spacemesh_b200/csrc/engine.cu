@@ -60,7 +60,10 @@ void DeviceEngine::release() {
         cudaFreeHost(h_commit_[b]); h_commit_[b] = nullptr;
         cudaFreeHost(h_idx_[b]); h_idx_[b] = nullptr;
         cudaFree(d_cidx_[b]); d_cidx_[b] = nullptr; cudaFreeHost(h_cidx_[b]); h_cidx_[b] = nullptr;
-        cudaEvent_t *evs[] = {&ev_done_[b], &ev_in_[b], &ev_k3_[b], &ev_k2a_[b], &ev_k2b_[b], &ev_call_[b]};
+        cudaFree(d_exp_[b]); d_exp_[b] = nullptr; cudaFreeHost(h_exp_[b]); h_exp_[b] = nullptr;
+        cudaFree(d_bits_[b]); d_bits_[b] = nullptr;
+        cudaFree(d_cnt_[b]); d_cnt_[b] = nullptr; cudaFreeHost(h_cnt_[b]); h_cnt_[b] = nullptr;
+        cudaEvent_t *evs[] = {&ev_done_[b], &ev_in_[b], &ev_k3_[b], &ev_k2a_[b], &ev_k2b_[b], &ev_call_[b], &ev_exp_[b]};
         for (cudaEvent_t *e : evs) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
         k2_pending_[b] = false; in_pending_[b] = false; pend_[b].live = false;
     }
@@ -96,6 +99,9 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
             CU_TRY(cudaEventCreate(&ev_k2a_[b]));
             CU_TRY(cudaEventCreate(&ev_k2b_[b]));
             CU_TRY(cudaEventCreate(&ev_call_[b]));
+            CU_TRY(cudaEventCreateWithFlags(&ev_exp_[b], cudaEventDisableTiming));
+            CU_TRY(cudaMalloc(&d_cnt_[b], 4));
+            CU_TRY(cudaMallocHost(&h_cnt_[b], 4));
         }
         CU_TRY(cudaMalloc(&d_diff_, 32));
         CU_TRY(cudaMalloc(&d_range_commit_, 32));
@@ -158,7 +164,8 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
         for (int b = 0; b < 2; b++) {
             cudaFree(X_[b]); cudaFree(d_commit_[b]); cudaFree(d_idx_[b]); cudaFree(d_out_[b]); cudaFree(d_cidx_[b]);
             cudaFreeHost(h_commit_[b]); cudaFreeHost(h_idx_[b]); cudaFreeHost(h_out_[b]); cudaFreeHost(h_cidx_[b]);
-            d_cidx_[b] = nullptr; h_cidx_[b] = nullptr;
+            cudaFree(d_exp_[b]); cudaFreeHost(h_exp_[b]); cudaFree(d_bits_[b]);
+            d_cidx_[b] = nullptr; h_cidx_[b] = nullptr; d_exp_[b] = nullptr; h_exp_[b] = nullptr; d_bits_[b] = nullptr;
             X_[b] = nullptr; d_commit_[b] = nullptr; d_idx_[b] = nullptr; d_out_[b] = nullptr;
             h_commit_[b] = nullptr; h_idx_[b] = nullptr; h_out_[b] = nullptr;
         }
@@ -174,6 +181,9 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
             CU_TRY(cudaMallocHost(&h_out_[b], (size_t)need * 16));
             CU_TRY(cudaMalloc(&d_cidx_[b], (size_t)need * 4));
             CU_TRY(cudaMallocHost(&h_cidx_[b], (size_t)need * 4));
+            CU_TRY(cudaMalloc(&d_exp_[b], (size_t)need * 16));
+            CU_TRY(cudaMallocHost(&h_exp_[b], (size_t)need * 16));
+            CU_TRY(cudaMalloc(&d_bits_[b], (size_t)need / 32 * 4));
         }
         CU_TRY(cudaMalloc(&d_cta_cand_, (size_t)pbkdf2_final_ctas(need) * sizeof(VrfCandidate)));
         alloc_slots_ = need;
@@ -196,6 +206,15 @@ int DeviceEngine::retire(const Job &job, int b) {
     if (!pend_[b].live) return B200POST_OK;
     CU_TRY(cudaEventSynchronize(ev_done_[b]));
     if (job.out_host) memcpy(job.out_host + pend_[b].off * 16, h_out_[b], (size_t)pend_[b].n * 16);
+    if (job.cmp && *h_cnt_[b]) {
+        // rare path: the layer has mismatches; fetch its bitmap and decode positions (ascending: layers retire in order)
+        std::vector<uint32_t> bits(round_up(pend_[b].n, 32) / 32);
+        CU_TRY(cudaMemcpy(bits.data(), d_bits_[b], bits.size() * 4, cudaMemcpyDeviceToHost));
+        job.cmp->mismatches += *h_cnt_[b];
+        for (size_t w = 0; w < bits.size() && job.cmp->first.size() < CompareResult::kMaxReported; w++)
+            for (uint32_t v = bits[w]; v && job.cmp->first.size() < CompareResult::kMaxReported; v &= v - 1)
+                job.cmp->first.push_back(pend_[b].off + 32 * w + (uint64_t)__builtin_ctz(v));
+    }
     pend_[b].live = false;
     return B200POST_OK;
 }
@@ -211,6 +230,14 @@ int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_
         CU_TRY(cudaEventRecord(ev_in_[b], stream_));
         in_pending_[b] = true;
         *lj = LabelJob{reinterpret_cast<const uint32_t *>(d_ctab_), 0, d_idx_[b], 0, n_valid, d_cidx_[b]};
+    } else if (job.gather && !job.commitments) {
+        // one commitment for every item (compare jobs): only the indices travel
+        if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
+        memcpy(h_idx_[b], job.indices + off, (size_t)n_valid * 8);
+        CU_TRY(cudaMemcpyAsync(d_idx_[b], h_idx_[b], (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_));
+        CU_TRY(cudaEventRecord(ev_in_[b], stream_));
+        in_pending_[b] = true;
+        *lj = LabelJob{d_range_commit_, 0, d_idx_[b], 0, n_valid, nullptr};
     } else if (job.gather) {
         if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
         memcpy(h_commit_[b], job.commitments + off * 32, (size_t)n_valid * 32);
@@ -231,8 +258,20 @@ int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_
 int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj) {
     const uint64_t off = layer * (uint64_t)std::min<uint64_t>(wave_slots_, alloc_slots_);
     const uint32_t n_slots = round_up(n_valid, 32);
-    uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : d_out_[b];
-    CU_TRY(launch_pbkdf2_final(lj, X_[b], alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_, stream_));
+    if (job.expect_host) {
+        // K3c: the expected slice goes H2D on the copy stream (pinned staging, double-buffered by parity; retire(b) has
+        // seen the previous copy out of h_exp_[b] finish), and K3c waits for it by event
+        memcpy(h_exp_[b], job.expect_host + off * 16, (size_t)n_valid * 16);
+        CU_TRY(cudaMemcpyAsync(d_exp_[b], h_exp_[b], (size_t)n_valid * 16, cudaMemcpyHostToDevice, copy_stream_));
+        CU_TRY(cudaEventRecord(ev_exp_[b], copy_stream_));
+        CU_TRY(cudaStreamWaitEvent(stream_, ev_exp_[b], 0));
+        CU_TRY(cudaMemsetAsync(d_cnt_[b], 0, 4, stream_));
+        CU_TRY(launch_pbkdf2_final_compare(lj, X_[b], alloc_slots_, n_slots, d_exp_[b], d_bits_[b], d_cnt_[b], job.d_diff,
+                                           d_cta_cand_, stream_));
+    } else {
+        uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : d_out_[b];
+        CU_TRY(launch_pbkdf2_final(lj, X_[b], alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_, stream_));
+    }
     g_launches += 1;
     if (job.d_diff) {
         CU_TRY(launch_vrf_merge(d_cta_cand_, pbkdf2_final_ctas(n_slots), d_running_, stream_));
@@ -243,6 +282,12 @@ int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n
         CU_TRY(cudaEventRecord(ev_k3_[b], stream_));
         CU_TRY(cudaStreamWaitEvent(copy_stream_, ev_k3_[b], 0));
         CU_TRY(cudaMemcpyAsync(h_out_[b], d_out_[b], (size_t)n_valid * 16, cudaMemcpyDeviceToHost, copy_stream_));
+        CU_TRY(cudaEventRecord(ev_done_[b], copy_stream_));
+    } else if (job.expect_host) {
+        // only the 4-byte count comes back per layer; the bitmap follows in retire() when it is non-zero
+        CU_TRY(cudaEventRecord(ev_k3_[b], stream_));
+        CU_TRY(cudaStreamWaitEvent(copy_stream_, ev_k3_[b], 0));
+        CU_TRY(cudaMemcpyAsync(h_cnt_[b], d_cnt_[b], 4, cudaMemcpyDeviceToHost, copy_stream_));
         CU_TRY(cudaEventRecord(ev_done_[b], copy_stream_));
     } else {
         CU_TRY(cudaEventRecord(ev_done_[b], stream_));
@@ -387,9 +432,23 @@ int DeviceEngine::run_job(const Job &job) {
 
 int DeviceEngine::labels_range(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host,
                                uint8_t *out_dev, const uint8_t *vrf_difficulty, VrfResult *vrf, const volatile int *cancel) {
+    return range_call(commitment, N, start, count, out_host, out_dev, nullptr, nullptr, vrf_difficulty, vrf, cancel);
+}
+
+int DeviceEngine::labels_compare_range(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count,
+                                       const uint8_t *expect_host, const uint8_t *vrf_difficulty, VrfResult *vrf,
+                                       CompareResult *cmp, const volatile int *cancel) {
+    if (!expect_host || !cmp) { set_error("compare job without expected labels or result"); return B200POST_ERR_INVALID_ARGUMENT; }
+    return range_call(commitment, N, start, count, nullptr, nullptr, expect_host, cmp, vrf_difficulty, vrf, cancel);
+}
+
+int DeviceEngine::range_call(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host,
+                             uint8_t *out_dev, const uint8_t *expect_host, CompareResult *cmp, const uint8_t *vrf_difficulty,
+                             VrfResult *vrf, const volatile int *cancel) {
     std::lock_guard<std::mutex> lk(mu_);
     CU_TRY(cudaSetDevice(dev_));
     if (vrf) *vrf = VrfResult{};
+    if (cmp) *cmp = CompareResult{};
     if (count == 0) return B200POST_OK;
     int rc = ensure(N, count);
     if (rc) return rc;
@@ -400,6 +459,7 @@ int DeviceEngine::labels_range(const uint8_t commitment[32], uint64_t N, uint64_
     CU_TRY(cudaMemcpyAsync(d_range_commit_, commitment, 32, cudaMemcpyHostToDevice, stream_));
     Job job;
     job.start = start; job.total = count; job.N = N; job.out_host = out_host; job.out_dev = out_dev; job.cancel = cancel;
+    job.expect_host = expect_host; job.cmp = cmp;
     if (vrf_difficulty) {
         uint32_t be[8];
         for (int k = 0; k < 8; k++)
@@ -429,7 +489,7 @@ int DeviceEngine::labels_range(const uint8_t commitment[32], uint64_t N, uint64_
     CU_TRY(cudaStreamSynchronize(stream_));
     { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
     metrics().range_calls_total++; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
-    if (status == B200POST_OK) metrics().labels_range_total += count;
+    if (status == B200POST_OK && !expect_host) metrics().labels_range_total += count;
     if (status == B200POST_ERR_CANCELLED) set_error("cancelled");
     return status;
 }
@@ -490,6 +550,35 @@ int DeviceEngine::labels_gather_indexed(size_t n_items, size_t n_commit, const u
     CU_TRY(cudaStreamSynchronize(stream_));
     { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
     metrics().gather_calls_total++; metrics().labels_gather_total += n_items; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
+    return B200POST_OK;
+}
+
+int DeviceEngine::labels_compare_indexed(const uint8_t commitment[32], size_t n_items, const uint64_t *indices, uint64_t N,
+                                         const uint8_t *expect_host, CompareResult *cmp, const volatile int *cancel) {
+    std::lock_guard<std::mutex> lk(mu_);
+    CU_TRY(cudaSetDevice(dev_));
+    if (!commitment || !indices || !expect_host || !cmp) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    *cmp = CompareResult{};
+    if (n_items == 0) return B200POST_OK;
+    int rc = ensure(N, n_items);
+    if (rc) return rc;
+    CU_TRY(cudaEventRecord(ev_call_[0], stream_));
+    spec_.valid = false;   // the scratch is about to be reused
+    memcpy(cur_commitment_, commitment, 32);
+    CU_TRY(cudaMemcpyAsync(d_range_commit_, commitment, 32, cudaMemcpyHostToDevice, stream_));
+    CU_TRY(cudaStreamSynchronize(stream_));   // `commitment` belongs to the caller
+    Job job;
+    job.gather = true; job.indices = indices; job.total = n_items; job.N = N;
+    job.expect_host = expect_host; job.cmp = cmp; job.cancel = cancel;
+    if ((rc = run_job(job))) {
+        quiesce();
+        if (rc == B200POST_ERR_CANCELLED) set_error("cancelled");
+        return rc;
+    }
+    CU_TRY(cudaEventRecord(ev_call_[1], stream_));
+    CU_TRY(cudaStreamSynchronize(stream_));
+    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
+    metrics().gather_calls_total++; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
     return B200POST_OK;
 }
 

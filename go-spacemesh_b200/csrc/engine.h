@@ -10,6 +10,7 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <vector>
 
 #include "label_kernels.cuh"
 
@@ -35,6 +36,13 @@ Options &options();
 extern std::atomic<uint64_t> g_launches;
 
 struct VrfResult { bool found = false; uint64_t index = 0; uint8_t label32[32] = {0}; };
+// outcome of a compare job: how many recomputed labels differ from the expected bytes, and the lowest
+// kMaxReported of their positions in job order (ascending), whatever the layer shape
+struct CompareResult {
+    static constexpr size_t kMaxReported = 64;
+    uint64_t mismatches = 0;
+    std::vector<uint64_t> first;
+};
 
 void set_error(const std::string &msg);
 const char *last_error();
@@ -55,6 +63,13 @@ public:
     // path recomputes ~37 labels per identity, so the commitment H2D shrinks by that factor
     int labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
                               const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev);
+    // compare jobs (K3c): recompute labels and compare them with expect_host (16 bytes per item, in job order) instead of
+    // returning them.  Range form: labels [start, start + count), VRF scan as in labels_range.  Indexed form: the labels
+    // at `indices` under one commitment.  *cmp is reset by the call; on CANCELLED it holds what was compared so far.
+    int labels_compare_range(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, const uint8_t *expect_host,
+                             const uint8_t *vrf_difficulty, VrfResult *vrf, CompareResult *cmp, const volatile int *cancel);
+    int labels_compare_indexed(const uint8_t commitment[32], size_t n_items, const uint64_t *indices, uint64_t N,
+                               const uint8_t *expect_host, CompareResult *cmp, const volatile int *cancel);
     // accumulated ROMix kernel device time, launches, and label-equivalents processed by those launches
     void romix_time(double *ms_total, uint64_t *launches, double *labels, bool reset);
     // device time (CUDA events on the engine's stream) of the last labels_range / labels_gather call
@@ -73,6 +88,9 @@ private:
         const uint8_t *commitments = nullptr;   // gather: n x 32 (host)
         const uint64_t *indices = nullptr;      // gather: n (host)
         const uint32_t *commit_index = nullptr; // indexed gather: per-item row of the call-level commitment table
+                                                // (gather with neither: every item uses the call's one commitment)
+        const uint8_t *expect_host = nullptr;   // compare job: expected labels, 16 bytes per item in job order
+        CompareResult *cmp = nullptr;
         uint64_t start = 0, total = 0, N = 0;
         uint8_t *out_host = nullptr, *out_dev = nullptr;
         const uint32_t *d_diff = nullptr;
@@ -81,6 +99,9 @@ private:
     int ensure(uint64_t N, uint64_t want_slots);   // (re)allocates scratch; sets wave_slots_
     void release();
     int run_job(const Job &job);
+    int range_call(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host, uint8_t *out_dev,
+                   const uint8_t *expect_host, CompareResult *cmp, const uint8_t *vrf_difficulty, VrfResult *vrf,
+                   const volatile int *cancel);
     // b = buffer parity of the layer (layer index + parity offset of the call)
     int stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj);          // inputs + K1
     int finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj);   // K3 (+K4) + D2H + event
@@ -110,6 +131,10 @@ private:
     uint32_t *d_cidx_[2] = {nullptr, nullptr}, *h_cidx_[2] = {nullptr, nullptr};   // indexed gather: per-item commitment rows
     uint8_t *d_ctab_ = nullptr; size_t ctab_rows_ = 0;   // indexed gather: call-level commitment table
     uint32_t *d_diff_ = nullptr;
+    // compare jobs: expected labels (pinned staging -> device, on copy_stream_), K3c's mismatch bitmap and count
+    uint8_t *h_exp_[2] = {nullptr, nullptr}, *d_exp_[2] = {nullptr, nullptr};
+    uint32_t *d_bits_[2] = {nullptr, nullptr}, *d_cnt_[2] = {nullptr, nullptr}, *h_cnt_[2] = {nullptr, nullptr};
+    cudaEvent_t ev_exp_[2] = {nullptr, nullptr};   // the expected slice of the layer is on the device
     VrfCandidate *d_cta_cand_ = nullptr;
     VrfCandidate *d_running_ = nullptr;
     VrfCandidate *h_running_ = nullptr;            // pinned

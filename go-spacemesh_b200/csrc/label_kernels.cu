@@ -402,6 +402,62 @@ __device__ __forceinline__ bool cand_less(const uint32_t (&a)[8], uint64_t ai, c
     return ai < bi;
 }
 
+// warp arg-min of (best, best_i) over the lanes with has != 0, by shuffles; every lane ends with the warp's winner
+__device__ __forceinline__ void warp_argmin(uint32_t (&best)[8], uint64_t &best_i, uint32_t &has) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) {
+        uint32_t o[8];
+#pragma unroll
+        for (int k = 0; k < 8; k++) o[k] = __shfl_xor_sync(0xffffffffu, best[k], off);
+        const uint64_t oi = __shfl_xor_sync(0xffffffffu, best_i, off);
+        const uint32_t oh = __shfl_xor_sync(0xffffffffu, has, off);
+        const bool take = oh && (!has || cand_less(o, oi, best, best_i));
+        if (take) {
+#pragma unroll
+            for (int k = 0; k < 8; k++) best[k] = o[k];
+            best_i = oi; has = 1;
+        }
+    }
+}
+
+// VRF nonce candidate of one CTA: min over valid slots with label32 < difficulty (strict), lowest index on ties.
+// Block-wide: every thread of the CTA calls it.
+__device__ __forceinline__ void cta_vrf_candidate(bool valid, const uint32_t (&lab)[8], uint64_t index,
+                                                  const uint32_t *__restrict__ vrf_be, VrfCandidate *warp_best,
+                                                  VrfCandidate *__restrict__ cta_cand) {
+    uint32_t diff[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) diff[k] = vrf_be[k];
+    // cand_less with equal labels compares indices 0 < 0 = false => strict '<' on the label
+    const bool cand = valid && cand_less(lab, 0, diff, 0);
+    if (!__syncthreads_or(cand)) {
+        if (threadIdx.x == 0) cta_cand[blockIdx.x].found = 0;
+        return;
+    }
+    // rare path: warp argmin by shuffles, then thread 0 merges the per-warp winners
+    uint32_t best[8];
+    uint64_t best_i = index;
+    uint32_t has = cand ? 1u : 0u;
+#pragma unroll
+    for (int k = 0; k < 8; k++) best[k] = lab[k];
+    warp_argmin(best, best_i, has);
+    if ((threadIdx.x & 31) == 0) {
+        VrfCandidate &w = warp_best[threadIdx.x >> 5];
+#pragma unroll
+        for (int k = 0; k < 8; k++) w.label_be[k] = best[k];
+        w.index = best_i; w.found = has; w.pad = 0;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        VrfCandidate r = warp_best[0];
+        for (int wv = 1; wv < FINAL_TPB / 32; wv++) {
+            const VrfCandidate c = warp_best[wv];
+            if (c.found && (!r.found || cand_less(c.label_be, c.index, r.label_be, r.index))) r = c;
+        }
+        cta_cand[blockIdx.x] = r;
+    }
+}
+
 __global__ void __launch_bounds__(FINAL_TPB) pbkdf2_final_kernel(LabelJob job, const uint4 *__restrict__ X, uint32_t x_stride,
                                                                  uint32_t n_slots, uint8_t *__restrict__ out16,
                                                                  const uint32_t *__restrict__ vrf_be,
@@ -437,53 +493,64 @@ __global__ void __launch_bounds__(FINAL_TPB) pbkdf2_final_kernel(LabelJob job, c
         bulk_wait_all<0>();
     }
     if (vrf_be == nullptr) return;
+    cta_vrf_candidate(valid, lab, index, vrf_be, warp_best, cta_cand);
+}
 
-    // ---- VRF nonce candidate: min over valid slots with label32 < difficulty (strict), lowest index on ties
-    uint32_t diff[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) diff[k] = vrf_be[k];
-    bool cand = valid && cand_less(lab, 0, diff, 0) ;
-    if (cand) {   // cand_less with equal labels compares indices 0 < 0 = false => strict '<' on the label
+// K3c: K3's label, compared with the expected 16 bytes instead of stored (checking stored POST data).  The CTA's
+// expected labels arrive by one TMA bulk load issued before the PBKDF2, so the load overlaps its Keccak-f work.
+// Each warp writes one ballot word of mismatching slots to mismatch_bits[slot / 32] (n_slots / 32 words, all
+// written) and adds its popcount to *mismatch_count only when it is non-zero.  VRF candidates as in K3.
+__global__ void __launch_bounds__(FINAL_TPB) pbkdf2_final_compare_kernel(LabelJob job, const uint4 *__restrict__ X, uint32_t x_stride,
+                                                                         uint32_t n_slots, const uint8_t *__restrict__ expect16,
+                                                                         uint32_t *__restrict__ mismatch_bits,
+                                                                         uint32_t *__restrict__ mismatch_count,
+                                                                         const uint32_t *__restrict__ vrf_be,
+                                                                         VrfCandidate *__restrict__ cta_cand) {
+    __shared__ __align__(128) uint4 expect[FINAL_TPB];
+    __shared__ __align__(8) uint64_t bar_storage;
+    __shared__ VrfCandidate warp_best[FINAL_TPB / 32];
+    const uint32_t cta_first = blockIdx.x * FINAL_TPB;
+    const uint32_t slot = cta_first + threadIdx.x;
+    const bool valid = slot < job.n_valid;
+    const bool any_valid = cta_first < job.n_valid;
+    const uint32_t bar = smem_u32(&bar_storage);
+    if (threadIdx.x == 0 && any_valid) {
+        mbar_init(bar, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        const uint32_t n_here = min((uint32_t)FINAL_TPB, job.n_valid - cta_first);
+        mbar_expect_tx(bar, n_here * 16);
+        bulk_g2s(smem_u32(expect), expect16 + (size_t)cta_first * 16, n_here * 16, bar);
     }
-    if (!__syncthreads_or(cand)) {
-        if (threadIdx.x == 0) cta_cand[blockIdx.x].found = 0;
-        return;
+    uint32_t lab[8];
+    uint64_t index = 0;
+    if (slot < n_slots) {
+        uint32_t c[8];
+        load_commit(job, valid ? slot : 0, c);
+        uint32_t lo[16], hi[16];
+#pragma unroll
+        for (int k = 0; k < 8; k++) set_chunk(lo, hi, k, X[(size_t)k * x_stride + slot]);
+        index = slot_index(job, slot);
+        label_final(c, index, lo, hi, lab);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; k++) lab[k] = 0xffffffffu;
     }
-    // rare path: warp argmin by shuffles, then thread 0 merges the per-warp winners
-    uint32_t best[8];
-    uint64_t best_i = index;
-    uint32_t has = cand ? 1u : 0u;
-#pragma unroll
-    for (int k = 0; k < 8; k++) best[k] = lab[k];
-#pragma unroll
-    for (int off = 16; off > 0; off >>= 1) {
-        uint32_t o[8];
-#pragma unroll
-        for (int k = 0; k < 8; k++) o[k] = __shfl_xor_sync(0xffffffffu, best[k], off);
-        const uint64_t oi = __shfl_xor_sync(0xffffffffu, best_i, off);
-        const uint32_t oh = __shfl_xor_sync(0xffffffffu, has, off);
-        const bool take = oh && (!has || cand_less(o, oi, best, best_i));
-        if (take) {
-#pragma unroll
-            for (int k = 0; k < 8; k++) best[k] = o[k];
-            best_i = oi; has = 1;
+    __syncthreads();   // the barrier is initialised before anyone waits on it
+    bool bad = false;
+    if (any_valid) {
+        mbar_wait(bar, 0);
+        if (valid) {
+            const uint4 e = expect[threadIdx.x];
+            bad = (e.x != bswap32(lab[0])) | (e.y != bswap32(lab[1])) | (e.z != bswap32(lab[2])) | (e.w != bswap32(lab[3]));
         }
     }
-    if ((threadIdx.x & 31) == 0) {
-        VrfCandidate &w = warp_best[threadIdx.x >> 5];
-#pragma unroll
-        for (int k = 0; k < 8; k++) w.label_be[k] = best[k];
-        w.index = best_i; w.found = has; w.pad = 0;
+    const uint32_t ballot = __ballot_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0 && slot < n_slots) {
+        mismatch_bits[slot >> 5] = ballot;
+        if (ballot) atomicAdd(mismatch_count, (uint32_t)__popc(ballot));
     }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        VrfCandidate r = warp_best[0];
-        for (int wv = 1; wv < FINAL_TPB / 32; wv++) {
-            const VrfCandidate c = warp_best[wv];
-            if (c.found && (!r.found || cand_less(c.label_be, c.index, r.label_be, r.index))) r = c;
-        }
-        cta_cand[blockIdx.x] = r;
-    }
+    if (vrf_be == nullptr) return;
+    cta_vrf_candidate(valid, lab, index, vrf_be, warp_best, cta_cand);
 }
 
 // K4: merge the per-CTA candidates of one wave into the running minimum (1 CTA, 256 threads)
@@ -525,6 +592,15 @@ cudaError_t launch_pbkdf2_expand(const LabelJob &job, uint4 *X, uint32_t x_strid
 }
 
 uint32_t pbkdf2_final_ctas(uint32_t n_slots) { return (n_slots + FINAL_TPB - 1) / FINAL_TPB; }
+
+cudaError_t launch_pbkdf2_final_compare(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots,
+                                        const uint8_t *expect16, uint32_t *mismatch_bits, uint32_t *mismatch_count,
+                                        const uint32_t *vrf_difficulty_be, VrfCandidate *cta_cand, cudaStream_t s) {
+    if (n_slots == 0) return cudaSuccess;
+    pbkdf2_final_compare_kernel<<<pbkdf2_final_ctas(n_slots), FINAL_TPB, 0, s>>>(job, X, x_stride, n_slots, expect16, mismatch_bits,
+                                                                                 mismatch_count, vrf_difficulty_be, cta_cand);
+    return cudaGetLastError();
+}
 
 cudaError_t launch_pbkdf2_final(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots, uint8_t *out16,
                                 const uint32_t *vrf_difficulty_be, VrfCandidate *cta_cand, cudaStream_t s) {

@@ -6,6 +6,7 @@
 //   K1 pbkdf2_expand_kernel    (commitment, index) -> X[32 words]: PBKDF2-HMAC-Keccak512, scrypt step 1
 //   K2 romix_kernel<VARIANT>   X <- ROMix(X) with the ChaCha20/8 BlockMix, the 99.5 % kernel (scrypt step 2)
 //   K3 pbkdf2_final_kernel     X -> label32 (PBKDF2 again); 16-byte labels out via TMA bulk store; VRF candidates
+//   K3c pbkdf2_final_compare_kernel   K3's label compared with expected stored bytes (TMA bulk load): mismatch bitmap + count
 //   K4 vrf_merge_kernel        per-CTA VRF candidates -> running minimum
 //
 // Reference anchors: activation/post.go:295 (Initialize -> labels over a contiguous range),
@@ -76,6 +77,11 @@ bool romix_mask_supported(int mw);
 cudaError_t launch_pbkdf2_final(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots,
                                 uint8_t *out16, const uint32_t *vrf_difficulty_be, VrfCandidate *cta_cand,
                                 cudaStream_t s);
+// K3c: expect16 = n_valid x 16 expected bytes (device).  mismatch_bits: n_slots / 32 words, all overwritten (bit = slot
+// whose label differs); *mismatch_count is incremented by the number of mismatching slots (the caller zeroes it).
+cudaError_t launch_pbkdf2_final_compare(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots,
+                                        const uint8_t *expect16, uint32_t *mismatch_bits, uint32_t *mismatch_count,
+                                        const uint32_t *vrf_difficulty_be, VrfCandidate *cta_cand, cudaStream_t s);
 cudaError_t launch_vrf_merge(const VrfCandidate *cta_cand, uint32_t n_cta, VrfCandidate *running, cudaStream_t s);
 uint32_t pbkdf2_final_ctas(uint32_t n_slots);
 // bytes of dynamic shared memory the ROMix variant needs per CTA

@@ -52,6 +52,8 @@ extern "C" size_t b200post_metrics_text(char *buf, size_t cap) {
     line("b200post_proofs_generated_total", "proofs generated", "counter", m.proofs_generated_total);
     line("b200post_setup_sessions_total", "setup sessions started", "counter", m.setup_sessions_total);
     line("b200post_setup_label_mismatch_total", "reference-label cross-check failures", "counter", m.setup_label_mismatch_total);
+    line("b200post_post_data_labels_verified_total", "stored POST labels recomputed and compared (verify_pos)", "counter", m.post_data_labels_verified_total);
+    line("b200post_post_data_label_mismatch_total", "stored POST labels that differed from their recomputation (verify_pos)", "counter", m.post_data_label_mismatch_total);
     if (buf && cap) {
         const size_t n = o.size() < cap - 1 ? o.size() : cap - 1;
         memcpy(buf, o.data(), n);

@@ -20,6 +20,7 @@ struct Metrics {
     std::atomic<uint64_t> verify_seconds_sum_us{0};
     std::atomic<uint64_t> prove_labels_scanned_total{0}, proofs_generated_total{0};
     std::atomic<uint64_t> setup_sessions_total{0}, setup_label_mismatch_total{0};
+    std::atomic<uint64_t> post_data_labels_verified_total{0}, post_data_label_mismatch_total{0};   // b200post_verify_pos
 };
 Metrics &metrics();
 void observe_verify_seconds(double s);

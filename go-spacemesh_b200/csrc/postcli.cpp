@@ -6,11 +6,17 @@
 // This tool accepts the same flags (single-dash, Go `flag` style; "-flag value" or "-flag=value") and drives a
 // PostSetupManager session (include/b200post_setup.h).  Differences: `-provider` takes a CUDA ordinal or
 // "all"; the CPU provider id 4294967295 is refused (the library has no CPU path).
+//
+// `-verify` checks data already on disk instead (postcli's flags as recalled, unpinned):
+//   b200postcli -verify -datadir /data [-fraction 0.2] [-fromFile 0] [-toFile N] [-seed S] [-provider 0|all]
+// recomputes `-fraction` percent of each file's labels on the GPU, prints `file N offset K (label I)` for each
+// reported mismatch and exits 0 when the data is valid, 1 otherwise.
 #include <signal.h>
 
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <thread>
@@ -30,10 +36,66 @@ static bool unhex32(const std::string &s, uint8_t out[32]) {
     return true;
 }
 
+static int run_verify(const std::string &datadir, const std::string &provider, double fraction, uint64_t from_file, int64_t to_file,
+                      uint64_t seed) {
+    b200post_verify_pos_opts o;
+    b200post_default_verify_pos_opts(&o);
+    o.provider_id = provider == "all" ? B200POST_PROVIDER_ALL : (int64_t)strtoull(provider.c_str(), nullptr, 10);
+    if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) { fprintf(stderr, "provider 4294967295 (CPU) is not served: this build has no CPU path\n"); return 2; }
+    o.fraction = fraction; o.from_file = from_file; o.to_file = to_file; o.seed = seed;
+    // what the progress line counts towards: the sample sizes of the checked files
+    uint64_t total = 0, per_file = 0;
+    b200post_post_metadata md;
+    if (b200post_load_metadata(datadir.c_str(), &md) == 0 && md.max_file_size >= 16) {
+        const uint64_t nl = (uint64_t)md.num_units * md.labels_per_unit;
+        per_file = md.max_file_size / 16;
+        const uint64_t n_files = (nl + per_file - 1) / per_file, last = to_file < 0 ? n_files - 1 : (uint64_t)to_file;
+        for (uint64_t f = from_file; f <= last && f < n_files; f++) {
+            uint64_t n = 0;
+            if (b200post_verify_pos_sample(1, f, std::min(per_file, nl - f * per_file), fraction, nullptr, 0, &n) == 0) total += n;
+        }
+    }
+    volatile uint64_t progress = 0;
+    o.progress = &progress;
+    signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
+    b200post_verify_pos_result r;
+    volatile int done = 0;
+    std::thread show([&] {
+        const auto t0 = std::chrono::steady_clock::now();
+        while (!done) {
+            for (int k = 0; k < 20 && !done; k++) std::this_thread::sleep_for(std::chrono::milliseconds(100));
+            const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+            const uint64_t p = progress;
+            fprintf(stderr, "\r%llu / %llu labels checked (%.1f %%), %.0f labels/s   ", (unsigned long long)p, (unsigned long long)total,
+                    total ? 100.0 * p / (double)total : 0.0, el > 0 ? p / el : 0.0);
+        }
+        fprintf(stderr, "\n");
+    });
+    const int rc = b200post_verify_pos(datadir.c_str(), &o, &r, &g_cancel);
+    done = 1;
+    show.join();
+    if (rc == B200POST_ERR_CANCELLED) { fprintf(stderr, "stopped\n"); return 130; }
+    if (rc != 0 && rc != B200POST_ERR_LABEL_MISMATCH && rc != B200POST_ERR_STATE) { fprintf(stderr, "verify failed: %s (%d)\n", b200post_last_error(), rc); return 1; }
+    printf("checked %llu labels in %llu files (seed %llu): %llu mismatches\n", (unsigned long long)r.labels_checked,
+           (unsigned long long)r.files_checked, (unsigned long long)r.seed, (unsigned long long)r.mismatches);
+    for (uint32_t i = 0; i < r.n_reported && per_file; i++)
+        printf("file %llu offset %llu (label %llu)\n", (unsigned long long)(r.bad_index[i] / per_file),
+               (unsigned long long)(r.bad_index[i] % per_file * 16), (unsigned long long)r.bad_index[i]);
+    if (rc == B200POST_ERR_STATE) printf("%s\n", b200post_last_error());
+    else if (!r.nonce_ok) printf("the VRF nonce's label does not match the metadata\n");
+    if (r.argmin_checked) printf("VRF nonce is the arg-min of the data: %s\n", r.argmin_ok ? "yes" : "no");
+    if (rc == 0) { printf("POST data is valid\n"); return 0; }
+    printf(rc == B200POST_ERR_STATE ? "POST data is not complete\n" : "POST data is INVALID\n");
+    return 1;
+}
+
 int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
-    bool print_providers = false;
+    bool print_providers = false, verify = false;
+    double fraction = 0.2;
+    uint64_t from_file = 0, seed = 0;
+    int64_t to_file = -1;
     for (int i = 1; i < argc; i++) {
         std::string a = argv[i], v;
         while (!a.empty() && a[0] == '-') a.erase(0, 1);
@@ -51,6 +113,11 @@ int main(int argc, char **argv) {
         else if (a == "provider") provider = val();
         else if (a == "printProviders") print_providers = true;
         else if (a == "yes") {}
+        else if (a == "verify") verify = true;
+        else if (a == "fraction") fraction = strtod(val().c_str(), nullptr);
+        else if (a == "fromFile") from_file = strtoull(val().c_str(), nullptr, 10);
+        else if (a == "toFile") to_file = strtoll(val().c_str(), nullptr, 10);
+        else if (a == "seed") seed = strtoull(val().c_str(), nullptr, 10);
         else { fprintf(stderr, "unknown flag -%s\n", a.c_str()); return 2; }
     }
     if (print_providers) {
@@ -59,6 +126,7 @@ int main(int argc, char **argv) {
         for (int k = 0; k < n && k < 16; k++) printf("{ID: %u, Model: \"%s\", DeviceType: GPU, HBM: %llu}\n", p[k].id, p[k].model, (unsigned long long)p[k].hbm_bytes);
         return 0;
     }
+    if (verify) return run_verify(datadir, provider, fraction, from_file, to_file, seed);
     uint8_t node_id[32], atx_id[32];
     if (!unhex32(id, node_id) || !unhex32(atx, atx_id)) { fprintf(stderr, "-id and -commitmentAtxId must be 32-byte hex strings\n"); return 2; }
     b200post_post_config cfg;

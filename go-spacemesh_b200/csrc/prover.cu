@@ -5,10 +5,6 @@
 // hit lists and stops when a nonce owns K2 of them.  Bandwidth view: 16 B in per label, ~nothing out; the
 // kernel is far faster than PCIe/NVMe can feed it, so the design goal is simply to keep copies and compute
 // overlapped.  Conventions: post-rs Prover8_56 from memory (ASSUMED, unpinned).
-#include <fcntl.h>
-#include <sys/stat.h>
-#include <unistd.h>
-
 #include <algorithm>
 #include <map>
 #include <mutex>
@@ -21,6 +17,7 @@
 #include "aes_device.cuh"
 #include "engine.h"
 #include "metrics.h"
+#include "postdata_io.h"
 #include "proof_common.h"
 
 namespace b200post {
@@ -274,31 +271,6 @@ int finish(const Scanner &sc, uint32_t nonces, const uint64_t *pows, uint64_t nu
 using namespace b200post;
 
 namespace {
-// pread of [off, off + bytes) into dst on up to 8 threads (pread is position-independent, so slices are independent)
-bool parallel_pread(int fd, uint8_t *dst, size_t bytes, off_t off) {
-    auto read_all = [fd](uint8_t *d, size_t n, off_t o) {
-        while (n) {
-            const ssize_t r = pread(fd, d, n, o);
-            if (r <= 0) return false;
-            d += r; n -= (size_t)r; o += r;
-        }
-        return true;
-    };
-    const size_t kMinSlice = (size_t)4 << 20;
-    const unsigned hw = std::max(1u, std::thread::hardware_concurrency());
-    const size_t nt = std::min<size_t>({(size_t)8, (size_t)hw, std::max<size_t>(1, bytes / kMinSlice)});
-    if (nt <= 1) return read_all(dst, bytes, off);
-    std::vector<std::thread> th;
-    std::vector<char> ok(nt, 0);
-    const size_t per = (bytes / nt + 15) & ~(size_t)15;
-    for (size_t t = 0; t < nt; t++) {
-        const size_t lo = std::min(bytes, t * per), hi = t + 1 == nt ? bytes : std::min(bytes, (t + 1) * per);
-        th.emplace_back([&, t, lo, hi] { ok[t] = read_all(dst + lo, hi - lo, off + (off_t)lo); });
-    }
-    for (auto &x : th) x.join();
-    for (char c : ok) if (!c) return false;
-    return true;
-}
 // the same for labels already in (pageable) host memory
 void parallel_copy(uint8_t *dst, const uint8_t *src, size_t bytes) {
     const size_t kMinSlice = (size_t)4 << 20;
@@ -380,33 +352,18 @@ int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], c
     const uint64_t per_file = md.max_file_size / 16;
     if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
     bool found = false;
-    int b = 0, fd = -1;
-    uint64_t open_file = ~0ull;
+    int b = 0;
+    PostDataReader reader(data_dir, per_file);
     for (uint64_t pos = 0; pos < num_labels && !found; b ^= 1) {
-        if (cancel && *cancel) { if (fd >= 0) close(fd); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
-        if ((rc = sc.collect(b, &found))) { if (fd >= 0) close(fd); return rc; }
+        if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
+        if ((rc = sc.collect(b, &found))) return rc;
         if (found) break;
         // fill the staging buffer from the files (a chunk may span files)
-        uint64_t n = 0;
-        const uint64_t want = std::min<uint64_t>(chunk, num_labels - pos);
-        while (n < want) {
-            const uint64_t file = (pos + n) / per_file, in_file = (pos + n) % per_file;
-            if (file != open_file) {
-                if (fd >= 0) close(fd);
-                const std::string path = std::string(data_dir) + "/postdata_" + std::to_string(file) + ".bin";
-                fd = open(path.c_str(), O_RDONLY);
-                if (fd < 0) { set_error("open " + path + ": " + strerror(errno)); return B200POST_ERR_IO; }
-                open_file = file;
-            }
-            const uint64_t take = std::min<uint64_t>(want - n, per_file - in_file);
-            // the read into the pinned staging buffer was the scan's bound (6.7-7.5 GB/s on one thread, r01): split it
-            if (!parallel_pread(fd, sc.staging(b) + n * 16, (size_t)take * 16, (off_t)(in_file * 16))) { close(fd); set_error("POST data is incomplete (short read): initialisation not finished?"); return B200POST_ERR_IO; }
-            n += take;
-        }
-        if ((rc = sc.submit(b, pos, (uint32_t)n))) { close(fd); return rc; }
+        const uint64_t n = std::min<uint64_t>(chunk, num_labels - pos);
+        if ((rc = reader.read(pos, n, sc.staging(b)))) return rc;
+        if ((rc = sc.submit(b, pos, (uint32_t)n))) return rc;
         pos += n;
     }
-    if (fd >= 0) close(fd);
     for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, &found))) return rc;   // older chunk first
     if ((rc = finish(sc, o.nonces, pows.data(), num_labels, out))) return rc;
     if (meta_out) {

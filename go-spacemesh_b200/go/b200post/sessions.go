@@ -17,6 +17,7 @@ import (
 	"context"
 	"errors"
 	"fmt"
+	"runtime"
 	"sync/atomic"
 	"unsafe"
 )
@@ -298,4 +299,70 @@ func GenerateProof(provider uint32, dataDir string, challenge []byte, cfg SetupC
 		return nil, err
 	}
 	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Checking stored POST data (postcli -verify; verifying.VerifyPos, recalled, unpinned)
+// ---------------------------------------------------------------------------------------------------------
+
+type VerifyPosOpts struct {
+	ProviderID uint32  // CUDA ordinal or AllProviders
+	Fraction   float64 // percent of each file's labels, (0, 100]; 100 = every label
+	FromFile   uint64
+	ToFile     int64   // inclusive; -1 = the last file
+	Seed       uint64  // 0 = drawn from the OS (returned in the result)
+	Progress   *uint64 // optional: labels checked so far (read it with atomic.LoadUint64)
+}
+
+type VerifyPosResult struct {
+	FilesChecked, LabelsChecked, Mismatches, Seed uint64
+	NonceOK, ArgminChecked, ArgminOK             bool
+	BadIndices                                   []uint64 // lowest mismatching global label indices, ascending (<= 64)
+}
+
+// VerifyPos recomputes a share of each file's labels on the GPU and compares them with the stored bytes.  Invalid data
+// returns the result together with ErrLabelMismatch; matching labels without a VRF nonce in the metadata return the
+// result and an error saying initialisation has not finished; a cancelled ctx returns the partial result and
+// context.Canceled.  Progress needs Go 1.21 (runtime.Pinner).
+func VerifyPos(ctx context.Context, dataDir string, o VerifyPosOpts) (*VerifyPosResult, error) {
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var co C.b200post_verify_pos_opts
+	C.b200post_default_verify_pos_opts(&co)
+	if o.ProviderID == AllProviders {
+		co.provider_id = C.B200POST_PROVIDER_ALL
+	} else {
+		co.provider_id = C.int64_t(o.ProviderID)
+	}
+	co.fraction, co.from_file, co.to_file, co.seed = C.double(o.Fraction), C.uint64_t(o.FromFile), C.int64_t(o.ToFile), C.uint64_t(o.Seed)
+	if o.Progress != nil {
+		// co is passed to C, so the Go pointer it holds must be pinned for the call (cgo pointer-passing rules)
+		var pin runtime.Pinner
+		pin.Pin(o.Progress)
+		defer pin.Unpin()
+		co.progress = (*C.uint64_t)(unsafe.Pointer(o.Progress))
+	}
+	var cancel int32
+	done := make(chan struct{})
+	defer close(done)
+	go func() {
+		select {
+		case <-ctx.Done():
+			atomic.StoreInt32(&cancel, 1)
+		case <-done:
+		}
+	}()
+	var out C.b200post_verify_pos_result
+	rc, msg := checked(func() C.int { return C.b200post_verify_pos(dir, &co, &out, (*C.int)(unsafe.Pointer(&cancel))) })
+	r := &VerifyPosResult{FilesChecked: uint64(out.files_checked), LabelsChecked: uint64(out.labels_checked),
+		Mismatches: uint64(out.mismatches), Seed: uint64(out.seed), NonceOK: out.nonce_ok != 0,
+		ArgminChecked: out.argmin_checked != 0, ArgminOK: out.argmin_ok != 0}
+	for i := 0; i < int(out.n_reported); i++ {
+		r.BadIndices = append(r.BadIndices, uint64(out.bad_index[i]))
+	}
+	switch rc {
+	case C.B200POST_OK, C.B200POST_ERR_LABEL_MISMATCH, C.B200POST_ERR_STATE, C.B200POST_ERR_CANCELLED:
+		return r, setupErr(rc, msg)
+	}
+	return nil, setupErr(rc, msg)
 }

@@ -38,6 +38,30 @@ class _Metadata(ctypes.Structure):
                 ("nonce", ctypes.c_uint64), ("nonce_value", ctypes.c_uint8 * 32), ("last_position", ctypes.c_uint64)]
 
 
+class _VerifyPosOpts(ctypes.Structure):
+    _fields_ = [("provider_id", ctypes.c_int64), ("fraction", ctypes.c_double), ("from_file", ctypes.c_uint64),
+                ("to_file", ctypes.c_int64), ("seed", ctypes.c_uint64), ("progress", ctypes.c_void_p)]
+
+
+class _VerifyPosResult(ctypes.Structure):
+    _fields_ = [("files_checked", ctypes.c_uint64), ("labels_checked", ctypes.c_uint64), ("mismatches", ctypes.c_uint64),
+                ("seed", ctypes.c_uint64), ("nonce_ok", ctypes.c_uint32), ("argmin_checked", ctypes.c_uint32),
+                ("argmin_ok", ctypes.c_uint32), ("n_reported", ctypes.c_uint32), ("bad_index", ctypes.c_uint64 * 64)]
+
+
+@dataclass
+class VerifyPosResult:       # b200post_verify_pos_result; `code` is the call's status (OK, ERR_LABEL_MISMATCH, ERR_CANCELLED)
+    code: int
+    files_checked: int
+    labels_checked: int
+    mismatches: int
+    seed: int
+    nonce_ok: bool
+    argmin_checked: bool
+    argmin_ok: bool
+    bad_index: list[int]
+
+
 @dataclass
 class PostConfig:            # activation/post.go:27-38
     min_num_units: int = 1
@@ -84,6 +108,9 @@ def _bind():
     L.b200post_load_metadata.argtypes = [ctypes.c_char_p, ctypes.POINTER(_Metadata)]
     L.b200post_default_post_config.argtypes = [ctypes.POINTER(_PostConfig)]
     L.b200post_default_post_config.restype = None
+    L.b200post_verify_pos.argtypes = [ctypes.c_char_p, ctypes.POINTER(_VerifyPosOpts), ctypes.POINTER(_VerifyPosResult), vp]
+    L.b200post_verify_pos_sample.argtypes = [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_double, vp,
+                                             ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]
     L._setup_bound = True
     return L
 
@@ -101,6 +128,33 @@ def load_metadata(data_dir: str) -> dict:
                 num_units=m.num_units, max_file_size=m.max_file_size, scrypt_n=m.scrypt_n,
                 nonce=int(m.nonce) if m.has_nonce else None, nonce_value=bytes(m.nonce_value) if m.has_nonce else None,
                 last_position=m.last_position)
+
+
+def verify_pos(data_dir: str, *, fraction: float = 0.2, provider_id: int = 0, from_file: int = 0, to_file: int = -1,
+               seed: int = 0, progress: ctypes.c_uint64 | None = None, cancel: ctypes.c_int | None = None) -> VerifyPosResult:
+    """postcli -verify: recompute `fraction` percent of each file's labels on the GPU and compare them with the stored
+    bytes.  Returns the result for OK, ERR_LABEL_MISMATCH (data invalid), ERR_STATE (labels fine, but the metadata has no
+    VRF nonce: initialisation has not finished) and ERR_CANCELLED; raises on other errors."""
+    o = _VerifyPosOpts(provider_id, fraction, from_file, to_file, seed,
+                       ctypes.addressof(progress) if progress is not None else None)
+    r = _VerifyPosResult()
+    rc = _bind().b200post_verify_pos(data_dir.encode(), ctypes.byref(o), ctypes.byref(r),
+                                     ctypes.addressof(cancel) if cancel is not None else None)
+    if rc not in (OK, ERR_LABEL_MISMATCH, ERR_STATE, ERR_CANCELLED):
+        _err(rc)
+    return VerifyPosResult(rc, r.files_checked, r.labels_checked, r.mismatches, r.seed, bool(r.nonce_ok), bool(r.argmin_checked),
+                           bool(r.argmin_ok), [int(r.bad_index[i]) for i in range(r.n_reported)])
+
+
+def verify_pos_sample(seed: int, file: int, labels_in_file: int, fraction: float):
+    """The positions (within the file, ascending, numpy uint64) that verify_pos checks for this seed and file."""
+    import numpy as np
+    L = _bind()
+    n = ctypes.c_uint64()
+    _err(L.b200post_verify_pos_sample(seed, file, labels_in_file, fraction, None, 0, ctypes.byref(n)))
+    out = np.empty(n.value, dtype=np.uint64)
+    _err(L.b200post_verify_pos_sample(seed, file, labels_in_file, fraction, out.ctypes.data, n.value, ctypes.byref(n)))
+    return out
 
 
 class PostSetupManager:

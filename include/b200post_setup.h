@@ -110,6 +110,45 @@ int b200post_setup_commitment_atx(b200post_setup_manager *mgr, uint8_t out[32]);
 /* initialization.LoadMetadata: B200POST_ERR_IO + "metadata file is missing" text if absent. */
 int b200post_load_metadata(const char *data_dir, b200post_post_metadata *out);
 
+/*
+ * Checking stored POST data (postcli -verify; spacemeshos/post verifying.VerifyPos, from memory, unpinned):
+ * recompute a share of each file's labels on the GPU and compare them with the bytes in postdata_N.bin.
+ * Inputs come from postdata_metadata.json (commitment = blake3(NodeId || CommitmentAtxId), N, file size, label count).
+ * Host-side errors come first: bad arguments -> INVALID_ARGUMENT; no metadata -> ERR_IO "metadata file is missing";
+ * a file whose size differs from what the metadata implies (the last file may be short) -> ERR_IO "incomplete";
+ * then, without a GPU, ERR_NO_DEVICE (there is no CPU path).  Any mismatch, or a VRF nonce whose recomputed label
+ * differs from NonceValue, returns B200POST_ERR_LABEL_MISMATCH with `out` filled.  When every checked label matches but the metadata has no VRF nonce
+ * (initialisation stopped before finding it), the call returns B200POST_ERR_STATE with `out` filled, nonce_ok = 0 and
+ * argmin_checked = 0.  A set *cancel returns B200POST_ERR_CANCELLED with partial counts.
+ * A file of L labels contributes max(1, floor(L * fraction / 100)) distinct positions (all of them at 100), a
+ * deterministic function of (seed, file index), so shards and re-runs check the same labels.
+ */
+typedef struct b200post_verify_pos_opts {
+    int64_t provider_id;         /* CUDA ordinal or B200POST_PROVIDER_ALL                                  */
+    double fraction;             /* percent of each file's labels, (0, 100]; 100 = every label             */
+    uint64_t from_file;          /* first postdata_N.bin                                                    */
+    int64_t to_file;             /* last file, inclusive; -1 = the POST's last file                         */
+    uint64_t seed;               /* sample seed; 0 = draw one from the OS (returned in the result)          */
+    volatile uint64_t *progress; /* optional: labels checked so far                                         */
+} b200post_verify_pos_opts;
+
+typedef struct b200post_verify_pos_result {
+    uint64_t files_checked, labels_checked, mismatches, seed;
+    uint32_t nonce_ok;                    /* label32 at metadata Nonce == NonceValue (0 when there is no nonce)       */
+    uint32_t argmin_checked, argmin_ok;   /* full check of every file with a nonce: the fused VRF scan agrees with it  */
+    uint32_t n_reported;
+    uint64_t bad_index[64];               /* lowest mismatching global label indices, ascending                      */
+} b200post_verify_pos_result;
+
+/* provider 0, fraction 0.2, all files, seed 0 */
+void b200post_default_verify_pos_opts(b200post_verify_pos_opts *o);
+int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o, b200post_verify_pos_result *out,
+                        const volatile int *cancel);
+/* Which positions (within the file, ascending) a seed checks, for reproducing a run: *n = the sample size; out
+ * (may be NULL to ask for the size only) receives them when cap >= *n, else INVALID_ARGUMENT. */
+int b200post_verify_pos_sample(uint64_t seed, uint64_t file, uint64_t labels_in_file, double fraction,
+                               uint64_t *out, uint64_t cap, uint64_t *n);
+
 #ifdef __cplusplus
 }
 #endif
