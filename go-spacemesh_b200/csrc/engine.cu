@@ -15,6 +15,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <memory>
 #include <vector>
 
 #include "../../include/b200post.h"
@@ -29,57 +30,41 @@ static thread_local std::string t_error;
 void set_error(const std::string &msg) { t_error = msg; }
 const char *last_error() { return t_error.c_str(); }
 
-#define CU_TRY(expr)                                                                                     \
-    do {                                                                                                 \
-        cudaError_t e__ = (expr);                                                                        \
-        if (e__ != cudaSuccess) {                                                                        \
-            set_error(std::string(#expr) + ": " + cudaGetErrorString(e__));                              \
-            return e__ == cudaErrorMemoryAllocation ? B200POST_ERR_OUT_OF_MEMORY : B200POST_ERR_CUDA;    \
-        }                                                                                                \
-    } while (0)
-
 static inline uint32_t round_up(uint32_t x, uint32_t m) { return (x + m - 1) / m * m; }
 
 DeviceEngine::DeviceEngine(int device) : dev_(device) { cudaGetDeviceProperties(&prop_, device); }
 
 DeviceEngine::~DeviceEngine() {
+    // the members free themselves after this body, on this device and with no work of the engine in flight
     cudaSetDevice(dev_);
-    release();
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
+    if (copy_stream_.get()) cudaStreamSynchronize(copy_stream_.get());
 }
 
-void DeviceEngine::release() {
-    if (stream_) cudaStreamSynchronize(stream_);
-    if (copy_stream_) cudaStreamSynchronize(copy_stream_);
-    cudaFree(V_raw_); V_raw_ = nullptr; V_ = nullptr; v_bytes_ = 0; v_align_ = 0;
-    for (int b = 0; b < 2; b++) {
-        cudaFree(X_[b]); X_[b] = nullptr;
-        cudaFree(d_out_[b]); d_out_[b] = nullptr;
-        cudaFreeHost(h_out_[b]); h_out_[b] = nullptr;
-        cudaFree(d_commit_[b]); d_commit_[b] = nullptr;
-        cudaFree(d_idx_[b]); d_idx_[b] = nullptr;
-        cudaFreeHost(h_commit_[b]); h_commit_[b] = nullptr;
-        cudaFreeHost(h_idx_[b]); h_idx_[b] = nullptr;
-        cudaFree(d_cidx_[b]); d_cidx_[b] = nullptr; cudaFreeHost(h_cidx_[b]); h_cidx_[b] = nullptr;
-        cudaFree(d_exp_[b]); d_exp_[b] = nullptr; cudaFreeHost(h_exp_[b]); h_exp_[b] = nullptr;
-        cudaFree(d_bits_[b]); d_bits_[b] = nullptr;
-        cudaFree(d_cnt_[b]); d_cnt_[b] = nullptr; cudaFreeHost(h_cnt_[b]); h_cnt_[b] = nullptr;
-        cudaEvent_t *evs[] = {&ev_done_[b], &ev_in_[b], &ev_k3_[b], &ev_k2a_[b], &ev_k2b_[b], &ev_call_[b], &ev_exp_[b]};
-        for (cudaEvent_t *e : evs) { if (*e) cudaEventDestroy(*e); *e = nullptr; }
-        k2_pending_[b] = false; in_pending_[b] = false; pend_[b].live = false;
-    }
-    for (int b = 0; b < 2; b++) { if (ev_timer_[b]) cudaEventDestroy(ev_timer_[b]); ev_timer_[b] = nullptr; }
-    cudaFree(d_ctab_); d_ctab_ = nullptr; ctab_rows_ = 0;
-    cudaFree(d_range_commit_); d_range_commit_ = nullptr;
-    cudaFree(d_diff_); d_diff_ = nullptr;
-    cudaFree(d_cta_cand_); d_cta_cand_ = nullptr;
-    cudaFree(d_running_); d_running_ = nullptr;
-    cudaFreeHost(h_running_); h_running_ = nullptr;
-    if (stream_) cudaStreamDestroy(stream_);
-    if (copy_stream_) cudaStreamDestroy(copy_stream_);
-    copy_stream_ = nullptr;
-    stream_ = nullptr;
-    alloc_slots_ = 0;
-    wave_slots_ = 0;
+int DeviceEngine::Layer::allocate(uint32_t slots) {
+    CUDA_TRY(X.resize((size_t)slots * 8));
+    CUDA_TRY(d_out.resize((size_t)slots * 16));
+    CUDA_TRY(h_out.resize((size_t)slots * 16));
+    CUDA_TRY(d_commit.resize((size_t)slots * 32));
+    CUDA_TRY(h_commit.resize((size_t)slots * 32));
+    CUDA_TRY(d_idx.resize(slots));
+    CUDA_TRY(h_idx.resize(slots));
+    CUDA_TRY(d_cidx.resize(slots));
+    CUDA_TRY(h_cidx.resize(slots));
+    CUDA_TRY(d_exp.resize((size_t)slots * 16));
+    CUDA_TRY(h_exp.resize((size_t)slots * 16));
+    CUDA_TRY(d_bits.resize(slots / 32));
+    CUDA_TRY(d_cnt.resize(1));
+    CUDA_TRY(h_cnt.resize(1));
+    CUDA_TRY(ev_done.create(cudaEventDisableTiming));
+    CUDA_TRY(ev_k3.create(cudaEventDisableTiming));
+    CUDA_TRY(ev_in.create(cudaEventDisableTiming));
+    CUDA_TRY(ev_exp.create(cudaEventDisableTiming));
+    CUDA_TRY(ev_k2a.create(cudaEventDefault));
+    CUDA_TRY(ev_k2b.create(cudaEventDefault));
+    in_pending = k2_pending = false;
+    pend.live = false;
+    return B200POST_OK;
 }
 
 // Decide the layer size for scrypt-N and make sure scratch for min(layer, want_slots) slots exists.
@@ -89,29 +74,19 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
     int tpb = (int)o.tpb.load();
     if (variant != ROMIX_PIPELINED && tpb != 128 && tpb != 256) tpb = 128;   // the classic kernels are built for 128/256 only
     const int dr = (int)o.dr_unroll.load();
-    if (!stream_) {
-        CU_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-        CU_TRY(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; b++) {
-            CU_TRY(cudaEventCreateWithFlags(&ev_done_[b], cudaEventDisableTiming));
-            CU_TRY(cudaEventCreateWithFlags(&ev_in_[b], cudaEventDisableTiming));
-            CU_TRY(cudaEventCreateWithFlags(&ev_k3_[b], cudaEventDisableTiming));
-            CU_TRY(cudaEventCreate(&ev_k2a_[b]));
-            CU_TRY(cudaEventCreate(&ev_k2b_[b]));
-            CU_TRY(cudaEventCreate(&ev_call_[b]));
-            CU_TRY(cudaEventCreateWithFlags(&ev_exp_[b], cudaEventDisableTiming));
-            CU_TRY(cudaMalloc(&d_cnt_[b], 4));
-            CU_TRY(cudaMallocHost(&h_cnt_[b], 4));
-        }
-        CU_TRY(cudaMalloc(&d_diff_, 32));
-        CU_TRY(cudaMalloc(&d_range_commit_, 32));
-        CU_TRY(cudaMalloc(&d_running_, sizeof(VrfCandidate)));
-        CU_TRY(cudaMallocHost(&h_running_, sizeof(VrfCandidate)));
+    if (!stream_.get()) {
+        CUDA_TRY(stream_.create(cudaStreamNonBlocking));
+        CUDA_TRY(copy_stream_.create(cudaStreamNonBlocking));
+        for (Event &e : ev_call_) CUDA_TRY(e.create(cudaEventDefault));
+        CUDA_TRY(d_diff_.resize(8));
+        CUDA_TRY(d_range_commit_.resize(8));
+        CUDA_TRY(d_running_.resize(1));
+        CUDA_TRY(h_running_.resize(1));
     }
     const size_t pads = variant == ROMIX_PIPELINED ? 2 : 1;   // scratchpads per slot
     const size_t per_slot = 128 * (size_t)N * pads;
     size_t free_b = 0, total_b = 0;
-    CU_TRY(cudaMemGetInfo(&free_b, &total_b));
+    CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
     size_t budget = (size_t)((double)(free_b + v_bytes_) * 0.95);   // 0.95: headroom for the k2pow engine's dataset and scratchpads (~14 GiB) when it allocates after this one
     const int64_t cap_mib = o.max_scratch_mib.load();
     if (cap_mib > 0) budget = std::min(budget, (size_t)cap_mib << 20);
@@ -144,48 +119,29 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
         wave = budget / per_slot / 32 * 32;
         if (wave == 0) { set_error("not enough HBM for one warp of ROMix scratch"); return B200POST_ERR_OUT_OF_MEMORY; }
     }
+    if (wave != wave_slots_) spec_.valid = false;   // a pre-filled layer has the old layer's shape
     wave_slots_ = (uint32_t)wave;
 
     const uint32_t need = (uint32_t)std::min<uint64_t>(wave, round_up((uint32_t)std::min<uint64_t>(want_slots, wave), 32));
     const size_t need_v = per_slot * (size_t)need;
     if (need_v > v_bytes_ || 128 * (size_t)N * 32 > v_align_) {
-        CU_TRY(cudaStreamSynchronize(stream_));
-        cudaFree(V_raw_); V_raw_ = nullptr; V_ = nullptr; v_bytes_ = 0;
+        CUDA_TRY(cudaStreamSynchronize(stream_.get()));
+        spec_.valid = false;
+        V_raw_.reset(); V_ = nullptr; v_bytes_ = 0;
         // align to the largest per-warp region this allocation can be used with (N * 4 KiB, <= 4 GiB) so
         // that no region straddles a 4 GiB boundary: the kernels do 32-bit address arithmetic inside one
         const size_t align = std::min<size_t>(128 * (size_t)N * 32, (size_t)1 << 32);
-        CU_TRY(cudaMalloc(&V_raw_, need_v + align));
-        V_ = reinterpret_cast<uint4 *>(((uintptr_t)V_raw_ + align - 1) / align * align);
+        CUDA_TRY(V_raw_.resize(need_v + align));
+        V_ = reinterpret_cast<uint4 *>(((uintptr_t)V_raw_.get() + align - 1) / align * align);
         v_bytes_ = need_v;
         v_align_ = align;
     }
     if (need > alloc_slots_) {
-        CU_TRY(cudaStreamSynchronize(stream_));
-        for (int b = 0; b < 2; b++) {
-            cudaFree(X_[b]); cudaFree(d_commit_[b]); cudaFree(d_idx_[b]); cudaFree(d_out_[b]); cudaFree(d_cidx_[b]);
-            cudaFreeHost(h_commit_[b]); cudaFreeHost(h_idx_[b]); cudaFreeHost(h_out_[b]); cudaFreeHost(h_cidx_[b]);
-            cudaFree(d_exp_[b]); cudaFreeHost(h_exp_[b]); cudaFree(d_bits_[b]);
-            d_cidx_[b] = nullptr; h_cidx_[b] = nullptr; d_exp_[b] = nullptr; h_exp_[b] = nullptr; d_bits_[b] = nullptr;
-            X_[b] = nullptr; d_commit_[b] = nullptr; d_idx_[b] = nullptr; d_out_[b] = nullptr;
-            h_commit_[b] = nullptr; h_idx_[b] = nullptr; h_out_[b] = nullptr;
-        }
-        cudaFree(d_cta_cand_); d_cta_cand_ = nullptr;
+        CUDA_TRY(cudaStreamSynchronize(stream_.get()));
+        spec_.valid = false;
         alloc_slots_ = 0;
-        for (int b = 0; b < 2; b++) {
-            CU_TRY(cudaMalloc(&X_[b], (size_t)need * 128));
-            CU_TRY(cudaMalloc(&d_commit_[b], (size_t)need * 32));
-            CU_TRY(cudaMalloc(&d_idx_[b], (size_t)need * 8));
-            CU_TRY(cudaMalloc(&d_out_[b], (size_t)need * 16));
-            CU_TRY(cudaMallocHost(&h_commit_[b], (size_t)need * 32));
-            CU_TRY(cudaMallocHost(&h_idx_[b], (size_t)need * 8));
-            CU_TRY(cudaMallocHost(&h_out_[b], (size_t)need * 16));
-            CU_TRY(cudaMalloc(&d_cidx_[b], (size_t)need * 4));
-            CU_TRY(cudaMallocHost(&h_cidx_[b], (size_t)need * 4));
-            CU_TRY(cudaMalloc(&d_exp_[b], (size_t)need * 16));
-            CU_TRY(cudaMallocHost(&h_exp_[b], (size_t)need * 16));
-            CU_TRY(cudaMalloc(&d_bits_[b], (size_t)need / 32 * 4));
-        }
-        CU_TRY(cudaMalloc(&d_cta_cand_, (size_t)pbkdf2_final_ctas(need) * sizeof(VrfCandidate)));
+        for (Layer &l : layer_) { int rc = l.allocate(need); if (rc) return rc; }
+        CUDA_TRY(d_cta_cand_.resize(pbkdf2_final_ctas(need)));
         alloc_slots_ = need;
     }
     return B200POST_OK;
@@ -193,106 +149,101 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
 
 // collect the ROMix device time recorded under parity `buf` (blocks until that launch has finished)
 void DeviceEngine::harvest(int buf) {
-    if (!k2_pending_[buf]) return;
+    Layer &l = layer_[buf];
+    if (!l.k2_pending) return;
     float ms = 0;
-    if (cudaEventSynchronize(ev_k2b_[buf]) == cudaSuccess &&
-        cudaEventElapsedTime(&ms, ev_k2a_[buf], ev_k2b_[buf]) == cudaSuccess) {
-        romix_ms_ += ms; romix_launches_++; romix_labels_ += k2_labels_[buf];
+    if (cudaEventSynchronize(l.ev_k2b.get()) == cudaSuccess &&
+        cudaEventElapsedTime(&ms, l.ev_k2a.get(), l.ev_k2b.get()) == cudaSuccess) {
+        romix_ms_ += ms; romix_launches_++; romix_labels_ += l.k2_labels;
     }
-    k2_pending_[buf] = false;
+    l.k2_pending = false;
 }
 
 int DeviceEngine::retire(const Job &job, int b) {
-    if (!pend_[b].live) return B200POST_OK;
-    CU_TRY(cudaEventSynchronize(ev_done_[b]));
-    if (job.out_host) memcpy(job.out_host + pend_[b].off * 16, h_out_[b], (size_t)pend_[b].n * 16);
-    if (job.cmp && *h_cnt_[b]) {
+    Layer &l = layer_[b];
+    if (!l.pend.live) return B200POST_OK;
+    CUDA_TRY(cudaEventSynchronize(l.ev_done.get()));
+    if (job.out_host) memcpy(job.out_host + l.pend.off * 16, l.h_out.get(), (size_t)l.pend.n * 16);
+    if (job.cmp && *l.h_cnt.get()) {
         // rare path: the layer has mismatches; fetch its bitmap and decode positions (ascending: layers retire in order)
-        std::vector<uint32_t> bits(round_up(pend_[b].n, 32) / 32);
-        CU_TRY(cudaMemcpy(bits.data(), d_bits_[b], bits.size() * 4, cudaMemcpyDeviceToHost));
-        job.cmp->mismatches += *h_cnt_[b];
+        std::vector<uint32_t> bits(round_up(l.pend.n, 32) / 32);
+        CUDA_TRY(cudaMemcpy(bits.data(), l.d_bits.get(), bits.size() * 4, cudaMemcpyDeviceToHost));
+        job.cmp->mismatches += *l.h_cnt.get();
         for (size_t w = 0; w < bits.size() && job.cmp->first.size() < CompareResult::kMaxReported; w++)
             for (uint32_t v = bits[w]; v && job.cmp->first.size() < CompareResult::kMaxReported; v &= v - 1)
-                job.cmp->first.push_back(pend_[b].off + 32 * w + (uint64_t)__builtin_ctz(v));
+                job.cmp->first.push_back(l.pend.off + 32 * w + (uint64_t)__builtin_ctz(v));
     }
-    pend_[b].live = false;
+    l.pend.live = false;
     return B200POST_OK;
 }
 
 int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj) {
+    Layer &l = layer_[b];
     const uint64_t off = layer * (uint64_t)std::min<uint64_t>(wave_slots_, alloc_slots_);
-    if (job.gather && job.commit_index) {
-        if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
-        memcpy(h_cidx_[b], job.commit_index + off, (size_t)n_valid * 4);
-        memcpy(h_idx_[b], job.indices + off, (size_t)n_valid * 8);
-        CU_TRY(cudaMemcpyAsync(d_cidx_[b], h_cidx_[b], (size_t)n_valid * 4, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaMemcpyAsync(d_idx_[b], h_idx_[b], (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaEventRecord(ev_in_[b], stream_));
-        in_pending_[b] = true;
-        *lj = LabelJob{reinterpret_cast<const uint32_t *>(d_ctab_), 0, d_idx_[b], 0, n_valid, d_cidx_[b]};
-    } else if (job.gather && !job.commitments) {
-        // one commitment for every item (compare jobs): only the indices travel
-        if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
-        memcpy(h_idx_[b], job.indices + off, (size_t)n_valid * 8);
-        CU_TRY(cudaMemcpyAsync(d_idx_[b], h_idx_[b], (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaEventRecord(ev_in_[b], stream_));
-        in_pending_[b] = true;
-        *lj = LabelJob{d_range_commit_, 0, d_idx_[b], 0, n_valid, nullptr};
-    } else if (job.gather) {
-        if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
-        memcpy(h_commit_[b], job.commitments + off * 32, (size_t)n_valid * 32);
-        memcpy(h_idx_[b], job.indices + off, (size_t)n_valid * 8);
-        CU_TRY(cudaMemcpyAsync(d_commit_[b], h_commit_[b], (size_t)n_valid * 32, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaMemcpyAsync(d_idx_[b], h_idx_[b], (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaEventRecord(ev_in_[b], stream_));
-        in_pending_[b] = true;
-        *lj = LabelJob{reinterpret_cast<const uint32_t *>(d_commit_[b]), 8, d_idx_[b], 0, n_valid, nullptr};
-    } else {
-        *lj = LabelJob{d_range_commit_, 0, nullptr, job.start + off, n_valid, nullptr};
+    *lj = LabelJob{d_range_commit_.get(), 0, nullptr, job.start + off, n_valid, nullptr};
+    if (job.gather) {
+        // the staging buffers of this parity are free once the previous layer's inputs have left them
+        if (l.in_pending) { CUDA_TRY(cudaEventSynchronize(l.ev_in.get())); l.in_pending = false; }
+        memcpy(l.h_idx.get(), job.indices + off, (size_t)n_valid * 8);
+        CUDA_TRY(cudaMemcpyAsync(l.d_idx.get(), l.h_idx.get(), (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_.get()));
+        lj->indices = l.d_idx.get();
+        lj->start = 0;
+        if (job.commit_index) {
+            memcpy(l.h_cidx.get(), job.commit_index + off, (size_t)n_valid * 4);
+            CUDA_TRY(cudaMemcpyAsync(l.d_cidx.get(), l.h_cidx.get(), (size_t)n_valid * 4, cudaMemcpyHostToDevice, stream_.get()));
+            lj->commit = reinterpret_cast<const uint32_t *>(d_ctab_.get());
+            lj->commit_index = l.d_cidx.get();
+        } else if (job.commitments) {
+            memcpy(l.h_commit.get(), job.commitments + off * 32, (size_t)n_valid * 32);
+            CUDA_TRY(cudaMemcpyAsync(l.d_commit.get(), l.h_commit.get(), (size_t)n_valid * 32, cudaMemcpyHostToDevice, stream_.get()));
+            lj->commit = reinterpret_cast<const uint32_t *>(l.d_commit.get());
+            lj->commit_stride = 8;
+        }   // else one commitment for every item (compare jobs): only the indices travel
+        CUDA_TRY(cudaEventRecord(l.ev_in.get(), stream_.get()));
+        l.in_pending = true;
     }
-    CU_TRY(launch_pbkdf2_expand(*lj, X_[b], alloc_slots_, round_up(n_valid, 32), stream_));
+    CUDA_TRY(launch_pbkdf2_expand(*lj, l.X.get(), alloc_slots_, round_up(n_valid, 32), stream_.get()));
     g_launches += 1;
     return B200POST_OK;
 }
 
 int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj) {
+    Layer &l = layer_[b];
     const uint64_t off = layer * (uint64_t)std::min<uint64_t>(wave_slots_, alloc_slots_);
     const uint32_t n_slots = round_up(n_valid, 32);
     if (job.expect_host) {
         // K3c: the expected slice goes H2D on the copy stream (pinned staging, double-buffered by parity; retire(b) has
-        // seen the previous copy out of h_exp_[b] finish), and K3c waits for it by event
-        memcpy(h_exp_[b], job.expect_host + off * 16, (size_t)n_valid * 16);
-        CU_TRY(cudaMemcpyAsync(d_exp_[b], h_exp_[b], (size_t)n_valid * 16, cudaMemcpyHostToDevice, copy_stream_));
-        CU_TRY(cudaEventRecord(ev_exp_[b], copy_stream_));
-        CU_TRY(cudaStreamWaitEvent(stream_, ev_exp_[b], 0));
-        CU_TRY(cudaMemsetAsync(d_cnt_[b], 0, 4, stream_));
-        CU_TRY(launch_pbkdf2_final_compare(lj, X_[b], alloc_slots_, n_slots, d_exp_[b], d_bits_[b], d_cnt_[b], job.d_diff,
-                                           d_cta_cand_, stream_));
+        // seen the previous copy out of h_exp finish), and K3c waits for it by event
+        memcpy(l.h_exp.get(), job.expect_host + off * 16, (size_t)n_valid * 16);
+        CUDA_TRY(cudaMemcpyAsync(l.d_exp.get(), l.h_exp.get(), (size_t)n_valid * 16, cudaMemcpyHostToDevice, copy_stream_.get()));
+        CUDA_TRY(cudaEventRecord(l.ev_exp.get(), copy_stream_.get()));
+        CUDA_TRY(cudaStreamWaitEvent(stream_.get(), l.ev_exp.get(), 0));
+        CUDA_TRY(cudaMemsetAsync(l.d_cnt.get(), 0, 4, stream_.get()));
+        CUDA_TRY(launch_pbkdf2_final_compare(lj, l.X.get(), alloc_slots_, n_slots, l.d_exp.get(), l.d_bits.get(), l.d_cnt.get(),
+                                           job.d_diff, d_cta_cand_.get(), stream_.get()));
     } else {
-        uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : d_out_[b];
-        CU_TRY(launch_pbkdf2_final(lj, X_[b], alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_, stream_));
+        uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : l.d_out.get();
+        CUDA_TRY(launch_pbkdf2_final(lj, l.X.get(), alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_.get(), stream_.get()));
     }
     g_launches += 1;
     if (job.d_diff) {
-        CU_TRY(launch_vrf_merge(d_cta_cand_, pbkdf2_final_ctas(n_slots), d_running_, stream_));
+        CUDA_TRY(launch_vrf_merge(d_cta_cand_.get(), pbkdf2_final_ctas(n_slots), d_running_.get(), stream_.get()));
         g_launches += 1;
     }
-    if (job.out_host) {
-        // the copy runs on its own stream: the next layers' kernels do not queue behind PCIe
-        CU_TRY(cudaEventRecord(ev_k3_[b], stream_));
-        CU_TRY(cudaStreamWaitEvent(copy_stream_, ev_k3_[b], 0));
-        CU_TRY(cudaMemcpyAsync(h_out_[b], d_out_[b], (size_t)n_valid * 16, cudaMemcpyDeviceToHost, copy_stream_));
-        CU_TRY(cudaEventRecord(ev_done_[b], copy_stream_));
-    } else if (job.expect_host) {
-        // only the 4-byte count comes back per layer; the bitmap follows in retire() when it is non-zero
-        CU_TRY(cudaEventRecord(ev_k3_[b], stream_));
-        CU_TRY(cudaStreamWaitEvent(copy_stream_, ev_k3_[b], 0));
-        CU_TRY(cudaMemcpyAsync(h_cnt_[b], d_cnt_[b], 4, cudaMemcpyDeviceToHost, copy_stream_));
-        CU_TRY(cudaEventRecord(ev_done_[b], copy_stream_));
+    if (job.out_host || job.expect_host) {
+        // the copy runs on its own stream: the next layers' kernels do not queue behind PCIe.  A compare job brings
+        // back only its 4-byte count; the bitmap follows in retire() when it is non-zero.
+        CUDA_TRY(cudaEventRecord(l.ev_k3.get(), stream_.get()));
+        CUDA_TRY(cudaStreamWaitEvent(copy_stream_.get(), l.ev_k3.get(), 0));
+        if (job.expect_host)
+            CUDA_TRY(cudaMemcpyAsync(l.h_cnt.get(), l.d_cnt.get(), 4, cudaMemcpyDeviceToHost, copy_stream_.get()));
+        else
+            CUDA_TRY(cudaMemcpyAsync(l.h_out.get(), l.d_out.get(), (size_t)n_valid * 16, cudaMemcpyDeviceToHost, copy_stream_.get()));
+        CUDA_TRY(cudaEventRecord(l.ev_done.get(), copy_stream_.get()));
     } else {
-        CU_TRY(cudaEventRecord(ev_done_[b], stream_));
+        CUDA_TRY(cudaEventRecord(l.ev_done.get(), stream_.get()));
     }
-    pend_[b] = Pending{off, n_valid, true};
+    l.pend = Layer::Pending{off, n_valid, true};
     return B200POST_OK;
 }
 
@@ -301,50 +252,43 @@ int DeviceEngine::run_job(const Job &job) {
     const uint64_t M = (job.total + S - 1) / S;
     int rc_ = B200POST_OK, status = B200POST_OK;
     auto layer_count = [&](uint64_t m) { return (uint32_t)std::min<uint64_t>(S, job.total - m * S); };
+    cudaStream_t st = stream_.get();
 
     // small jobs (a proof's K2 labels, one VRF-nonce label, ...): the low-latency kernel, one launch
     const int64_t lowlat_max = options().lowlat_max_labels.load();
     const bool lowlat = variant_ == ROMIX_PIPELINED && M == 1 && lowlat_max > 0 && job.total <= (uint64_t)lowlat_max &&
                         job.total <= (uint64_t)prop_.multiProcessorCount * 4 * 32;
-    if (lowlat) {
-        spec_.valid = false;
-        if (job.cancel && *job.cancel) return B200POST_ERR_CANCELLED;
-        for (int b = 0; b < 2; b++) { if ((rc_ = retire(job, b))) return rc_; harvest(b); }
-        const uint32_t n_valid = (uint32_t)job.total;
-        LabelJob lj;
-        if ((rc_ = stage_layer(job, 0, 0, n_valid, &lj))) return rc_;
-        RomixParams rp;
-        rp.V = V_; rp.X = X_[0]; rp.x_stride = alloc_slots_; rp.N = (uint32_t)job.N; rp.n_slots = n_valid; rp.flags = 0;
-        CU_TRY(cudaEventRecord(ev_k2a_[0], stream_));
-        CU_TRY(launch_romix_lowlat(mw_, rp, romix_lowlat_warps(n_valid, prop_.multiProcessorCount), stream_));
-        CU_TRY(cudaEventRecord(ev_k2b_[0], stream_));
-        k2_pending_[0] = true; k2_labels_[0] = n_valid;
-        g_launches += 1;
-        if ((rc_ = finish_layer(job, 0, 0, n_valid, lj))) return rc_;
-    } else if (variant_ != ROMIX_PIPELINED) {
+    if (lowlat || variant_ != ROMIX_PIPELINED) {
+        // one ROMix launch per layer: the low-latency kernel (a single layer) or a classic variant
         spec_.valid = false;
         for (uint64_t m = 0; m < M; m++) {
             if (job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; break; }
             const int b = (int)(m & 1);
+            Layer &l = layer_[b];
             if ((rc_ = retire(job, b))) return rc_;
             harvest(b);
             const uint32_t n_valid = layer_count(m);
             LabelJob lj;
             if ((rc_ = stage_layer(job, m, b, n_valid, &lj))) return rc_;
             RomixParams rp;
-            rp.V = V_; rp.X = X_[b]; rp.x_stride = alloc_slots_; rp.N = (uint32_t)job.N; rp.n_slots = round_up(n_valid, 32);
-            rp.flags = (uint32_t)options().debug_skip_phase.load();
-            CU_TRY(cudaEventRecord(ev_k2a_[b], stream_));
-            CU_TRY(launch_romix(variant_, mw_, tpb_, rp, stream_));
-            CU_TRY(cudaEventRecord(ev_k2b_[b], stream_));
-            k2_pending_[b] = true; k2_labels_[b] = n_valid;
+            rp.V = V_; rp.X = l.X.get(); rp.x_stride = alloc_slots_; rp.N = (uint32_t)job.N;
+            CUDA_TRY(cudaEventRecord(l.ev_k2a.get(), st));
+            if (lowlat) {
+                rp.n_slots = n_valid; rp.flags = 0;
+                CUDA_TRY(launch_romix_lowlat(mw_, rp, romix_lowlat_warps(n_valid, prop_.multiProcessorCount), st));
+            } else {
+                rp.n_slots = round_up(n_valid, 32); rp.flags = (uint32_t)options().debug_skip_phase.load();
+                CUDA_TRY(launch_romix(variant_, mw_, tpb_, rp, st));
+            }
+            CUDA_TRY(cudaEventRecord(l.ev_k2b.get(), st));
+            l.k2_pending = true; l.k2_labels = n_valid;
             g_launches += 1;
             if ((rc_ = finish_layer(job, m, b, n_valid, lj))) return rc_;
         }
     } else {
         // consume a matching speculation: layer 0 of this call was filled by the previous call's last launch
-        const bool resume = !job.gather && spec_.valid && spec_.N == job.N && spec_.next_start == job.start && spec_.slots == S &&
-                            spec_.alloc_slots == alloc_slots_ && spec_.V == V_ && !memcmp(spec_.commitment, cur_commitment_, 32);
+        const bool resume = !job.gather && spec_.valid && spec_.N == job.N && spec_.next_start == job.start &&
+                            !memcmp(spec_.commitment, cur_commitment_, 32);
         const int poff = resume ? spec_.parity : 0;
         spec_.valid = false;
         const bool speculate = !job.gather && options().speculate_next.load() != 0 && M >= 4 && job.start + job.total + S > job.start + job.total;
@@ -355,13 +299,14 @@ int DeviceEngine::run_job(const Job &job) {
         for (uint64_t m = 0; m <= M; m++) {
             if (m < M && job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; break; }
             const int b = par(m);
+            Layer &l = layer_[b];
             harvest(b);
             bool fill = false;
             uint32_t n_fill = 0;
             if (m < M) {
                 nv[b] = layer_count(m);
                 if (m == 0 && resume) {
-                    lj[b] = LabelJob{d_range_commit_, 0, nullptr, job.start, nv[b], nullptr};   // already filled: X_[b] holds its mid-state
+                    lj[b] = LabelJob{d_range_commit_.get(), 0, nullptr, job.start, nv[b], nullptr};   // already filled: X holds its mid-state
                 } else {
                     if ((rc_ = stage_layer(job, m, b, nv[b], &lj[b]))) return rc_;
                     fill = true; n_fill = round_up(nv[b], 32);
@@ -378,31 +323,30 @@ int DeviceEngine::run_job(const Job &job) {
             if (n_fill == 0 && n_mix == 0) continue;   // resumed call: nothing to launch for m = 0
             PipeParams pp;
             pp.V = V_; pp.x_stride = alloc_slots_; pp.N = (uint32_t)job.N;
-            pp.Xfill = X_[b]; pp.Xmix = X_[b ^ 1];
+            pp.Xfill = l.X.get(); pp.Xmix = layer_[b ^ 1].X.get();
             pp.n_fill = n_fill;
             pp.n_mix = n_mix;
             pp.fill_parity = (uint32_t)b;
             pp.cta_trace = nullptr;
             // diagnostics: B200POST_CTA_TRACE=<file> dumps {start ns, end ns, smid} per CTA of the last steady launch
             static const char *trace_path = getenv("B200POST_CTA_TRACE");
-            unsigned long long *d_trace = nullptr;
+            DeviceBuffer<unsigned long long> d_trace;
             const uint32_t n_cta = (std::max(pp.n_fill, pp.n_mix) + tpb_ - 1) / tpb_;
             if (trace_path && m >= 1 && m + 1 == M) {
-                CU_TRY(cudaMalloc(&d_trace, (size_t)n_cta * 24));
-                CU_TRY(cudaMemsetAsync(d_trace, 0, (size_t)n_cta * 24, stream_));
-                pp.cta_trace = d_trace;
+                CUDA_TRY(d_trace.resize((size_t)n_cta * 3));
+                CUDA_TRY(cudaMemsetAsync(d_trace.get(), 0, (size_t)n_cta * 24, st));
+                pp.cta_trace = d_trace.get();
             }
-            CU_TRY(cudaEventRecord(ev_k2a_[b], stream_));
-            CU_TRY(launch_romix_pipe(mw_, tpb_, dr_unroll_, pp, stream_));
-            CU_TRY(cudaEventRecord(ev_k2b_[b], stream_));
-            k2_pending_[b] = true;
-            k2_labels_[b] = 0.5 * ((fill ? (m < M ? nv[b] : (uint32_t)S) : 0) + (m >= 1 ? nv[b ^ 1] : 0));
+            CUDA_TRY(cudaEventRecord(l.ev_k2a.get(), st));
+            CUDA_TRY(launch_romix_pipe(mw_, tpb_, dr_unroll_, pp, st));
+            CUDA_TRY(cudaEventRecord(l.ev_k2b.get(), st));
+            l.k2_pending = true;
+            l.k2_labels = 0.5 * ((fill ? (m < M ? nv[b] : (uint32_t)S) : 0) + (m >= 1 ? nv[b ^ 1] : 0));
             g_launches += 1;
-            if (d_trace) {
+            if (d_trace.get()) {
                 std::vector<unsigned long long> h((size_t)n_cta * 3);
-                CU_TRY(cudaMemcpyAsync(h.data(), d_trace, h.size() * 8, cudaMemcpyDeviceToHost, stream_));
-                CU_TRY(cudaStreamSynchronize(stream_));
-                cudaFree(d_trace);
+                CUDA_TRY(cudaMemcpyAsync(h.data(), d_trace.get(), h.size() * 8, cudaMemcpyDeviceToHost, st));
+                CUDA_TRY(cudaStreamSynchronize(st));
                 if (FILE *f = fopen(trace_path, "w")) {
                     for (uint32_t c = 0; c < n_cta; c++) fprintf(f, "%u,%llu,%llu,%llu\n", c, h[3 * c], h[3 * c + 1], h[3 * c + 2]);
                     fclose(f);
@@ -418,168 +362,137 @@ int DeviceEngine::run_job(const Job &job) {
         }
         if (spec_filled && status == B200POST_OK) {
             spec_.valid = true; spec_.N = job.N; spec_.next_start = job.start + job.total; spec_.parity = par(M);
-            spec_.slots = (uint32_t)S; spec_.alloc_slots = alloc_slots_; spec_.V = V_;
             memcpy(spec_.commitment, cur_commitment_, 32);
         }
     }
     for (int b = 0; b < 2; b++) {
+        Layer &l = layer_[b];
         if ((rc_ = retire(job, b))) return rc_;
         harvest(b);
-        if (in_pending_[b]) { CU_TRY(cudaEventSynchronize(ev_in_[b])); in_pending_[b] = false; }
+        if (l.in_pending) { CUDA_TRY(cudaEventSynchronize(l.ev_in.get())); l.in_pending = false; }
     }
     return status;
 }
 
+int DeviceEngine::call(Job &job, const std::function<int()> &setup) {
+    std::lock_guard<std::mutex> lk(mu_);
+    CUDA_TRY(cudaSetDevice(dev_));
+    if (job.vrf) *job.vrf = VrfResult{};
+    if (job.cmp) *job.cmp = CompareResult{};
+    if (job.total == 0) return B200POST_OK;
+    int rc = ensure(job.N, job.total);
+    if (rc) return rc;
+    cudaStream_t st = stream_.get();
+    CUDA_TRY(cudaEventRecord(ev_call_[0].get(), st));
+    if ((rc = setup())) return rc;
+    // A cancelled job has drained what it started: like a finished one it is timed and counted, without its labels.
+    const int status = run_job(job);
+    if (status != B200POST_OK && status != B200POST_ERR_CANCELLED) { quiesce(); return status; }
+    if (status == B200POST_OK && job.vrf && job.d_diff) {
+        CUDA_TRY(cudaMemcpyAsync(h_running_.get(), d_running_.get(), sizeof(VrfCandidate), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        const VrfCandidate &c = *h_running_.get();
+        job.vrf->found = c.found != 0;
+        if (job.vrf->found) {
+            job.vrf->index = c.index;
+            for (int k = 0; k < 8; k++) {
+                const uint32_t v = c.label_be[k];
+                job.vrf->label32[4 * k] = (uint8_t)(v >> 24); job.vrf->label32[4 * k + 1] = (uint8_t)(v >> 16);
+                job.vrf->label32[4 * k + 2] = (uint8_t)(v >> 8); job.vrf->label32[4 * k + 3] = (uint8_t)v;
+            }
+        }
+    }
+    CUDA_TRY(cudaEventRecord(ev_call_[1].get(), st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0].get(), ev_call_[1].get()) == cudaSuccess) last_call_ms_ = ms; }
+    Metrics &mx = metrics();
+    (job.gather ? mx.gather_calls_total : mx.range_calls_total)++;
+    mx.device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
+    if (status == B200POST_OK && !job.expect_host) (job.gather ? mx.labels_gather_total : mx.labels_range_total) += job.total;
+    if (status == B200POST_ERR_CANCELLED) set_error("cancelled");
+    return status;
+}
+
+// the commitment every item of the call shares (range and compare-indexed jobs); copied from a member, so the
+// caller's buffer is free when this returns
+int DeviceEngine::upload_commitment(const uint8_t commitment[32]) {
+    memcpy(cur_commitment_, commitment, 32);
+    CUDA_TRY(cudaMemcpyAsync(d_range_commit_.get(), cur_commitment_, 32, cudaMemcpyHostToDevice, stream_.get()));
+    return B200POST_OK;
+}
+
 int DeviceEngine::labels_range(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host,
                                uint8_t *out_dev, const uint8_t *vrf_difficulty, VrfResult *vrf, const volatile int *cancel) {
-    return range_call(commitment, N, start, count, out_host, out_dev, nullptr, nullptr, vrf_difficulty, vrf, cancel);
+    Job job;
+    job.start = start; job.total = count; job.N = N; job.out_host = out_host; job.out_dev = out_dev; job.vrf = vrf; job.cancel = cancel;
+    return range_call(job, commitment, vrf_difficulty);
 }
 
 int DeviceEngine::labels_compare_range(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count,
                                        const uint8_t *expect_host, const uint8_t *vrf_difficulty, VrfResult *vrf,
                                        CompareResult *cmp, const volatile int *cancel) {
     if (!expect_host || !cmp) { set_error("compare job without expected labels or result"); return B200POST_ERR_INVALID_ARGUMENT; }
-    return range_call(commitment, N, start, count, nullptr, nullptr, expect_host, cmp, vrf_difficulty, vrf, cancel);
+    Job job;
+    job.start = start; job.total = count; job.N = N; job.expect_host = expect_host; job.cmp = cmp; job.vrf = vrf; job.cancel = cancel;
+    return range_call(job, commitment, vrf_difficulty);
 }
 
-int DeviceEngine::range_call(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host,
-                             uint8_t *out_dev, const uint8_t *expect_host, CompareResult *cmp, const uint8_t *vrf_difficulty,
-                             VrfResult *vrf, const volatile int *cancel) {
-    std::lock_guard<std::mutex> lk(mu_);
-    CU_TRY(cudaSetDevice(dev_));
-    if (vrf) *vrf = VrfResult{};
-    if (cmp) *cmp = CompareResult{};
-    if (count == 0) return B200POST_OK;
-    int rc = ensure(N, count);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ev_call_[0], stream_));
-
-    // per-call constants: commitment, VRF threshold, running candidate
-    memcpy(cur_commitment_, commitment, 32);
-    CU_TRY(cudaMemcpyAsync(d_range_commit_, commitment, 32, cudaMemcpyHostToDevice, stream_));
-    Job job;
-    job.start = start; job.total = count; job.N = N; job.out_host = out_host; job.out_dev = out_dev; job.cancel = cancel;
-    job.expect_host = expect_host; job.cmp = cmp;
-    if (vrf_difficulty) {
+// per-call constants of a range job: commitment, VRF threshold, running candidate
+int DeviceEngine::range_call(Job &job, const uint8_t commitment[32], const uint8_t *vrf_difficulty) {
+    return call(job, [&]() -> int {
+        const int rc = upload_commitment(commitment);
+        if (rc || !vrf_difficulty) return rc;
         uint32_t be[8];
         for (int k = 0; k < 8; k++)
             be[k] = ((uint32_t)vrf_difficulty[4 * k] << 24) | ((uint32_t)vrf_difficulty[4 * k + 1] << 16) |
                     ((uint32_t)vrf_difficulty[4 * k + 2] << 8) | vrf_difficulty[4 * k + 3];
-        CU_TRY(cudaMemcpyAsync(d_diff_, be, 32, cudaMemcpyHostToDevice, stream_));
-        CU_TRY(cudaMemsetAsync(d_running_, 0, sizeof(VrfCandidate), stream_));
-        CU_TRY(cudaStreamSynchronize(stream_));   // `be` is a stack buffer
-        job.d_diff = d_diff_;
-    }
-    const int status = run_job(job);
-    if (status != B200POST_OK && status != B200POST_ERR_CANCELLED) { quiesce(); return status; }
-    if (status == B200POST_OK && vrf_difficulty && vrf) {
-        CU_TRY(cudaMemcpyAsync(h_running_, d_running_, sizeof(VrfCandidate), cudaMemcpyDeviceToHost, stream_));
-        CU_TRY(cudaStreamSynchronize(stream_));
-        vrf->found = h_running_->found != 0;
-        if (vrf->found) {
-            vrf->index = h_running_->index;
-            for (int k = 0; k < 8; k++) {
-                const uint32_t v = h_running_->label_be[k];
-                vrf->label32[4 * k] = (uint8_t)(v >> 24); vrf->label32[4 * k + 1] = (uint8_t)(v >> 16);
-                vrf->label32[4 * k + 2] = (uint8_t)(v >> 8); vrf->label32[4 * k + 3] = (uint8_t)v;
-            }
-        }
-    }
-    CU_TRY(cudaEventRecord(ev_call_[1], stream_));
-    CU_TRY(cudaStreamSynchronize(stream_));
-    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
-    metrics().range_calls_total++; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
-    if (status == B200POST_OK && !expect_host) metrics().labels_range_total += count;
-    if (status == B200POST_ERR_CANCELLED) set_error("cancelled");
-    return status;
+        CUDA_TRY(cudaMemcpyAsync(d_diff_.get(), be, 32, cudaMemcpyHostToDevice, stream_.get()));
+        CUDA_TRY(cudaMemsetAsync(d_running_.get(), 0, sizeof(VrfCandidate), stream_.get()));
+        CUDA_TRY(cudaStreamSynchronize(stream_.get()));   // `be` is a stack buffer
+        job.d_diff = d_diff_.get();
+        return B200POST_OK;
+    });
 }
 
 int DeviceEngine::labels_gather(size_t n_items, const uint8_t *commitments, const uint64_t *indices, uint64_t N, uint8_t *out_host,
                                 uint8_t *out_dev) {
-    std::lock_guard<std::mutex> lk(mu_);
-    CU_TRY(cudaSetDevice(dev_));
-    if (n_items == 0) return B200POST_OK;
-    int rc = ensure(N, n_items);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ev_call_[0], stream_));
     Job job;
-    spec_.valid = false;   // the scratch is about to be reused
     job.gather = true; job.commitments = commitments; job.indices = indices; job.total = n_items; job.N = N;
     job.out_host = out_host; job.out_dev = out_dev;
-    if ((rc = run_job(job))) { quiesce(); return rc; }
-    CU_TRY(cudaEventRecord(ev_call_[1], stream_));
-    CU_TRY(cudaStreamSynchronize(stream_));
-    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
-    metrics().gather_calls_total++; metrics().labels_gather_total += n_items; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
-    return B200POST_OK;
+    return call(job, []() -> int { return B200POST_OK; });
+}
+
+int DeviceEngine::labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
+                                        const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev) {
+    Job job;
+    job.gather = true; job.commit_index = commit_index; job.indices = indices; job.total = n_items; job.N = N;
+    job.out_host = out_host; job.out_dev = out_dev;
+    return call(job, [&]() -> int {
+        CUDA_TRY(d_ctab_.grow(n_commit * 32));
+        CUDA_TRY(cudaMemcpyAsync(d_ctab_.get(), commitments, n_commit * 32, cudaMemcpyHostToDevice, stream_.get()));
+        return B200POST_OK;
+    });
+}
+
+int DeviceEngine::labels_compare_indexed(const uint8_t commitment[32], size_t n_items, const uint64_t *indices, uint64_t N,
+                                         const uint8_t *expect_host, CompareResult *cmp, const volatile int *cancel) {
+    if (!commitment || !indices || !expect_host || !cmp) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    Job job;
+    job.gather = true; job.indices = indices; job.total = n_items; job.N = N; job.expect_host = expect_host; job.cmp = cmp;
+    job.cancel = cancel;
+    return call(job, [&] { return upload_commitment(commitment); });
 }
 
 // After a failed job: drain the stream and forget every in-flight buffer, so that the next call starts clean
 // (the error text of the failure is preserved).
 void DeviceEngine::quiesce() {
     const std::string keep = last_error();
-    if (stream_) cudaStreamSynchronize(stream_);
-    if (copy_stream_) cudaStreamSynchronize(copy_stream_);
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
+    if (copy_stream_.get()) cudaStreamSynchronize(copy_stream_.get());
     cudaGetLastError();
-    for (int b = 0; b < 2; b++) { pend_[b].live = false; k2_pending_[b] = false; in_pending_[b] = false; }
+    for (Layer &l : layer_) { l.pend.live = false; l.k2_pending = false; l.in_pending = false; }
     spec_.valid = false;
     set_error(keep);
-}
-
-int DeviceEngine::labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
-                                        const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev) {
-    std::lock_guard<std::mutex> lk(mu_);
-    CU_TRY(cudaSetDevice(dev_));
-    if (n_items == 0) return B200POST_OK;
-    int rc = ensure(N, n_items);
-    if (rc) return rc;
-    if (n_commit > ctab_rows_) {
-        CU_TRY(cudaStreamSynchronize(stream_));
-        cudaFree(d_ctab_); d_ctab_ = nullptr; ctab_rows_ = 0;
-        CU_TRY(cudaMalloc(&d_ctab_, n_commit * 32));
-        ctab_rows_ = n_commit;
-    }
-    CU_TRY(cudaEventRecord(ev_call_[0], stream_));
-    CU_TRY(cudaMemcpyAsync(d_ctab_, commitments, n_commit * 32, cudaMemcpyHostToDevice, stream_));
-    spec_.valid = false;   // the scratch is about to be reused
-    Job job;
-    job.gather = true; job.commit_index = commit_index; job.indices = indices; job.total = n_items; job.N = N;
-    job.out_host = out_host; job.out_dev = out_dev;
-    if ((rc = run_job(job))) { quiesce(); return rc; }
-    CU_TRY(cudaEventRecord(ev_call_[1], stream_));
-    CU_TRY(cudaStreamSynchronize(stream_));
-    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
-    metrics().gather_calls_total++; metrics().labels_gather_total += n_items; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
-    return B200POST_OK;
-}
-
-int DeviceEngine::labels_compare_indexed(const uint8_t commitment[32], size_t n_items, const uint64_t *indices, uint64_t N,
-                                         const uint8_t *expect_host, CompareResult *cmp, const volatile int *cancel) {
-    std::lock_guard<std::mutex> lk(mu_);
-    CU_TRY(cudaSetDevice(dev_));
-    if (!commitment || !indices || !expect_host || !cmp) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    *cmp = CompareResult{};
-    if (n_items == 0) return B200POST_OK;
-    int rc = ensure(N, n_items);
-    if (rc) return rc;
-    CU_TRY(cudaEventRecord(ev_call_[0], stream_));
-    spec_.valid = false;   // the scratch is about to be reused
-    memcpy(cur_commitment_, commitment, 32);
-    CU_TRY(cudaMemcpyAsync(d_range_commit_, commitment, 32, cudaMemcpyHostToDevice, stream_));
-    CU_TRY(cudaStreamSynchronize(stream_));   // `commitment` belongs to the caller
-    Job job;
-    job.gather = true; job.indices = indices; job.total = n_items; job.N = N;
-    job.expect_host = expect_host; job.cmp = cmp; job.cancel = cancel;
-    if ((rc = run_job(job))) {
-        quiesce();
-        if (rc == B200POST_ERR_CANCELLED) set_error("cancelled");
-        return rc;
-    }
-    CU_TRY(cudaEventRecord(ev_call_[1], stream_));
-    CU_TRY(cudaStreamSynchronize(stream_));
-    { float ms = 0; if (cudaEventElapsedTime(&ms, ev_call_[0], ev_call_[1]) == cudaSuccess) last_call_ms_ = ms; }
-    metrics().gather_calls_total++; metrics().device_ns_total += (uint64_t)(last_call_ms_ * 1e6);
-    return B200POST_OK;
 }
 
 uint32_t DeviceEngine::wave_slots(uint64_t N) {
@@ -591,19 +504,19 @@ uint32_t DeviceEngine::wave_slots(uint64_t N) {
 
 int DeviceEngine::timer_mark(int which) {
     std::lock_guard<std::mutex> lk(mu_);
-    CU_TRY(cudaSetDevice(dev_));
+    CUDA_TRY(cudaSetDevice(dev_));
     if (which < 0 || which > 1) return B200POST_ERR_INVALID_ARGUMENT;
-    if (!stream_) { int rc = ensure(2, 32); if (rc) return rc; }
-    if (!ev_timer_[which]) CU_TRY(cudaEventCreate(&ev_timer_[which]));
-    CU_TRY(cudaEventRecord(ev_timer_[which], stream_));
+    if (!stream_.get()) { int rc = ensure(2, 32); if (rc) return rc; }
+    if (!ev_timer_[which].get()) CUDA_TRY(ev_timer_[which].create(cudaEventDefault));
+    CUDA_TRY(cudaEventRecord(ev_timer_[which].get(), stream_.get()));
     return B200POST_OK;
 }
 
 double DeviceEngine::timer_elapsed_ms() {
     std::lock_guard<std::mutex> lk(mu_);
-    if (!ev_timer_[0] || !ev_timer_[1] || cudaSetDevice(dev_) != cudaSuccess) return -1.0;
+    if (!ev_timer_[0].get() || !ev_timer_[1].get() || cudaSetDevice(dev_) != cudaSuccess) return -1.0;
     float ms = 0;
-    if (cudaEventSynchronize(ev_timer_[1]) != cudaSuccess || cudaEventElapsedTime(&ms, ev_timer_[0], ev_timer_[1]) != cudaSuccess) return -1.0;
+    if (cudaEventSynchronize(ev_timer_[1].get()) != cudaSuccess || cudaEventElapsedTime(&ms, ev_timer_[0].get(), ev_timer_[1].get()) != cudaSuccess) return -1.0;
     return ms;
 }
 

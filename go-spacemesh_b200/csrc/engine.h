@@ -7,12 +7,13 @@
 
 #include <atomic>
 #include <cstdint>
-#include <memory>
+#include <functional>
 #include <mutex>
 #include <string>
 #include <vector>
 
 #include "label_kernels.cuh"
+#include "cuda_util.h"
 
 namespace b200post {
 
@@ -91,17 +92,42 @@ private:
                                                 // (gather with neither: every item uses the call's one commitment)
         const uint8_t *expect_host = nullptr;   // compare job: expected labels, 16 bytes per item in job order
         CompareResult *cmp = nullptr;
+        VrfResult *vrf = nullptr;
         uint64_t start = 0, total = 0, N = 0;
         uint8_t *out_host = nullptr, *out_dev = nullptr;
         const uint32_t *d_diff = nullptr;
         const volatile int *cancel = nullptr;
     };
+    // Everything one layer parity owns: its slot buffers, events and in-flight bookkeeping.
+    struct Layer {
+        DeviceBuffer<uint4> X;
+        DeviceBuffer<uint8_t> d_out, d_commit;
+        PinnedBuffer<uint8_t> h_out, h_commit;          // pinned staging of outputs and gather inputs
+        DeviceBuffer<uint64_t> d_idx;
+        PinnedBuffer<uint64_t> h_idx;
+        DeviceBuffer<uint32_t> d_cidx;                  // indexed gather: per-item commitment rows
+        PinnedBuffer<uint32_t> h_cidx;
+        // compare jobs: expected labels (pinned staging -> device, on copy_stream_), K3c's mismatch bitmap and count
+        DeviceBuffer<uint8_t> d_exp;
+        PinnedBuffer<uint8_t> h_exp;
+        DeviceBuffer<uint32_t> d_bits, d_cnt;
+        PinnedBuffer<uint32_t> h_cnt;
+        Event ev_done;        // layer outputs are in h_out
+        Event ev_k3;          // K3 of the layer has written d_out (the copy stream waits on it)
+        Event ev_in;          // layer inputs have left h_commit / h_idx / h_cidx
+        Event ev_exp;         // the expected slice of the layer is on the device
+        Event ev_k2a, ev_k2b; // bracket the ROMix launch (timed)
+        bool in_pending = false, k2_pending = false;
+        double k2_labels = 0;
+        struct Pending { uint64_t off; uint32_t n; bool live; } pend{0, 0, false};
+        int allocate(uint32_t slots);   // (re)creates every buffer and event for `slots` slots
+    };
+    // the shared body of the label calls: lock, scratch, `setup` (per-call uploads), the timed job, metrics
+    int call(Job &job, const std::function<int()> &setup);
     int ensure(uint64_t N, uint64_t want_slots);   // (re)allocates scratch; sets wave_slots_
-    void release();
     int run_job(const Job &job);
-    int range_call(const uint8_t commitment[32], uint64_t N, uint64_t start, uint64_t count, uint8_t *out_host, uint8_t *out_dev,
-                   const uint8_t *expect_host, CompareResult *cmp, const uint8_t *vrf_difficulty, VrfResult *vrf,
-                   const volatile int *cancel);
+    int range_call(Job &job, const uint8_t commitment[32], const uint8_t *vrf_difficulty);
+    int upload_commitment(const uint8_t commitment[32]);
     // b = buffer parity of the layer (layer index + parity offset of the call)
     int stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj);          // inputs + K1
     int finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj);   // K3 (+K4) + D2H + event
@@ -112,57 +138,35 @@ private:
     int dev_;
     cudaDeviceProp prop_{};
     std::mutex mu_;
-    cudaStream_t stream_ = nullptr;
+    Stream stream_;
+    Stream copy_stream_;                   // D2H of finished labels, off the kernels' stream
     // scratch
-    uint4 *V_ = nullptr;         // aligned view into V_raw_
-    void *V_raw_ = nullptr;
+    DeviceBuffer<uint8_t> V_raw_;
+    uint4 *V_ = nullptr;                   // aligned view into V_raw_
     size_t v_bytes_ = 0, v_align_ = 0;
-    uint32_t alloc_slots_ = 0;   // capacity of the per-slot buffers below
-    uint32_t wave_slots_ = 0;    // slots per layer for the current (N, options)
-    // per-layer state, double-buffered by layer parity
-    uint4 *X_[2] = {nullptr, nullptr};
-    uint8_t *d_out_[2] = {nullptr, nullptr};
-    uint8_t *h_out_[2] = {nullptr, nullptr};       // pinned
-    uint8_t *d_commit_[2] = {nullptr, nullptr};
-    uint64_t *d_idx_[2] = {nullptr, nullptr};
-    uint8_t *h_commit_[2] = {nullptr, nullptr};    // pinned staging for gather inputs
-    uint64_t *h_idx_[2] = {nullptr, nullptr};
-    uint32_t *d_range_commit_ = nullptr;   // the commitment of the current range call (32 bytes)
-    uint32_t *d_cidx_[2] = {nullptr, nullptr}, *h_cidx_[2] = {nullptr, nullptr};   // indexed gather: per-item commitment rows
-    uint8_t *d_ctab_ = nullptr; size_t ctab_rows_ = 0;   // indexed gather: call-level commitment table
-    uint32_t *d_diff_ = nullptr;
-    // compare jobs: expected labels (pinned staging -> device, on copy_stream_), K3c's mismatch bitmap and count
-    uint8_t *h_exp_[2] = {nullptr, nullptr}, *d_exp_[2] = {nullptr, nullptr};
-    uint32_t *d_bits_[2] = {nullptr, nullptr}, *d_cnt_[2] = {nullptr, nullptr}, *h_cnt_[2] = {nullptr, nullptr};
-    cudaEvent_t ev_exp_[2] = {nullptr, nullptr};   // the expected slice of the layer is on the device
-    VrfCandidate *d_cta_cand_ = nullptr;
-    VrfCandidate *d_running_ = nullptr;
-    VrfCandidate *h_running_ = nullptr;            // pinned
-    cudaEvent_t ev_done_[2] = {nullptr, nullptr};  // layer outputs are in h_out_[b]
-    cudaEvent_t ev_k3_[2] = {nullptr, nullptr};    // K3 of the layer has written d_out_[b] (the copy stream waits on it)
-    cudaStream_t copy_stream_ = nullptr;           // D2H of finished labels, off the kernels' stream
-    cudaEvent_t ev_in_[2] = {nullptr, nullptr};    // layer inputs have left h_commit_/h_idx_[b]
-    bool in_pending_[2] = {false, false};
-    cudaEvent_t ev_k2a_[2] = {nullptr, nullptr}, ev_k2b_[2] = {nullptr, nullptr};
-    bool k2_pending_[2] = {false, false};
-    double k2_labels_[2] = {0, 0};
-    struct Pending { uint64_t off; uint32_t n; bool live; } pend_[2] = {{0, 0, false}, {0, 0, false}};
-    cudaEvent_t ev_call_[2] = {nullptr, nullptr};
+    uint32_t alloc_slots_ = 0;             // capacity of the per-slot buffers of layer_
+    uint32_t wave_slots_ = 0;              // slots per layer for the current (N, options)
+    Layer layer_[2];                       // per-layer state, double-buffered by layer parity
+    DeviceBuffer<uint32_t> d_range_commit_;   // the commitment of the current call (32 bytes)
+    DeviceBuffer<uint8_t> d_ctab_;            // indexed gather: call-level commitment table
+    DeviceBuffer<uint32_t> d_diff_;
+    DeviceBuffer<VrfCandidate> d_cta_cand_, d_running_;
+    PinnedBuffer<VrfCandidate> h_running_;
+    Event ev_call_[2];
     double last_call_ms_ = 0;
-    cudaEvent_t ev_timer_[2] = {nullptr, nullptr};
+    Event ev_timer_[2];
     double romix_ms_ = 0, romix_labels_ = 0;
     uint64_t romix_launches_ = 0;
     // Speculative continuation (pipelined range jobs): the launch that mixes the last layer of a call also fills
     // the first layer of the range that would follow it (start + count ...).  If the next call is exactly that
-    // range (same commitment, N, buffers), it starts with that layer already filled, so back-to-back initialize()
-    // batches run as one uninterrupted software pipeline instead of draining after every call.
+    // range (same commitment and N), it starts with that layer already filled, so back-to-back initialize()
+    // batches run as one uninterrupted software pipeline instead of draining after every call.  ensure() drops it
+    // whenever it reallocates the scratch or changes the layer size.
     struct Speculation {
         bool valid = false;
         uint8_t commitment[32] = {0};
         uint64_t N = 0, next_start = 0;
         int parity = 0;
-        uint32_t slots = 0, alloc_slots = 0;
-        const void *V = nullptr;
     } spec_;
     uint8_t cur_commitment_[32] = {0};
     // current tuning

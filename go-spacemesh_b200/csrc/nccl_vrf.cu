@@ -68,8 +68,8 @@ static_assert(sizeof(Record) == 64, "one NCCL element block per rank");
 struct b200post_vrf_comm {
     ncclComm_t comm = nullptr;
     int dev = 0, world = 0, rank = 0;
-    cudaStream_t stream = nullptr;
-    Record *d_send = nullptr, *d_recv = nullptr;
+    Stream stream;
+    DeviceBuffer<Record> d_send, d_recv;
     std::vector<Record> host;
 };
 
@@ -99,10 +99,10 @@ int b200post_vrf_comm_init(uint32_t provider, int rank, int world, const uint8_t
     memcpy(id.bytes, id128, 128);
     int rc = n->init_rank(&c->comm, world, id, rank);
     if (rc) { delete c; return nccl_fail("ncclCommInitRank", rc); }
-    if (cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking) != cudaSuccess || cudaMalloc(&c->d_send, sizeof(Record)) != cudaSuccess ||
-        cudaMalloc(&c->d_recv, sizeof(Record) * (size_t)world) != cudaSuccess) {
+    if (c->stream.create(cudaStreamNonBlocking) != cudaSuccess || c->d_send.resize(1) != cudaSuccess ||
+        c->d_recv.resize((size_t)world) != cudaSuccess) {
         set_error("CUDA allocation for the VRF exchange failed");
-        n->destroy(c->comm); cudaFree(c->d_send); cudaFree(c->d_recv); if (c->stream) cudaStreamDestroy(c->stream);
+        n->destroy(c->comm);
         delete c;
         return B200POST_ERR_CUDA;
     }
@@ -117,11 +117,11 @@ int b200post_vrf_comm_min(b200post_vrf_comm *c, const b200post_vrf_nonce *mine, 
     if (cudaSetDevice(c->dev) != cudaSuccess) { set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
     Record r{};
     r.found = mine->found; r.index = mine->index; memcpy(r.label32, mine->label32, 32);
-    if (cudaMemcpyAsync(c->d_send, &r, sizeof r, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) { set_error("H2D failed"); return B200POST_ERR_CUDA; }
-    const int rc = n->all_gather(c->d_send, c->d_recv, sizeof(Record), 1 /* ncclUint8 */, c->comm, c->stream);
+    if (cudaMemcpyAsync(c->d_send.get(), &r, sizeof r, cudaMemcpyHostToDevice, c->stream.get()) != cudaSuccess) { set_error("H2D failed"); return B200POST_ERR_CUDA; }
+    const int rc = n->all_gather(c->d_send.get(), c->d_recv.get(), sizeof(Record), 1 /* ncclUint8 */, c->comm, c->stream.get());
     if (rc) return nccl_fail("ncclAllGather", rc);
-    if (cudaMemcpyAsync(c->host.data(), c->d_recv, sizeof(Record) * (size_t)c->world, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
-        cudaStreamSynchronize(c->stream) != cudaSuccess) { set_error("VRF exchange failed"); return B200POST_ERR_CUDA; }
+    if (cudaMemcpyAsync(c->host.data(), c->d_recv.get(), sizeof(Record) * (size_t)c->world, cudaMemcpyDeviceToHost, c->stream.get()) != cudaSuccess ||
+        cudaStreamSynchronize(c->stream.get()) != cudaSuccess) { set_error("VRF exchange failed"); return B200POST_ERR_CUDA; }
     memset(best, 0, sizeof *best);
     for (const Record &x : c->host) {
         if (!x.found) continue;
@@ -136,9 +136,7 @@ void b200post_vrf_comm_free(b200post_vrf_comm *c) {
     Nccl *n = nccl();
     cudaSetDevice(c->dev);
     if (n && c->comm) n->destroy(c->comm);
-    cudaFree(c->d_send); cudaFree(c->d_recv);
-    if (c->stream) cudaStreamDestroy(c->stream);
-    delete c;
+    delete c;   // frees the buffers and the stream on c->dev
 }
 
 }  // extern "C"

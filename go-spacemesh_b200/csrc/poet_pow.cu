@@ -145,8 +145,8 @@ int b200post_poet_pow_find(uint32_t provider, const uint8_t *pc, size_t pc_len, 
         return B200POST_ERR_INVALID_ARGUMENT;
     }
     if (cudaSetDevice(e->device()) != cudaSuccess) { set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
-    unsigned long long *d_best = nullptr;
-    if (cudaMalloc(&d_best, 8) != cudaSuccess) { set_error("cudaMalloc failed"); return B200POST_ERR_CUDA; }
+    DeviceBuffer<unsigned long long> d_best;
+    if (d_best.resize(1) != cudaSuccess) { set_error("cudaMalloc failed"); return B200POST_ERR_CUDA; }
     const uint64_t chunk = 1ull << 28;
     const int grid = e->prop().multiProcessorCount * 8;
     uint64_t done = 0;
@@ -155,16 +155,15 @@ int b200post_poet_pow_find(uint32_t provider, const uint8_t *pc, size_t pc_len, 
         if (cancel && *cancel) { rc = B200POST_ERR_CANCELLED; set_error("cancelled"); break; }
         const uint64_t n = std::min<uint64_t>(chunk, max_nonces - done);
         unsigned long long best = ~0ull;
-        cudaMemcpy(d_best, &best, 8, cudaMemcpyHostToDevice);
-        poet_pow_kernel<<<grid, 256>>>(job, start_nonce + done, n, d_best);
+        cudaMemcpy(d_best.get(), &best, 8, cudaMemcpyHostToDevice);
+        poet_pow_kernel<<<grid, 256>>>(job, start_nonce + done, n, d_best.get());
         g_launches += 1;
-        if (cudaMemcpy(&best, d_best, 8, cudaMemcpyDeviceToHost) != cudaSuccess) { set_error(std::string("poet_pow_kernel: ") + cudaGetErrorString(cudaGetLastError())); rc = B200POST_ERR_CUDA; break; }
+        if (cudaMemcpy(&best, d_best.get(), 8, cudaMemcpyDeviceToHost) != cudaSuccess) { set_error(std::string("poet_pow_kernel: ") + cudaGetErrorString(cudaGetLastError())); rc = B200POST_ERR_CUDA; break; }
         done += n;
         if (best != ~0ull) { *nonce = best; rc = B200POST_OK; break; }
     }
     if (rc == B200POST_ERR_INVALID_PROOF) set_error("no valid nonce in the search window");
     if (hashes) *hashes = done;
-    cudaFree(d_best);
     return rc;
 }
 

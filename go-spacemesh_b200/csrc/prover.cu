@@ -106,24 +106,10 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
     }
 }
 
-#define P_TRY(expr)                                                                                                   \
-    do {                                                                                                              \
-        cudaError_t e__ = (expr);                                                                                     \
-        if (e__ != cudaSuccess) {                                                                                     \
-            set_error(std::string(#expr) + ": " + cudaGetErrorString(e__));                                           \
-            return e__ == cudaErrorMemoryAllocation ? B200POST_ERR_OUT_OF_MEMORY : B200POST_ERR_CUDA;                 \
-        }                                                                                                             \
-    } while (0)
-
 // Streaming scan state: device buffers, keys, per-nonce hit lists.
 class Scanner {
 public:
-    ~Scanner() {
-        if (dev_ >= 0) cudaSetDevice(dev_);
-        cudaFree(d_cands_); cudaFree(d_ncands_);
-        for (int b = 0; b < 2; b++) { cudaFree(d_labels_[b]); cudaFreeHost(h_labels_[b]); if (ev_[b]) cudaEventDestroy(ev_[b]); if (st_[b]) cudaStreamDestroy(st_[b]); cudaFree(d_hits_[b]); cudaFree(d_nhits_[b]); cudaFreeHost(h_hits_[b]); cudaFreeHost(h_nhits_[b]); cudaFreeHost(h_ncands_[b]); }
-        cudaFree(d_rk_); cudaFree(d_lazy_); cudaFree(d_tables_);
-    }
+    ~Scanner() { if (dev_ >= 0) cudaSetDevice(dev_); }   // the members free themselves on the scan's device
     int init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
              uint64_t num_labels, uint64_t chunk) {
         DeviceEngine *e = engine_for(provider);
@@ -138,7 +124,7 @@ public:
         // hits per chunk are ~ chunk * nonces * K1/numLabels; leave generous slack, cap the buffer at 64 MiB
         const double expect = (double)chunk * nonces * ((double)k1 / (double)num_labels);
         hit_cap_ = (uint32_t)std::min<double>(std::max<double>(4.0 * expect + 65536.0, 65536.0), 4.0 * 1024 * 1024);
-        P_TRY(cudaSetDevice(dev_));
+        CUDA_TRY(cudaSetDevice(dev_));
         std::vector<uint8_t> rk((size_t)(nonces / 16) * 176), lazy((size_t)nonces * 176);
         for (uint32_t g = 0; g < nonces / 16; g++) {
             uint8_t key[16];
@@ -155,64 +141,66 @@ public:
         static AesTables host_tables;
         static std::once_flag once;
         std::call_once(once, [] { aes_build_tables(host_tables); });
-        P_TRY(cudaMalloc(&d_rk_, rk.size()));
-        P_TRY(cudaMalloc(&d_lazy_, lazy.size()));
-        P_TRY(cudaMalloc(&d_tables_, sizeof(AesTables)));
-        P_TRY(cudaMemcpy(d_rk_, rk.data(), rk.size(), cudaMemcpyHostToDevice));
-        P_TRY(cudaMemcpy(d_lazy_, lazy.data(), lazy.size(), cudaMemcpyHostToDevice));
-        P_TRY(cudaMemcpy(d_tables_, &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice));
+        CUDA_TRY(d_rk_.resize(rk.size()));
+        CUDA_TRY(d_lazy_.resize(lazy.size()));
+        CUDA_TRY(d_tables_.resize(1));
+        CUDA_TRY(cudaMemcpy(d_rk_.get(), rk.data(), rk.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(d_lazy_.get(), lazy.data(), lazy.size(), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(d_tables_.get(), &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice));
         for (int b = 0; b < 2; b++) {
-            P_TRY(cudaStreamCreateWithFlags(&st_[b], cudaStreamNonBlocking));
-            P_TRY(cudaEventCreateWithFlags(&ev_[b], cudaEventDisableTiming));
-            P_TRY(cudaMalloc(&d_labels_[b], chunk * 16));
-            P_TRY(cudaMallocHost(&h_labels_[b], chunk * 16));
-            P_TRY(cudaMalloc(&d_hits_[b], (size_t)hit_cap_ * sizeof(Hit)));
-            P_TRY(cudaMalloc(&d_nhits_[b], 4));
-            P_TRY(cudaMallocHost(&h_hits_[b], (size_t)hit_cap_ * sizeof(Hit)));
-            P_TRY(cudaMallocHost(&h_nhits_[b], 4));
-            P_TRY(cudaMallocHost(&h_ncands_[b], 4));
+            CUDA_TRY(st_[b].create(cudaStreamNonBlocking));
+            CUDA_TRY(ev_[b].create(cudaEventDisableTiming));
+            CUDA_TRY(d_labels_[b].resize(chunk * 16));
+            CUDA_TRY(h_labels_[b].resize(chunk * 16));
+            CUDA_TRY(d_hits_[b].resize(hit_cap_));
+            CUDA_TRY(d_nhits_[b].resize(1));
+            CUDA_TRY(h_hits_[b].resize(hit_cap_));
+            CUDA_TRY(h_nhits_[b].resize(1));
+            CUDA_TRY(h_ncands_[b].resize(1));
         }
         // lazy-cipher candidates: one ciphertext byte in 256 equals the MSB; 2x slack, shared by both buffers
         // (chunks are processed in stream order on alternating streams, so the queue is fenced by events below)
         cand_cap_ = (uint32_t)std::min<uint64_t>((chunk * nonces) / 128 + 65536, 1u << 27);
-        P_TRY(cudaMalloc(&d_cands_, (size_t)cand_cap_ * sizeof(uint2)));
-        P_TRY(cudaMalloc(&d_ncands_, 8));
+        CUDA_TRY(d_cands_.resize(cand_cap_));
+        CUDA_TRY(d_ncands_.resize(2));
         cudaDeviceProp p;
-        P_TRY(cudaGetDeviceProperties(&p, dev_));
+        CUDA_TRY(cudaGetDeviceProperties(&p, dev_));
         grid_ = (uint32_t)p.multiProcessorCount * 6;   // 6 CTAs x 32 KiB of lane-replicated AES table per SM
         return B200POST_OK;
     }
-    uint8_t *staging(int b) { return h_labels_[b]; }
+    uint8_t *staging(int b) { return h_labels_[b].get(); }
     // enqueue chunk in staging(b): labels [first, first+count)
     int submit(int b, uint64_t first, uint32_t count) {
-        P_TRY(cudaMemcpyAsync(d_labels_[b], h_labels_[b], (size_t)count * 16, cudaMemcpyHostToDevice, st_[b]));
-        P_TRY(cudaMemsetAsync(d_nhits_[b], 0, 4, st_[b]));
+        CUDA_TRY(cudaMemcpyAsync(d_labels_[b].get(), h_labels_[b].get(), (size_t)count * 16, cudaMemcpyHostToDevice, st_[b].get()));
+        CUDA_TRY(cudaMemsetAsync(d_nhits_[b].get(), 0, 4, st_[b].get()));
         // the single candidate queue is reused by consecutive chunks: wait for the other stream's lazy pass
-        if (pending_[b ^ 1]) P_TRY(cudaStreamWaitEvent(st_[b], ev_[b ^ 1], 0));
-        P_TRY(cudaMemsetAsync(d_ncands_, 0, 8, st_[b]));
-        prove_scan_kernel<<<grid_, 256, AES_SMEM_BYTES, st_[b]>>>(reinterpret_cast<const uint4 *>(d_labels_[b]), first, count,
-                                                                reinterpret_cast<const uint4 *>(d_rk_), nonces_ / 16, msb_, d_tables_,
-                                                                d_hits_[b], hit_cap_, d_nhits_[b], d_cands_, cand_cap_, d_ncands_);
-        prove_lazy_kernel<<<grid_, 256, AES_SMEM_BYTES, st_[b]>>>(reinterpret_cast<const uint4 *>(d_labels_[b]), first, d_cands_, d_ncands_,
-                                                                cand_cap_, reinterpret_cast<const uint4 *>(d_lazy_), lsb_, d_tables_,
-                                                                d_hits_[b], hit_cap_, d_nhits_[b]);
+        if (pending_[b ^ 1]) CUDA_TRY(cudaStreamWaitEvent(st_[b].get(), ev_[b ^ 1].get(), 0));
+        CUDA_TRY(cudaMemsetAsync(d_ncands_.get(), 0, 8, st_[b].get()));
+        cudaStream_t st = st_[b].get();
+        const uint4 *labels = reinterpret_cast<const uint4 *>(d_labels_[b].get());
+        prove_scan_kernel<<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
+                                                              msb_, d_tables_.get(), d_hits_[b].get(), hit_cap_, d_nhits_[b].get(),
+                                                              d_cands_.get(), cand_cap_, d_ncands_.get());
+        prove_lazy_kernel<<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
+                                                              reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
+                                                              d_hits_[b].get(), hit_cap_, d_nhits_[b].get());
         g_launches += 2;
-        P_TRY(cudaGetLastError());
-        P_TRY(cudaMemcpyAsync(h_ncands_[b], d_ncands_, 4, cudaMemcpyDeviceToHost, st_[b]));
-        P_TRY(cudaMemcpyAsync(h_nhits_[b], d_nhits_[b], 4, cudaMemcpyDeviceToHost, st_[b]));
-        P_TRY(cudaMemcpyAsync(h_hits_[b], d_hits_[b], (size_t)hit_cap_ * sizeof(Hit), cudaMemcpyDeviceToHost, st_[b]));
-        P_TRY(cudaEventRecord(ev_[b], st_[b]));
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaMemcpyAsync(h_ncands_[b].get(), d_ncands_.get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
+        CUDA_TRY(cudaMemcpyAsync(h_nhits_[b].get(), d_nhits_[b].get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
+        CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * sizeof(Hit), cudaMemcpyDeviceToHost, st_[b].get()));
+        CUDA_TRY(cudaEventRecord(ev_[b].get(), st_[b].get()));
         pending_[b] = true; end_[b] = first + count;
         return B200POST_OK;
     }
     // wait for chunk b and fold its hits in; *found set when some nonce has K2 hits
     int collect(int b, bool *found) {
         if (!pending_[b]) return B200POST_OK;
-        P_TRY(cudaEventSynchronize(ev_[b]));
+        CUDA_TRY(cudaEventSynchronize(ev_[b].get()));
         pending_[b] = false;
-        const uint32_t n = *h_nhits_[b];
-        if (n > hit_cap_ || *h_ncands_[b] > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
-        std::vector<Hit> v(h_hits_[b], h_hits_[b] + n);
+        const uint32_t n = *h_nhits_[b].get();
+        if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
+        std::vector<Hit> v(h_hits_[b].get(), h_hits_[b].get() + n);
         std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
         for (const Hit &h : v) {
             std::vector<uint64_t> &l = lists_[h.nonce];
@@ -237,15 +225,18 @@ private:
     int dev_ = -1;
     uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0;
     uint64_t lsb_ = 0, chunk_ = 0, scanned_ = 0;
-    uint8_t *d_rk_ = nullptr, *d_lazy_ = nullptr;
-    AesTables *d_tables_ = nullptr;
-    cudaStream_t st_[2] = {nullptr, nullptr};
-    cudaEvent_t ev_[2] = {nullptr, nullptr};
-    uint8_t *d_labels_[2] = {nullptr, nullptr}, *h_labels_[2] = {nullptr, nullptr};
-    Hit *d_hits_[2] = {nullptr, nullptr}, *h_hits_[2] = {nullptr, nullptr};
-    uint32_t *d_nhits_[2] = {nullptr, nullptr}, *h_nhits_[2] = {nullptr, nullptr}, *h_ncands_[2] = {nullptr, nullptr};
-    uint2 *d_cands_ = nullptr;
-    uint32_t *d_ncands_ = nullptr;
+    DeviceBuffer<uint8_t> d_rk_, d_lazy_;
+    DeviceBuffer<AesTables> d_tables_;
+    Stream st_[2];
+    Event ev_[2];
+    DeviceBuffer<uint8_t> d_labels_[2];
+    PinnedBuffer<uint8_t> h_labels_[2];
+    DeviceBuffer<Hit> d_hits_[2];
+    PinnedBuffer<Hit> h_hits_[2];
+    DeviceBuffer<uint32_t> d_nhits_[2];
+    PinnedBuffer<uint32_t> h_nhits_[2], h_ncands_[2];
+    DeviceBuffer<uint2> d_cands_;
+    DeviceBuffer<uint32_t> d_ncands_;
     uint32_t cand_cap_ = 0;
     bool pending_[2] = {false, false};
     uint64_t end_[2] = {0, 0};

@@ -12,28 +12,15 @@
 
 namespace b200post {
 
-#define RX_TRY(expr)                                                                                     \
-    do {                                                                                                 \
-        cudaError_t e__ = (expr);                                                                        \
-        if (e__ != cudaSuccess) {                                                                        \
-            set_error(std::string(#expr) + ": " + cudaGetErrorString(e__));                              \
-            cudaGetLastError();                                                                          \
-            return e__ == cudaErrorMemoryAllocation ? B200POST_ERR_OUT_OF_MEMORY : B200POST_ERR_CUDA;    \
-        }                                                                                                \
-    } while (0)
-
 RandomxEngine::RandomxEngine(int device) : dev_(device) {
     cudaGetDeviceProperties(&prop_, device);
 }
 
 RandomxEngine::~RandomxEngine() {
-    if (cudaSetDevice(dev_) != cudaSuccess) return;
-    if (stream_) cudaStreamSynchronize(stream_);
+    // the other members free themselves after this body, on this device and with no work of the engine in flight
+    cudaSetDevice(dev_);
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
     release_batch();
-    cudaFree(d_dataset_); cudaFree(d_inputs_); cudaFree(d_diff_); cudaFree(d_found_);
-    cudaFreeHost(h_stage_);
-    for (auto &e : ev_) if (e) cudaEventDestroy(e);
-    if (stream_) cudaStreamDestroy(stream_);
 }
 
 void RandomxEngine::release_batch() {
@@ -50,15 +37,15 @@ uint32_t RandomxEngine::desired_batch() const {
 }
 
 int RandomxEngine::ensure_dataset(const std::string &key) {
-    RX_TRY(cudaSetDevice(dev_));
-    if (!stream_) {
-        RX_TRY(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
-        for (auto &e : ev_) RX_TRY(cudaEventCreate(&e));
-        RX_TRY(cudaMalloc(&d_diff_, 32));
-        RX_TRY(cudaMalloc(&d_found_, 4));
+    CUDA_TRY(cudaSetDevice(dev_));
+    if (!stream_.get()) {
+        CUDA_TRY(stream_.create(cudaStreamNonBlocking));
+        for (Event &e : ev_) CUDA_TRY(e.create(cudaEventDefault));
+        CUDA_TRY(d_diff_.resize(32));
+        CUDA_TRY(d_found_.resize(1));
     }
-    if (!tables_) { RX_TRY(rx::upload_tables()); tables_ = true; }
-    if (d_dataset_ && key_ == key) return B200POST_OK;
+    if (!tables_) { CUDA_TRY(rx::upload_tables()); tables_ = true; }
+    if (d_dataset_.get() && key_ == key) return B200POST_OK;
     // host: Argon2d cache + the 8 SuperscalarHash programs (sequential by construction, ~0.7 s)
     rx::CacheImage img;
     rx::build_cache(key.data(), key.size(), img);
@@ -70,20 +57,18 @@ int RandomxEngine::ensure_dataset(const std::string &key) {
         flat.insert(flat.end(), img.programs[i].ops.begin(), img.programs[i].ops.end());
     }
     ss.first[rx::kCacheAccesses] = (uint32_t)flat.size();
-    uint64_t *d_cache = nullptr;
-    rx::SsOp *d_ops = nullptr;
+    DeviceBuffer<uint64_t> d_cache;
+    DeviceBuffer<rx::SsOp> d_ops;
     key_.clear();
-    if (!d_dataset_) RX_TRY(cudaMalloc(&d_dataset_, rx::kDatasetItems * 64));
-    RX_TRY(cudaMalloc(&d_cache, img.memory.size() * 8));
-    cudaError_t e = cudaMalloc(&d_ops, flat.size() * sizeof(rx::SsOp));
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_cache, img.memory.data(), img.memory.size() * 8, cudaMemcpyHostToDevice, stream_);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_ops, flat.data(), flat.size() * sizeof(rx::SsOp), cudaMemcpyHostToDevice, stream_);
-    ss.ops = d_ops;
-    if (e == cudaSuccess) e = rx::launch_dataset(d_cache, ss, d_dataset_, 0, rx::kDatasetItems, stream_);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(stream_);
-    cudaFree(d_cache); cudaFree(d_ops);
+    if (!d_dataset_.get()) CUDA_TRY(d_dataset_.resize(rx::kDatasetItems * 8));
+    CUDA_TRY(d_cache.resize(img.memory.size()));
+    CUDA_TRY(d_ops.resize(flat.size()));
+    CUDA_TRY(cudaMemcpyAsync(d_cache.get(), img.memory.data(), img.memory.size() * 8, cudaMemcpyHostToDevice, stream_.get()));
+    CUDA_TRY(cudaMemcpyAsync(d_ops.get(), flat.data(), flat.size() * sizeof(rx::SsOp), cudaMemcpyHostToDevice, stream_.get()));
+    ss.ops = d_ops.get();
+    CUDA_TRY(rx::launch_dataset(d_cache.get(), ss, d_dataset_.get(), 0, rx::kDatasetItems, stream_.get()));
     g_launches.fetch_add(1);
-    RX_TRY(e);
+    CUDA_TRY(cudaStreamSynchronize(stream_.get()));
     key_ = key;
     return B200POST_OK;
 }
@@ -91,12 +76,12 @@ int RandomxEngine::ensure_dataset(const std::string &key) {
 int RandomxEngine::ensure_batch(uint32_t want) {
     want = std::max<uint32_t>(32, (want + 31) / 32 * 32);
     if (want <= cap_) return B200POST_OK;
-    RX_TRY(cudaStreamSynchronize(stream_));
+    CUDA_TRY(cudaStreamSynchronize(stream_.get()));
     release_batch();
     // shrink until it fits next to whatever else lives on the device (the label engine's scratch, other datasets)
     for (uint32_t cap = want;; cap = std::max<uint32_t>(32, cap / 2 / 32 * 32)) {
         size_t free_b = 0, total_b = 0;
-        RX_TRY(cudaMemGetInfo(&free_b, &total_b));
+        CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
         const size_t per_vm = (size_t)rx::kScratchpadL3 + rx::kScratchpadL1 + 256 * 8 + rx::kRcpSlots * 8 + 64 + 256 + 32 + 1 + 32;
         if ((size_t)cap * per_vm + ((size_t)256 << 20) <= free_b) {
             rx::BatchBuffers b;
@@ -120,30 +105,26 @@ int RandomxEngine::ensure_batch(uint32_t want) {
     // (A persisting-L2 access-policy window over the hot plane was measured twice: 4 361 vs 4 370 H/s with the first
     // warp-per-VM kernel and 6 367 vs 6 377 H/s with the current one, no gain; the L2 set-aside also slowed the label
     // kernels of a following verify batch by a third.  Not used.)
-    if ((size_t)cap_ * 32 > stage_cap_) {
-        cudaFreeHost(h_stage_); h_stage_ = nullptr; stage_cap_ = 0;
-        RX_TRY(cudaMallocHost(&h_stage_, (size_t)cap_ * 32));
-        stage_cap_ = (size_t)cap_ * 32;
-    }
+    CUDA_TRY(h_stage_.grow((size_t)cap_ * 32));
     return B200POST_OK;
 }
 
 int RandomxEngine::run_chain(uint32_t n) {
     const int vm_mode = (int)options().rx_vm_mode.load();
-    RX_TRY(rx::launch_fill_scratchpads(buf_, n, stream_));
+    CUDA_TRY(rx::launch_fill_scratchpads(buf_, n, stream_.get()));
     for (int p = 0; p < rx::kProgramCount; p++) {
-        RX_TRY(rx::launch_program(buf_, n, p == 0, stream_));
-        RX_TRY(cudaEventRecord(ev_[2], stream_));
-        RX_TRY(rx::launch_execute(buf_, n, d_dataset_, vm_mode, stream_));
-        RX_TRY(cudaEventRecord(ev_[3], stream_));
-        if (p + 1 < rx::kProgramCount) RX_TRY(rx::launch_chain_seed(buf_, n, stream_));
+        CUDA_TRY(rx::launch_program(buf_, n, p == 0, stream_.get()));
+        CUDA_TRY(cudaEventRecord(ev_[2].get(), stream_.get()));
+        CUDA_TRY(rx::launch_execute(buf_, n, d_dataset_.get(), vm_mode, stream_.get()));
+        CUDA_TRY(cudaEventRecord(ev_[3].get(), stream_.get()));
+        if (p + 1 < rx::kProgramCount) CUDA_TRY(rx::launch_chain_seed(buf_, n, stream_.get()));
         // the VM kernel's own time: events bracket it on the launching stream; summed after the sync below
-        RX_TRY(cudaEventSynchronize(ev_[3]));
+        CUDA_TRY(cudaEventSynchronize(ev_[3].get()));
         float ms = 0;
-        RX_TRY(cudaEventElapsedTime(&ms, ev_[2], ev_[3]));
+        CUDA_TRY(cudaEventElapsedTime(&ms, ev_[2].get(), ev_[3].get()));
         vm_ms_ += ms; vm_launches_++;
     }
-    RX_TRY(rx::launch_finalize(buf_, n, stream_));
+    CUDA_TRY(rx::launch_finalize(buf_, n, stream_.get()));
     g_launches.fetch_add(1 + 8 * 2 + 7 + 2);
     return B200POST_OK;
 }
@@ -176,22 +157,22 @@ int RandomxEngine::hash_inputs(const std::string &key, const uint8_t *inputs, si
     rc = ensure_batch((uint32_t)std::min<size_t>(n, desired_batch()));
     if (rc != B200POST_OK) return rc;
     const size_t need_in = (size_t)cap_ * std::max<size_t>(input_len, 1);
-    if (need_in > inputs_cap_) { cudaFree(d_inputs_); d_inputs_ = nullptr; inputs_cap_ = 0; RX_TRY(cudaMalloc(&d_inputs_, need_in)); inputs_cap_ = need_in; }
+    CUDA_TRY(d_inputs_.grow(need_in));
     const uint32_t batch = std::min<uint32_t>(cap_, desired_batch());
     for (size_t off = 0; off < n; off += batch) {
         const uint32_t m = (uint32_t)std::min<size_t>(batch, n - off);
-        RX_TRY(cudaEventRecord(ev_[0], stream_));
-        if (input_len) RX_TRY(cudaMemcpyAsync(d_inputs_, inputs + off * input_len, (size_t)m * input_len, cudaMemcpyHostToDevice, stream_));
-        RX_TRY(rx::launch_seed_inputs(buf_, m, d_inputs_, (uint32_t)input_len, stream_));
+        CUDA_TRY(cudaEventRecord(ev_[0].get(), stream_.get()));
+        if (input_len) CUDA_TRY(cudaMemcpyAsync(d_inputs_.get(), inputs + off * input_len, (size_t)m * input_len, cudaMemcpyHostToDevice, stream_.get()));
+        CUDA_TRY(rx::launch_seed_inputs(buf_, m, d_inputs_.get(), (uint32_t)input_len, stream_.get()));
         rc = run_chain(m);
         if (rc != B200POST_OK) return rc;
-        RX_TRY(cudaMemcpyAsync(h_stage_, buf_.hashes, (size_t)m * 32, cudaMemcpyDeviceToHost, stream_));
-        RX_TRY(cudaEventRecord(ev_[1], stream_));
-        RX_TRY(cudaStreamSynchronize(stream_));
+        CUDA_TRY(cudaMemcpyAsync(h_stage_.get(), buf_.hashes, (size_t)m * 32, cudaMemcpyDeviceToHost, stream_.get()));
+        CUDA_TRY(cudaEventRecord(ev_[1].get(), stream_.get()));
+        CUDA_TRY(cudaStreamSynchronize(stream_.get()));
         float ms = 0;
-        RX_TRY(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
+        CUDA_TRY(cudaEventElapsedTime(&ms, ev_[0].get(), ev_[1].get()));
         total_ms_ += ms; hashes_ += m;
-        memcpy(out32 + off * 32, h_stage_, (size_t)m * 32);
+        memcpy(out32 + off * 32, h_stage_.get(), (size_t)m * 32);
     }
     return B200POST_OK;
 }
@@ -208,7 +189,7 @@ int RandomxEngine::k2pow(const std::string &key, const rx::K2powTemplate &tmpl, 
     if (count == 0) return B200POST_OK;
     rc = ensure_batch((uint32_t)std::min<uint64_t>(count, desired_batch()));
     if (rc != B200POST_OK) return rc;
-    if (difficulty) RX_TRY(cudaMemcpyAsync(d_diff_, difficulty, 32, cudaMemcpyHostToDevice, stream_));
+    if (difficulty) CUDA_TRY(cudaMemcpyAsync(d_diff_.get(), difficulty, 32, cudaMemcpyHostToDevice, stream_.get()));
     // batch_stride != 0: this device owns batches at start + k * batch_stride (interleaved multi-device search)
     const uint32_t batch = std::min<uint32_t>(cap_, desired_batch());   // cap_ may be left over from a larger setting
     const uint64_t step = batch_stride ? batch_stride : batch;
@@ -218,24 +199,24 @@ int RandomxEngine::k2pow(const std::string &key, const rx::K2powTemplate &tmpl, 
         const uint32_t m = (uint32_t)std::min<uint64_t>(batch, count - off);
         rx::K2powTemplate t = tmpl;
         t.start = start + off;
-        RX_TRY(cudaEventRecord(ev_[0], stream_));
-        RX_TRY(rx::launch_seed_k2pow(buf_, m, t, stream_));
+        CUDA_TRY(cudaEventRecord(ev_[0].get(), stream_.get()));
+        CUDA_TRY(rx::launch_seed_k2pow(buf_, m, t, stream_.get()));
         rc = run_chain(m);
         if (rc != B200POST_OK) return rc;
         uint32_t hit = 0xffffffffu;
         if (difficulty) {
-            RX_TRY(cudaMemsetAsync(d_found_, 0xff, 4, stream_));
-            RX_TRY(rx::launch_find_below(buf_, m, d_diff_, d_found_, stream_));
-            RX_TRY(cudaMemcpyAsync(&hit, d_found_, 4, cudaMemcpyDeviceToHost, stream_));
+            CUDA_TRY(cudaMemsetAsync(d_found_.get(), 0xff, 4, stream_.get()));
+            CUDA_TRY(rx::launch_find_below(buf_, m, d_diff_.get(), d_found_.get(), stream_.get()));
+            CUDA_TRY(cudaMemcpyAsync(&hit, d_found_.get(), 4, cudaMemcpyDeviceToHost, stream_.get()));
         }
-        if (hashes) RX_TRY(cudaMemcpyAsync(h_stage_, buf_.hashes, (size_t)m * 32, cudaMemcpyDeviceToHost, stream_));
-        RX_TRY(cudaEventRecord(ev_[1], stream_));
-        RX_TRY(cudaStreamSynchronize(stream_));
+        if (hashes) CUDA_TRY(cudaMemcpyAsync(h_stage_.get(), buf_.hashes, (size_t)m * 32, cudaMemcpyDeviceToHost, stream_.get()));
+        CUDA_TRY(cudaEventRecord(ev_[1].get(), stream_.get()));
+        CUDA_TRY(cudaStreamSynchronize(stream_.get()));
         float ms = 0;
-        RX_TRY(cudaEventElapsedTime(&ms, ev_[0], ev_[1]));
+        CUDA_TRY(cudaEventElapsedTime(&ms, ev_[0].get(), ev_[1].get()));
         total_ms_ += ms; hashes_ += m;
         if (done) *done += m;
-        if (hashes) memcpy(hashes + off * 32, h_stage_, (size_t)m * 32);
+        if (hashes) memcpy(hashes + off * 32, h_stage_.get(), (size_t)m * 32);
         if (difficulty && hit != 0xffffffffu) { if (found) *found = t.start + hit; break; }
     }
     return B200POST_OK;

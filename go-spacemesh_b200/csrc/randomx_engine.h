@@ -7,6 +7,7 @@
 #include <mutex>
 #include <string>
 
+#include "cuda_util.h"
 #include "randomx_kernels.cuh"
 
 namespace b200post {
@@ -37,17 +38,17 @@ private:
     int dev_;
     cudaDeviceProp prop_{};
     std::mutex mu_;
-    cudaStream_t stream_ = nullptr;
+    Stream stream_;
     bool tables_ = false;
     std::string key_;                       // key of the resident dataset ("" = none)
-    uint64_t *d_dataset_ = nullptr;
+    DeviceBuffer<uint64_t> d_dataset_;
     rx::BatchBuffers buf_;
     uint32_t cap_ = 0;
-    uint8_t *d_inputs_ = nullptr; size_t inputs_cap_ = 0;
-    uint8_t *d_diff_ = nullptr;
-    uint32_t *d_found_ = nullptr;
-    uint8_t *h_stage_ = nullptr; size_t stage_cap_ = 0;   // pinned: hashes coming back
-    cudaEvent_t ev_[4] = {nullptr, nullptr, nullptr, nullptr};
+    DeviceBuffer<uint8_t> d_inputs_;
+    DeviceBuffer<uint8_t> d_diff_;
+    DeviceBuffer<uint32_t> d_found_;
+    PinnedBuffer<uint8_t> h_stage_;   // hashes coming back
+    Event ev_[4];
     double total_ms_ = 0, vm_ms_ = 0;
     uint64_t hashes_ = 0, vm_launches_ = 0;
 };

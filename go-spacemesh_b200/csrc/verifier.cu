@@ -271,38 +271,31 @@ void parallel_for(size_t n, F fn) {
     for (auto &x : th) x.join();
 }
 
-#define V_TRY(expr)                                                                   \
-    do {                                                                              \
-        cudaError_t e__ = (expr);                                                     \
-        if (e__ != cudaSuccess) {                                                     \
-            set_error(std::string(#expr) + ": " + cudaGetErrorString(e__));           \
-            return e__ == cudaErrorMemoryAllocation ? B200POST_ERR_OUT_OF_MEMORY : B200POST_ERR_CUDA; \
-        }                                                                             \
-    } while (0)
-
 // Recompute the labels of all OK jobs with scrypt-N `n` (gather kernels, labels stay in HBM) and run the
 // device epilogue.  first_bad[k] = position of the first failing label of the k-th such job, or 0xffffffff.
 // grow-only device buffers of the judge stage, one set per provider: a batch costs no cudaMalloc/cudaFree once warm
 struct JudgeScratch {
     std::mutex mu;
-    uint4 *labels = nullptr; uint32_t *item_job = nullptr, *first_bad = nullptr; DevJob *jobs = nullptr; AesTables *tables = nullptr;
-    size_t cap_items = 0, cap_jobs = 0;
+    DeviceBuffer<uint4> labels;
+    DeviceBuffer<uint32_t> item_job, first_bad;
+    DeviceBuffer<DevJob> jobs;
+    DeviceBuffer<AesTables> tables;
     int reserve(size_t n_items, size_t n_jobs, const AesTables &host_tables) {
-        if (!tables) {
-            if (cudaMalloc(&tables, sizeof(AesTables)) != cudaSuccess) return B200POST_ERR_CUDA;
-            if (cudaMemcpy(tables, &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice) != cudaSuccess) return B200POST_ERR_CUDA;
+        if (!tables.get()) {
+            CUDA_TRY(tables.resize(1));
+            CUDA_TRY(cudaMemcpy(tables.get(), &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice));
         }
-        if (n_items > cap_items) {
-            cudaFree(labels); cudaFree(item_job); labels = nullptr; item_job = nullptr; cap_items = 0;
+        if (n_items > item_job.size()) {   // item_job is allocated last: its size is the capacity of both
+            item_job.reset();
             const size_t c = n_items + n_items / 4;
-            if (cudaMalloc(&labels, c * 16) != cudaSuccess || cudaMalloc(&item_job, c * 4) != cudaSuccess) return B200POST_ERR_OUT_OF_MEMORY;
-            cap_items = c;
+            CUDA_TRY(labels.resize(c));
+            CUDA_TRY(item_job.resize(c));
         }
-        if (n_jobs > cap_jobs) {
-            cudaFree(jobs); cudaFree(first_bad); jobs = nullptr; first_bad = nullptr; cap_jobs = 0;
+        if (n_jobs > first_bad.size()) {   // likewise first_bad
+            first_bad.reset();
             const size_t c = n_jobs + n_jobs / 4;
-            if (cudaMalloc(&jobs, c * sizeof(DevJob)) != cudaSuccess || cudaMalloc(&first_bad, c * 4) != cudaSuccess) return B200POST_ERR_OUT_OF_MEMORY;
-            cap_jobs = c;
+            CUDA_TRY(jobs.resize(c));
+            CUDA_TRY(first_bad.resize(c));
         }
         return B200POST_OK;
     }
@@ -346,21 +339,22 @@ int gather_and_judge(uint32_t provider, std::vector<Job *> &jobs, uint64_t n, co
     std::call_once(once, [] { aes_build_tables(host_tables); });
 
     const uint32_t n_items = (uint32_t)indices.size();
-    V_TRY(cudaSetDevice(e->device()));
+    CUDA_TRY(cudaSetDevice(e->device()));
     JudgeScratch &s = judge_scratch(provider);
     std::lock_guard<std::mutex> lk(s.mu);
     int rc = s.reserve(n_items, dj.size(), host_tables);
     if (rc != B200POST_OK) return rc;
-    V_TRY(cudaMemcpy(s.item_job, item_job.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice));
-    V_TRY(cudaMemcpy(s.jobs, dj.data(), dj.size() * sizeof(DevJob), cudaMemcpyHostToDevice));
-    V_TRY(cudaMemset(s.first_bad, 0xff, dj.size() * 4));
+    CUDA_TRY(cudaMemcpy(s.item_job.get(), item_job.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(s.jobs.get(), dj.data(), dj.size() * sizeof(DevJob), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemset(s.first_bad.get(), 0xff, dj.size() * 4));
     rc = e->labels_gather_indexed(indices.size(), dj.size(), commitments.data(), item_job.data(), indices.data(), n, nullptr,
-                                  reinterpret_cast<uint8_t *>(s.labels));
+                                  reinterpret_cast<uint8_t *>(s.labels.get()));
     if (rc != B200POST_OK) return rc;
-    verify_judge_kernel<<<(n_items + 255) / 256, 256, AES_SMEM_BYTES>>>(s.labels, s.item_job, s.jobs, n_items, s.tables, s.first_bad);
+    verify_judge_kernel<<<(n_items + 255) / 256, 256, AES_SMEM_BYTES>>>(s.labels.get(), s.item_job.get(), s.jobs.get(), n_items,
+                                                                        s.tables.get(), s.first_bad.get());
     g_launches += 1;
-    V_TRY(cudaGetLastError());
-    V_TRY(cudaMemcpy(first_bad.data(), s.first_bad, dj.size() * 4, cudaMemcpyDeviceToHost));
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpy(first_bad.data(), s.first_bad.get(), dj.size() * 4, cudaMemcpyDeviceToHost));
     return B200POST_OK;
 }
 

@@ -374,6 +374,39 @@ def test_back_to_back_batches_resume_the_pipeline(b2, orc):
         b2.set_option("speculate_next", 1)
 
 
+def test_speculation_across_scratch_reallocation_and_cta_size_change(b2, orc):
+    """A pre-filled first layer must not outlive the scratch it lives in: a raised max_scratch_mib makes the next
+    contiguous call reallocate, and a CTA-size change lands between two contiguous calls.  Every call equals the
+    oracle and the same plan run without speculation."""
+    c = hashlib.sha256(b"speculate-realloc").digest()
+    tpb = b2.get_option("tpb")
+    try:
+        b2.set_option("max_scratch_mib", 1)
+        wave = b2.wave_slots(2)
+        batch = 4 * wave + 123                         # >= 4 layers at the 1 MiB cap arms the speculation
+        diff = orc.py_vrf_difficulty(8 * batch)
+        plan = [(dict(max_scratch_mib=1), 700, batch), (dict(max_scratch_mib=4), 700 + batch, batch),
+                (dict(max_scratch_mib=1, tpb=512), 5, batch), (dict(tpb=256), 5 + batch, batch),
+                (dict(tpb=512), 5 + 2 * batch, batch)]
+        results = {}
+        for spec in (1, 0):
+            b2.set_option("speculate_next", spec)
+            out = []
+            for opts, start, count in plan:
+                for k, v in opts.items():
+                    b2.set_option(k, v)
+                out.append(b2.labels_range(c, 2, start, count, vrf_difficulty_=diff))
+            results[spec] = out
+        for (_, start, count), (g1, v1), (g0, v0) in zip(plan, results[1], results[0]):
+            exp, found, idx, l32 = orc.c_labels_range(c, 2, start, count, diff)
+            assert (g1 == exp).all() and (g0 == exp).all(), start
+            assert v1 == v0 == ((idx, l32) if found else None), start
+    finally:
+        b2.set_option("speculate_next", 1)
+        b2.set_option("max_scratch_mib", 0)
+        b2.set_option("tpb", tpb)
+
+
 def test_low_latency_kernel_equals_throughput_kernel_and_oracle(b2, orc, gpu_ready):
     """Small jobs take the low-latency ROMix kernel (labels spread over warps, label-major scratch): same bytes as the
     pipelined kernel and the oracle, at the sizes where the spreading changes shape (1, K2 = 37, one more than the
