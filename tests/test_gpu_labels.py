@@ -246,17 +246,22 @@ def test_cancel_flag(b2):
 
 
 def test_all_romix_variants_agree(b2, orc):
-    """Every memory-path variant / rotate mix of the ROMix kernel is the same function."""
+    """Every memory-path variant / rotate mix of the ROMix kernel is the same function over one single-layer job.
+    The low-latency kernel is switched off so that the pipelined variant runs (two launches: fill, then mix);
+    test_gpu_romix_matrix.py runs every compiled instance over several layers."""
     c = hashlib.sha256(b"variants").digest()
-    keep = {k: b2.get_option(k) for k in ("romix_variant", "rotate_mask", "tpb", "dr_unroll")}
+    keep = {k: b2.get_option(k) for k in ("romix_variant", "rotate_mask", "tpb", "dr_unroll", "lowlat_max_labels")}
     try:
+        b2.set_option("lowlat_max_labels", 0)
         ref = None
         for variant in (4, 0, 1, 2):
             for mw in (0, 1):
                 for tpb in ((64, 128, 256, 512) if variant == 4 else (128, 256)):
                     b2.set_option("romix_variant", variant); b2.set_option("rotate_mask", mw); b2.set_option("tpb", tpb)
                     b2.set_option("dr_unroll", 1 if (mw == 1 and variant == 4 and tpb == 64) else 4)
+                    b2.romix_time(reset=True)
                     got, _ = b2.labels_range(c, 512, 2**35, 777)
+                    assert b2.romix_time()[1] == (2 if variant == 4 else 1), (variant, mw, tpb)
                     if ref is None:
                         ref = got
                         assert (ref == orc.c_labels_range(c, 512, 2**35, 777)[0]).all()
@@ -303,9 +308,12 @@ def test_small_scratch_budget_still_correct(b2, orc):
 
 
 def test_largest_supported_n(b2, orc):
-    """N = 2^20 (128 MiB per scratchpad) is the documented cap; one label each way."""
+    """N = 2^20 (128 MiB per scratchpad) is the documented cap: two labels through the low-latency kernel (one launch).
+    test_gpu_romix_matrix.py runs the pipelined and classic kernels over several layers at this N."""
     c = hashlib.sha256(b"big-n").digest()
+    b2.romix_time(reset=True)
     got, _ = b2.labels_range(c, 1 << 20, 7, 2)
+    assert b2.romix_time()[1] == 1
     assert (got == orc.c_labels_range(c, 1 << 20, 7, 2, threads=2)[0]).all()
 
 
