@@ -190,7 +190,7 @@ public:
         CUDA_TRY(cudaMemcpyAsync(h_nhits_[b].get(), d_nhits_[b].get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
         CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * sizeof(Hit), cudaMemcpyDeviceToHost, st_[b].get()));
         CUDA_TRY(cudaEventRecord(ev_[b].get(), st_[b].get()));
-        pending_[b] = true; end_[b] = first + count;
+        pending_[b] = true; count_[b] = count;
         return B200POST_OK;
     }
     // wait for chunk b and fold its hits in; *found set when some nonce has K2 hits
@@ -206,7 +206,7 @@ public:
             std::vector<uint64_t> &l = lists_[h.nonce];
             if (l.size() < k2_) l.push_back(h.index);
         }
-        scanned_ = std::max(scanned_, end_[b]);
+        scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
         for (auto &kv : lists_) if (kv.second.size() >= k2_) *found = true;
         return B200POST_OK;
     }
@@ -239,7 +239,7 @@ private:
     DeviceBuffer<uint32_t> d_ncands_;
     uint32_t cand_cap_ = 0;
     bool pending_[2] = {false, false};
-    uint64_t end_[2] = {0, 0};
+    uint32_t count_[2] = {0, 0};
     std::map<uint32_t, std::vector<uint64_t>> lists_;   // ordered: ties resolve to the lower nonce
 };
 

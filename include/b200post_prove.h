@@ -51,7 +51,9 @@ typedef struct b200post_proof_out {    /* types.Post / shared.Proof */
     uint64_t pow;
     size_t indices_len;
     uint8_t indices[800];              /* wire cap, activation/wire/wire_v1.go:43                               */
-    uint64_t labels_scanned;           /* how far the scan had to go                                            */
+    uint64_t labels_scanned;           /* labels streamed from the first index, in whole chunks (not an absolute
+                                          index): last proof index - first index < labels_scanned <= labels
+                                          offered (count, or num_labels for b200post_generate_proof)           */
 } b200post_proof_out;
 
 /* Proof over the POST data in `data_dir` (postdata_N.bin + postdata_metadata.json written by a setup session).

@@ -476,3 +476,44 @@ def py_prove_multi(labels: np.ndarray, challenge: bytes, nonces: int, pows, k1: 
         if len(hits) == k2 and (best is None or hits[-1] < best[1][-1]):
             best = (nonce, hits)
     return best if best else (None, None)
+
+
+def _np_aes128_ecb(key: bytes, blocks: np.ndarray) -> np.ndarray:
+    from cryptography.hazmat.primitives.ciphers import Cipher, algorithms, modes
+    enc = Cipher(algorithms.AES(key), modes.ECB()).encryptor()
+    return np.frombuffer(enc.update(blocks.tobytes()) + enc.finalize(), dtype=np.uint8).reshape(-1, 16)
+
+
+def np_prove_hits(labels: np.ndarray, challenge: bytes, nonces: int, pows, k1: int, k2: int, num_labels: int):
+    """{nonce: the first (up to) k2 positions in `labels` (uint8[n,16]) that pass py_label_passes, ascending},
+    array-at-a-time: one AES-128-ECB call per nonce group over all labels, and one per nonce over the labels whose
+    byte equals the difficulty MSB (the nonce's lazy cipher then compares its low 56 bits, little-endian)."""
+    labels = np.ascontiguousarray(labels, dtype=np.uint8).reshape(-1, 16)
+    diff = py_proving_difficulty(k1, num_labels)
+    msb, lsb = diff >> 56, diff & ((1 << 56) - 1)
+    out = {}
+    for g in range(nonces // 16):
+        ct = _np_aes128_ecb(py_cipher_key(challenge, g, int(pows[g])), labels)
+        rows, cols = np.nonzero(ct <= msb)                  # row-major: ascending label position
+        keep = ct[rows, cols] != msb
+        for b in np.unique(cols[~keep]):
+            sel = np.flatnonzero((cols == b) & ~keep)
+            lz = _np_aes128_ecb(py_cipher_key(challenge, g, int(pows[g]), 16 * g + int(b)), labels[rows[sel]])
+            low56 = lz[:, :8].copy().view("<u8")[:, 0] & np.uint64((1 << 56) - 1)
+            keep[sel[low56 < np.uint64(lsb)]] = True
+        rows, cols = rows[keep], cols[keep]
+        for b in range(16):
+            out[16 * g + b] = rows[cols == b][:k2]
+    return out
+
+
+def np_prove_multi(labels: np.ndarray, challenge: bytes, nonces: int, pows, k1: int, k2: int, num_labels: int,
+                   first_index: int = 0):
+    """py_prove_multi, vectorised, for labels holding indices first_index .. first_index + n - 1: the same
+    selection rule (lowest K2-th hit index wins, ties to the lower nonce).  Returns (nonce, [global indices]) or
+    (None, None)."""
+    best = None
+    for nonce, hits in np_prove_hits(labels, challenge, nonces, pows, k1, k2, num_labels).items():   # ascending nonce
+        if len(hits) == k2 and (best is None or hits[-1] < best[1][-1]):
+            best = (nonce, hits)
+    return (best[0], [first_index + int(i) for i in best[1]]) if best else (None, None)

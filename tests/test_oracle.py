@@ -179,6 +179,36 @@ def test_bad_parameters_rejected(orc):
     assert labels.shape == (0, 16) and not found
 
 
+# (labels, nonces, k1, num_labels, k2, first_index, proof expected): difficulty MSB noted per row
+PROVE_REGIMES = {
+    "msb0-lsb":    (400, 64, 4000, 1 << 20, 2, 0, True),           # 0x00, lsb != 0: every hit is a lazy-cipher hit
+    "round":       (300, 16, 1 << 15, 1 << 20, 4, 0, True),        # 0x08, lsb == 0: a byte equal to the MSB never passes
+    "mid-lsb":     (300, 32, 100003, 1 << 20, 6, 0, True),         # 0x18, lsb != 0
+    "saturated":   (64, 16, 300, 300, 5, 0, True),                 # 0xff: k1 >= num_labels
+    "no-proof":    (300, 16, 4000, 1 << 20, 10, 0, False),
+    "k2-1-ties":   (40, 256, 1 << 19, 1 << 20, 1, 0, True),        # 0x80: ~128 nonces tie at the first label
+    "first-index": (600, 64, 2**32 - 1, 1 << 41, 2, 2**40 + 3, True),   # 0x00, lsb != 0, 42-bit indices
+}
+
+
+@pytest.mark.parametrize("regime", PROVE_REGIMES)
+def test_vectorised_prove_oracle_matches_scalar(orc, regime):
+    """np_prove_multi (the GPU prove tests' oracle) is the scalar py_prove_multi: same winner, same indices, at every
+    difficulty regime, ties and an offset first index included."""
+    count, nonces, k1, num_labels, k2, first, found = PROVE_REGIMES[regime]
+    rng = np.random.default_rng(sorted(PROVE_REGIMES).index(regime) + 100)
+    labels = rng.integers(0, 256, (count, 16), dtype=np.uint8)
+    challenge = bytes(rng.integers(0, 256, 32, dtype=np.uint8))
+    pows = [int(p) for p in rng.integers(0, 2**56, nonces // 16)]
+    exp_nonce, exp_hits = orc.py_prove_multi(labels, challenge, nonces, pows, k1, k2, num_labels)
+    assert (exp_nonce is not None) == found
+    want = (exp_nonce, None if exp_hits is None else [first + i for i in exp_hits])
+    assert orc.np_prove_multi(labels, challenge, nonces, pows, k1, k2, num_labels, first_index=first) == want
+    if regime == "k2-1-ties":
+        hits = orc.np_prove_hits(labels, challenge, nonces, pows, k1, k2, num_labels)
+        assert exp_hits == [0] and sum(1 for h in hits.values() if list(h) == [0]) > 1
+
+
 def test_simd_and_scalar_romix_agree(orc):
     """The vectorised ROMix paths used for the timed CPU baseline (1 = SSE2, 2 = AVX2 with two labels per thread in
     lock-step, 3 = AVX-512 with four, where the CPU has it) are the same function as the scalar restatement, ragged
