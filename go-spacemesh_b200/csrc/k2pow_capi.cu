@@ -8,6 +8,7 @@
 
 #include "../../include/b200post_k2pow.h"
 #include "engine.h"
+#include "proof_common.h"
 #include "randomx_engine.h"
 
 using namespace b200post;
@@ -41,14 +42,8 @@ bool clamp_range(uint64_t start, uint64_t &count) {
 extern "C" {
 
 void b200post_k2pow_scale_difficulty(const uint8_t pow_difficulty[32], uint32_t num_units, uint8_t out[32]) {
-    // 256-bit big-endian long division by a 32-bit divisor
-    const uint64_t d = num_units ? num_units : 1;
-    uint64_t rem = 0;
-    for (int i = 0; i < 32; i++) {
-        const uint64_t cur = (rem << 8) | pow_difficulty[i];
-        out[i] = (uint8_t)(cur / d);
-        rem = cur % d;
-    }
+    // the prover and the verifier scale with the same division
+    div256_u32(pow_difficulty, num_units ? num_units : 1, out);
 }
 
 int b200post_randomx_prepare(uint32_t provider, const uint8_t *key, size_t key_len) {
@@ -63,6 +58,17 @@ int b200post_randomx_hash(uint32_t provider, const uint8_t *key, size_t key_len,
     RandomxEngine *e = randomx_engine_for(provider);
     if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
     return e->hash_inputs(key_of(key, key_len), inputs, input_len, n, out32);
+}
+
+int b200post_randomx_dataset_read(uint32_t provider, const uint8_t *key, size_t key_len, uint64_t first_item, uint64_t count,
+                                  uint64_t *out) {
+    if ((count && !out) || first_item > rx::kDatasetItems || count > rx::kDatasetItems - first_item) {
+        set_error("invalid argument: items past the end of the dataset, or no output buffer");
+        return B200POST_ERR_INVALID_ARGUMENT;
+    }
+    RandomxEngine *e = randomx_engine_for(provider);
+    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    return e->dataset_read(key_of(key, key_len), first_item, count, out);
 }
 
 int b200post_k2pow_hashes(uint32_t provider, const b200post_k2pow_params *p, uint64_t start, uint64_t count, uint8_t *out32) {

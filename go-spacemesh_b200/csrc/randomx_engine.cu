@@ -140,6 +140,15 @@ int RandomxEngine::batch_size(uint64_t *vms) {
     return B200POST_OK;
 }
 
+int RandomxEngine::dataset_read(const std::string &key, uint64_t first_item, uint64_t count, uint64_t *out) {
+    std::lock_guard<std::mutex> lk(mu_);
+    const int rc = ensure_dataset(key);
+    if (rc != B200POST_OK || count == 0) return rc;
+    CUDA_TRY(cudaMemcpyAsync(out, d_dataset_.get() + first_item * 8, count * 64, cudaMemcpyDeviceToHost, stream_.get()));
+    CUDA_TRY(cudaStreamSynchronize(stream_.get()));
+    return B200POST_OK;
+}
+
 void RandomxEngine::last_timing(double *total_ms, double *vm_ms, uint64_t *hashes, uint64_t *vm_launches) {
     std::lock_guard<std::mutex> lk(mu_);
     if (total_ms) *total_ms = total_ms_;

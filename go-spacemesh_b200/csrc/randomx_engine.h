@@ -25,6 +25,8 @@ public:
               uint8_t *hashes, uint64_t *found, uint64_t *done, const volatile int *cancel, uint64_t batch_stride = 0,
               const volatile int *peer_hit = nullptr);
     int batch_size(uint64_t *vms);
+    // dataset items [first_item, first_item + count) of `key` to host memory (64 bytes each; the range is checked by the caller)
+    int dataset_read(const std::string &key, uint64_t first_item, uint64_t count, uint64_t *out);
     void last_timing(double *total_ms, double *vm_ms, uint64_t *hashes, uint64_t *vm_launches);
 
 private:

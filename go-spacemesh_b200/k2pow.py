@@ -34,7 +34,9 @@ def _bind():
         L.b200post_k2pow_search.argtypes = [u32, ctypes.POINTER(_Params), u64, u64, ctypes.POINTER(u64), ctypes.POINTER(u64), vp]
         L.b200post_k2pow_search_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u64, u64,
                                                   ctypes.POINTER(u64), ctypes.POINTER(u64), vp]
+        L.b200post_k2pow_search_groups.argtypes = [u32, ctypes.POINTER(_Params), u32, u64, vp, ctypes.POINTER(u64), vp]
         L.b200post_k2pow_verify.argtypes = [u32, ctypes.POINTER(_Params), u64, ctypes.POINTER(ctypes.c_int)]
+        L.b200post_randomx_dataset_read.argtypes = [u32, ctypes.c_char_p, sz, u64, u64, vp]
         L.b200post_randomx_last_timing.argtypes = [u32, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
                                                    ctypes.POINTER(u64), ctypes.POINTER(u64)]
         L.b200post_randomx_batch_size.argtypes = [u32, ctypes.POINTER(u64)]
@@ -95,6 +97,26 @@ def search(nonce_group: int, challenge8: bytes, node_id: bytes, difficulty: byte
     else:
         _check(_bind().b200post_k2pow_search(provider, ctypes.byref(p), start, count, ctypes.byref(found), ctypes.byref(done), cptr))
     return (None if found.value == NOT_FOUND else found.value), done.value
+
+
+def search_groups(challenge8: bytes, node_id: bytes, difficulty: bytes, n_groups: int, max_nonces_per_group: int = 0, *,
+                  key: bytes | None = None, provider: int = 0):
+    """The prover's search: the smallest valid pow of each nonce group 0..n_groups-1 (None where there is none below
+    max_nonces_per_group; 0 = the whole nonce space).  -> (pows, hashes computed)."""
+    p = _params(0, challenge8, node_id, difficulty, key)
+    pows = np.zeros(n_groups, dtype=np.uint64)
+    done = ctypes.c_uint64(0)
+    _check(_bind().b200post_k2pow_search_groups(provider, ctypes.byref(p), n_groups, max_nonces_per_group, pows.ctypes.data,
+                                                ctypes.byref(done), None))
+    return [None if int(v) == NOT_FOUND else int(v) for v in pows], done.value
+
+
+def dataset(first: int, count: int, key: bytes | None = None, *, provider: int = 0) -> np.ndarray:
+    """RandomX dataset items first..first+count-1 of `key` as resident on the device: (count, 8) uint64."""
+    out = np.zeros((count, 8), dtype=np.uint64)
+    _check(_bind().b200post_randomx_dataset_read(provider, key, len(key) if key is not None else 0, first, count,
+                                                 out.ctypes.data))
+    return out
 
 
 def verify(pow_: int, nonce_group: int, challenge8: bytes, node_id: bytes, difficulty: bytes, *, key: bytes | None = None,

@@ -56,6 +56,11 @@ int b200post_randomx_prepare(uint32_t provider, const uint8_t *key, size_t key_l
 int b200post_randomx_hash(uint32_t provider, const uint8_t *key, size_t key_len, const uint8_t *inputs, size_t input_len,
                           size_t n, uint8_t *out32);
 
+/* Dataset items [first_item, first_item+count) of `key` on `provider` (out = count x 8 uint64, HOST), building the
+ * dataset first if it is not resident.  A range past the 34 078 719 items is INVALID_ARGUMENT.  Diagnostics / tests. */
+int b200post_randomx_dataset_read(uint32_t provider, const uint8_t *key, size_t key_len, uint64_t first_item, uint64_t count,
+                                  uint64_t *out);
+
 /* k2pow hashes of pow = start .. start+count-1 (out32 = count x 32 bytes, HOST).  Diagnostics / tests. */
 int b200post_k2pow_hashes(uint32_t provider, const b200post_k2pow_params *p, uint64_t start, uint64_t count, uint8_t *out32);
 

@@ -20,6 +20,8 @@ _lib = None
 
 # post-rs pow/randomx.rs (recollection, "parity unpinned"): the RandomX cache key of spacemesh's k2pow
 K2POW_CACHE_KEY = b"spacemesh-randomx-cache-key"
+# RandomX dataset: (2 GiB base + 32 MiB - 64 B extra) / 64-byte items
+DATASET_ITEMS = (2**31 + 33554368) // 64
 
 
 class SsInstr(ctypes.Structure):
@@ -59,6 +61,8 @@ def lib() -> ctypes.CDLL:
         L.rxo_dataset_item.argtypes = [vp, u64, vp]
         L.rxo_dataset_init.argtypes = [vp, ctypes.c_int]
         L.rxo_has_dataset.argtypes = [vp]
+        L.rxo_dataset_memory.restype = ctypes.POINTER(ctypes.c_uint64)
+        L.rxo_dataset_memory.argtypes = [vp]
         L.rxo_hash.argtypes = [vp, ctypes.c_char_p, sz, vp]
         L.rxo_vm_new.restype = vp
         L.rxo_vm_free.argtypes = [vp]
@@ -129,6 +133,13 @@ class Cache:
     def init_dataset(self, threads: int | None = None):
         if lib().rxo_dataset_init(self._h, threads or default_threads()) != 0:
             raise MemoryError("dataset allocation failed")
+
+    def dataset(self) -> np.ndarray:
+        """The fast-mode dataset as a (DATASET_ITEMS, 8) uint64 view (owned by the cache); init_dataset() first."""
+        p = lib().rxo_dataset_memory(self._h)
+        if not p:
+            raise ValueError("no dataset: call init_dataset() first")
+        return np.ctypeslib.as_array(p, shape=(DATASET_ITEMS, 8))
 
     def hash(self, data: bytes, trace: bool = False):
         o = ctypes.create_string_buffer(32)

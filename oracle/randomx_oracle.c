@@ -636,6 +636,7 @@ int rxo_dataset_init(rxo_cache *c, int threads) {
     return 0;
 }
 int rxo_has_dataset(const rxo_cache *c) { return c->dataset != NULL; }
+const uint8_t *rxo_dataset_memory(const rxo_cache *c) { return c->dataset; }
 
 /* ------------------------------------------------------------------------------------------------ */
 /* The virtual machine (spec §4, §5)                                                                  */

@@ -39,6 +39,8 @@ const rxo_ss_program *rxo_cache_programs(const rxo_cache *c);
 void rxo_dataset_item(const rxo_cache *c, uint64_t item, uint64_t out[8]);
 int rxo_dataset_init(rxo_cache *c, int threads);
 int rxo_has_dataset(const rxo_cache *c);
+/* the fast-mode dataset (34 078 719 items x 64 bytes, after rxo_dataset_init), or NULL if there is none */
+const uint8_t *rxo_dataset_memory(const rxo_cache *c);
 
 /* the hash */
 rxo_vm *rxo_vm_new(void);

@@ -84,13 +84,31 @@ def test_k2pow_api_without_a_device(b2):
     assert k2.scale_difficulty(d, 1) == d
     assert int.from_bytes(k2.scale_difficulty(d, 4), "big") == int.from_bytes(d, "big") // 4
     assert int.from_bytes(k2.scale_difficulty(b"\xff" * 32, 3), "big") == (2**256 - 1) // 3
+    assert k2.scale_difficulty(d, 0) == d                              # num_units 0 counts as 1
+    from oracle import pyrandomx as orx
+    for first, count in ((orx.DATASET_ITEMS - 1, 2), (orx.DATASET_ITEMS + 1, 0), (2**64 - 1, 2)):
+        with pytest.raises(b2.B200PostError) as e:                     # checked before any device is looked for
+            k2.dataset(first, count)
+        assert e.value.code == b2.ERR_INVALID_ARGUMENT
     if b2.providers():
         pytest.skip("a CUDA device is present: the no-device contract is covered on CPU-only boxes")
     for call in (lambda: k2.prepare(), lambda: k2.hashes(0, bytes(8), bytes(32), 0, 1), lambda: k2.search(0, bytes(8), bytes(32), b"\xff" * 32, 0, 1),
-                 lambda: k2.verify(0, 0, bytes(8), bytes(32), b"\xff" * 32), lambda: k2.randomx_hash(b"k", [b"x"])):
+                 lambda: k2.verify(0, 0, bytes(8), bytes(32), b"\xff" * 32), lambda: k2.randomx_hash(b"k", [b"x"]),
+                 lambda: k2.dataset(0, 1), lambda: k2.search_groups(bytes(8), bytes(32), b"\xff" * 32, 2)):
         with pytest.raises(b2.B200PostError) as e:
             call()
         assert e.value.code == b2.ERR_NO_DEVICE
     with pytest.raises(b2.B200PostError) as e:
         k2.prepare(provider=b2.CPU_PROVIDER_ID)
     assert e.value.code == b2.ERR_UNSUPPORTED
+
+
+def test_scale_difficulty_is_exact_integer_division(b2):
+    """The one division the prover, the verifier and the export share: floor(difficulty / num_units) over 256 bits."""
+    k2 = importlib.import_module("go-spacemesh_b200.k2pow")
+    rng = np.random.default_rng(31)
+    values = [0, 1, 2**256 - 1, 2**255, 2**224 - 1] + [int.from_bytes(bytes(rng.integers(0, 256, 32, dtype=np.uint8)), "big")
+                                                      for _ in range(40)]
+    for v in values:
+        for units in (1, 2, 3, 4, 7, 255, 256, 65537, 2**31 - 1, 2**32 - 1):
+            assert int.from_bytes(k2.scale_difficulty(v.to_bytes(32, "big"), units), "big") == v // units, (hex(v), units)
