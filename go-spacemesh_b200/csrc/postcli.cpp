@@ -11,6 +11,13 @@
 //   b200postcli -verify -datadir /data [-fraction 0.2] [-fromFile 0] [-toFile N] [-seed S] [-provider 0|all]
 // recomputes `-fraction` percent of each file's labels on the GPU, prints `file N offset K (label I)` for each
 // reported mismatch and exits 0 when the data is valid, 1 otherwise.
+//
+// One POST initialised on several machines (postcli's flag names as recalled, unpinned):
+//   b200postcli <init flags> -fromFile A -toFile B      writes only postdata_A.bin .. postdata_B.bin
+//   b200postcli -printNumFiles -numUnits N -labelsPerUnit L [-maxFileSize S]   how many files the POST has
+//   b200postcli -searchForNonce -datadir D [-provider 0|all] [-computeBatchSize B]
+// The last one finds the VRF nonce of the merged files from their stored labels and writes it to the metadata.
+// Exit codes: 0 ok, 1 error or damaged data, 2 usage, 130 stopped.
 #include <signal.h>
 
 #include <chrono>
@@ -89,10 +96,44 @@ static int run_verify(const std::string &datadir, const std::string &provider, d
     return 1;
 }
 
+static int run_search(const std::string &datadir, const std::string &provider, uint64_t batch) {
+    b200post_vrf_search_opts o;
+    b200post_default_vrf_search_opts(&o);
+    o.provider_id = provider == "all" ? B200POST_PROVIDER_ALL : (int64_t)strtoull(provider.c_str(), nullptr, 10);
+    if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) { fprintf(stderr, "provider 4294967295 (CPU) is not served: this build has no CPU path\n"); return 2; }
+    o.compute_batch_size = batch;
+    uint64_t total = 0;
+    b200post_post_metadata md;
+    if (b200post_load_metadata(datadir.c_str(), &md) == 0) total = (uint64_t)md.num_units * md.labels_per_unit;
+    volatile uint64_t progress = 0;
+    o.progress = &progress;
+    signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
+    volatile int done = 0;
+    std::thread show([&] {
+        const auto t0 = std::chrono::steady_clock::now();
+        while (!done) {
+            for (int k = 0; k < 20 && !done; k++) std::this_thread::sleep_for(std::chrono::milliseconds(100));
+            const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+            const uint64_t p = progress;
+            fprintf(stderr, "\r%llu / %llu stored labels scanned (%.1f %%), %.0f labels/s   ", (unsigned long long)p, (unsigned long long)total,
+                    total ? 100.0 * p / (double)total : 0.0, el > 0 ? p / el : 0.0);
+        }
+        fprintf(stderr, "\n");
+    });
+    b200post_vrf_nonce nn;
+    const int rc = b200post_search_vrf_nonce(datadir.c_str(), &o, &nn, &g_cancel);
+    done = 1;
+    show.join();
+    if (rc == B200POST_ERR_CANCELLED) { fprintf(stderr, "stopped; run again to finish the search\n"); return 130; }
+    if (rc) { fprintf(stderr, "search failed: %s (%d)\n", b200post_last_error(), rc); return 1; }
+    printf("VRF nonce %llu\n", (unsigned long long)nn.index);
+    return 0;
+}
+
 int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
-    bool print_providers = false, verify = false;
+    bool print_providers = false, verify = false, print_num_files = false, search = false, range = false;
     double fraction = 0.2;
     uint64_t from_file = 0, seed = 0;
     int64_t to_file = -1;
@@ -115,8 +156,10 @@ int main(int argc, char **argv) {
         else if (a == "yes") {}
         else if (a == "verify") verify = true;
         else if (a == "fraction") fraction = strtod(val().c_str(), nullptr);
-        else if (a == "fromFile") from_file = strtoull(val().c_str(), nullptr, 10);
-        else if (a == "toFile") to_file = strtoll(val().c_str(), nullptr, 10);
+        else if (a == "fromFile") { from_file = strtoull(val().c_str(), nullptr, 10); range = true; }
+        else if (a == "toFile") { to_file = strtoll(val().c_str(), nullptr, 10); range = true; }
+        else if (a == "printNumFiles") print_num_files = true;
+        else if (a == "searchForNonce") search = true;
         else if (a == "seed") seed = strtoull(val().c_str(), nullptr, 10);
         else { fprintf(stderr, "unknown flag -%s\n", a.c_str()); return 2; }
     }
@@ -126,7 +169,15 @@ int main(int argc, char **argv) {
         for (int k = 0; k < n && k < 16; k++) printf("{ID: %u, Model: \"%s\", DeviceType: GPU, HBM: %llu}\n", p[k].id, p[k].model, (unsigned long long)p[k].hbm_bytes);
         return 0;
     }
+    if (print_num_files) {
+        const unsigned __int128 nl = (unsigned __int128)num_units * (labels_per_unit ? labels_per_unit : 512);
+        if (nl == 0 || max_file_size < 16 || max_file_size % 16) { fprintf(stderr, "-numUnits, -labelsPerUnit and -maxFileSize (a multiple of 16) must be positive\n"); return 2; }
+        const unsigned __int128 per_file = max_file_size / 16;
+        printf("%llu\n", (unsigned long long)((nl + per_file - 1) / per_file));
+        return 0;
+    }
     if (verify) return run_verify(datadir, provider, fraction, from_file, to_file, seed);
+    if (search) return run_search(datadir, provider, batch);
     uint8_t node_id[32], atx_id[32];
     if (!unhex32(id, node_id) || !unhex32(atx, atx_id)) { fprintf(stderr, "-id and -commitmentAtxId must be 32-byte hex strings\n"); return 2; }
     b200post_post_config cfg;
@@ -143,9 +194,13 @@ int main(int argc, char **argv) {
 
     b200post_setup_manager *mgr = nullptr;
     if (b200post_setup_manager_new(&cfg, &mgr)) { fprintf(stderr, "error: %s\n", b200post_last_error()); return 1; }
-    if (int rc = b200post_setup_prepare_initializer(mgr, &o, node_id, atx_id)) { fprintf(stderr, "prepare: %s (%d)\n", b200post_last_error(), rc); return 1; }
+    if (int rc = b200post_setup_prepare_files(mgr, &o, node_id, atx_id, from_file, to_file)) {
+        fprintf(stderr, "prepare: %s (%d)\n", b200post_last_error(), rc);
+        return range && rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;   // a file range outside the POST is a usage error
+    }
     signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
-    const uint64_t total = (uint64_t)o.num_units * cfg.labels_per_unit;
+    const uint64_t per_file = o.max_file_size / 16, all = (uint64_t)o.num_units * cfg.labels_per_unit;
+    const uint64_t total = range ? std::min<uint64_t>(to_file < 0 ? all : (uint64_t)(to_file + 1) * per_file, all) - from_file * per_file : all;
     std::thread progress([&] {
         const auto t0 = std::chrono::steady_clock::now();
         b200post_setup_status st;
@@ -165,7 +220,12 @@ int main(int argc, char **argv) {
     if (rc == B200POST_ERR_CANCELLED) { fprintf(stderr, "stopped; run again to resume\n"); return 130; }
     if (rc) { fprintf(stderr, "init failed: %s (%d)\n", b200post_last_error(), rc); return 1; }
     b200post_post_metadata md;
-    if (b200post_load_metadata(datadir.c_str(), &md) == 0 && md.has_nonce) printf("initialization complete; VRF nonce %llu\n", (unsigned long long)md.nonce);
+    if (b200post_load_metadata(datadir.c_str(), &md) == 0) {
+        if (md.vrf_scan_pending)
+            printf("files %llu..%llu complete; copy every range's files and one metadata file into one directory, then search the VRF nonce "
+                   "with -searchForNonce\n", (unsigned long long)from_file, (unsigned long long)(from_file + (total + per_file - 1) / per_file - 1));
+        else if (md.has_nonce) printf("initialization complete; VRF nonce %llu\n", (unsigned long long)md.nonce);
+    }
     b200post_setup_manager_free(mgr);
     return 0;
 }

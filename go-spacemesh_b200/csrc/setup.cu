@@ -21,6 +21,7 @@
 #include "engine.h"
 #include "host_hash.h"
 #include "metrics.h"
+#include "setup_internal.h"
 
 using namespace b200post;
 
@@ -127,6 +128,7 @@ int save_metadata(const std::string &dir, const b200post_post_metadata &m) {
     j += " \"Nonce\": " + (m.has_nonce ? std::to_string(m.nonce) : std::string("null")) + ",\n";
     j += " \"NonceValue\": " + (m.has_nonce ? "\"" + hex(m.nonce_value, 32) + "\"" : std::string("null")) + ",\n";
     j += " \"LastPosition\": " + std::to_string(m.last_position) + ",\n";
+    if (m.vrf_scan_pending) j += " \"VrfScanPending\": true,\n";   // absent otherwise: such a file reads as before
     j += " \"Scrypt\": {\"N\": " + std::to_string(m.scrypt_n) + ", \"R\": " + std::to_string(m.scrypt_r) + ", \"P\": " + std::to_string(m.scrypt_p) + "}\n}\n";
     const std::string tmp = path_join(dir, std::string(kMetaFile) + ".tmp"), fin = path_join(dir, kMetaFile);
     FILE *f = fopen(tmp.c_str(), "w");
@@ -164,10 +166,46 @@ int load_metadata(const std::string &dir, b200post_post_metadata *m, bool *missi
     if (json_u64(doc, "R", &v)) m->scrypt_r = v;
     if (json_u64(doc, "P", &v)) m->scrypt_p = v;
     if (json_u64(doc, "Nonce", &v) && json_raw(doc, "NonceValue", &s) && unhex(s, m->nonce_value, 32)) { m->has_nonce = 1; m->nonce = v; }
+    m->vrf_scan_pending = json_raw(doc, "VrfScanPending", &s) && s == "true";
     return B200POST_OK;
 }
 
 }  // namespace
+
+namespace b200post {
+
+int save_post_metadata(const std::string &dir, const b200post_post_metadata &m) { return save_metadata(dir, m); }
+
+int compute_labels(int64_t provider_id, uint64_t N, const uint8_t commitment[32], uint64_t start, uint64_t count, uint8_t *out,
+                   const uint8_t *diff, b200post_vrf_nonce *nonce, const volatile int *cancel) {
+    if (nonce) memset(nonce, 0, sizeof *nonce);
+    if (provider_id == B200POST_PROVIDER_ALL) {
+        const int n = device_count();
+        if (n == 0) { set_error("no CUDA device available"); return B200POST_ERR_NO_DEVICE; }
+        std::vector<uint32_t> ids((size_t)n);
+        for (int i = 0; i < n; i++) ids[(size_t)i] = (uint32_t)i;
+        return b200post_labels_range_multi(ids.data(), n, commitment, N, start, count, out, diff, diff ? nonce : nullptr, cancel);
+    }
+    return b200post_labels_range((uint32_t)provider_id, commitment, N, start, count, out, diff, diff ? nonce : nullptr, cancel);
+}
+
+int search_past_end(const std::string &dir, b200post_post_metadata *md, uint64_t num_labels, int64_t provider_id, uint64_t batch,
+                    const uint8_t commitment[32], const uint8_t diff[32], const volatile int *cancel) {
+    uint64_t pos = std::max<uint64_t>(num_labels, md->last_position);
+    while (!md->has_nonce) {
+        if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
+        b200post_vrf_nonce nn;
+        int rc = compute_labels(provider_id, md->scrypt_n, commitment, pos, batch, nullptr, diff, &nn, cancel);
+        if (rc) return rc;
+        pos += batch;
+        md->last_position = pos;
+        if (nn.found) { md->has_nonce = 1; md->nonce = nn.index; memcpy(md->nonce_value, nn.label32, 32); }
+        if ((rc = save_metadata(dir, *md))) return rc;
+    }
+    return B200POST_OK;
+}
+
+}  // namespace b200post
 
 struct b200post_setup_manager {
     b200post_post_config cfg{};
@@ -179,8 +217,10 @@ struct b200post_setup_manager {
     std::string data_dir;
     uint8_t node_id[32] = {0};
     b200post_post_metadata meta{};
-    std::atomic<uint64_t> labels_written{0};
+    std::atomic<uint64_t> labels_written{0};   // of the session's label range
     uint64_t num_labels = 0;
+    uint64_t range_lo = 0, range_hi = 0;        // the session writes labels [range_lo, range_hi)
+    bool range() const { return range_lo != 0 || range_hi != num_labels; }
 };
 
 namespace {
@@ -189,19 +229,6 @@ int fail_state(b200post_setup_manager *m, int code, const std::string &msg) {
     m->state = B200POST_SETUP_ERROR;
     set_error(msg);
     return code;
-}
-
-// labels [start, start+count) on the selected provider(s)
-int compute(const b200post_setup_manager *m, uint64_t start, uint64_t count, uint8_t *out, const uint8_t *diff,
-            b200post_vrf_nonce *nonce, const volatile int *cancel, const uint8_t commitment[32]) {
-    if (m->opts.provider_id == B200POST_PROVIDER_ALL) {
-        const int n = device_count();
-        if (n == 0) { set_error("no CUDA device available"); return B200POST_ERR_NO_DEVICE; }
-        std::vector<uint32_t> ids((size_t)n);
-        for (int i = 0; i < n; i++) ids[(size_t)i] = (uint32_t)i;
-        return b200post_labels_range_multi(ids.data(), n, commitment, m->opts.scrypt_n, start, count, out, diff, nonce, cancel);
-    }
-    return b200post_labels_range((uint32_t)m->opts.provider_id, commitment, m->opts.scrypt_n, start, count, out, diff, nonce, cancel);
 }
 
 }  // namespace
@@ -236,6 +263,11 @@ void b200post_setup_manager_free(b200post_setup_manager *m) { delete m; }
 
 int b200post_setup_prepare_initializer(b200post_setup_manager *m, const b200post_setup_opts *o, const uint8_t node_id[32],
                                        const uint8_t commitment_atx_id[32]) {
+    return b200post_setup_prepare_files(m, o, node_id, commitment_atx_id, 0, -1);
+}
+
+int b200post_setup_prepare_files(b200post_setup_manager *m, const b200post_setup_opts *o, const uint8_t node_id[32],
+                                 const uint8_t commitment_atx_id[32], uint64_t from_file, int64_t to_file) {
     if (!m || !o || !node_id || !commitment_atx_id) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     std::lock_guard<std::mutex> lk(m->mu);
     if (m->state == B200POST_SETUP_PREPARED || m->state == B200POST_SETUP_IN_PROGRESS) {
@@ -255,6 +287,17 @@ int b200post_setup_prepare_initializer(b200post_setup_manager *m, const b200post
     const unsigned __int128 nl = (unsigned __int128)o->num_units * c.labels_per_unit;
     if (nl > (~0ull >> 4)) return fail_state(m, B200POST_ERR_INVALID_ARGUMENT, "NumUnits * LabelsPerUnit overflows");
     if (o->provider_id < B200POST_PROVIDER_ALL || o->provider_id > 0xfffffffe) return fail_state(m, B200POST_ERR_INVALID_ARGUMENT, "invalid `opts.ProviderID`");
+    const uint64_t num_labels = (uint64_t)nl, per_file = o->max_file_size / 16;
+    uint64_t lo = 0, hi = num_labels, last_file = ~0ull;   // the whole POST: no bound on the resume scan (as before ranges)
+    if (from_file != 0 || to_file != -1) {
+        const uint64_t n_files = (num_labels + per_file - 1) / per_file;
+        if (to_file < -1) return fail_state(m, B200POST_ERR_INVALID_ARGUMENT, "invalid file range: toFile < -1");
+        last_file = to_file == -1 ? n_files - 1 : (uint64_t)to_file;
+        if (n_files == 0 || from_file > last_file || last_file >= n_files)
+            return fail_state(m, B200POST_ERR_INVALID_ARGUMENT, "invalid file range: need fromFile <= toFile < " + std::to_string(n_files) + " (the POST's files)");
+        lo = from_file * per_file;
+        hi = std::min<uint64_t>((last_file + 1) * per_file, num_labels);
+    }
 
     const std::string dir = o->data_dir;
     int rc = mkdir_p(dir);
@@ -280,22 +323,26 @@ int b200post_setup_prepare_initializer(b200post_setup_manager *m, const b200post
         meta.scrypt_n = o->scrypt_n; meta.scrypt_r = 1; meta.scrypt_p = 1;
     }
 
-    // ---- resume point: full files 0..k-1, then one partial file
-    const uint64_t num_labels = (uint64_t)nl, per_file = o->max_file_size / 16;
+    // ---- resume point: full files from_file..k-1, then one partial file; nothing past the range is looked at
     uint64_t written = 0;
-    for (uint64_t i = 0;; i++) {
+    for (uint64_t i = from_file; i <= last_file; i++) {
         struct stat st;
         if (stat(data_file(dir, i).c_str(), &st) != 0) break;
         if (st.st_size % 16 || (uint64_t)st.st_size / 16 > per_file) return fail_state(m, B200POST_ERR_CONFIG_MISMATCH, "postdata file has an unexpected size");
         written += (uint64_t)st.st_size / 16;
         if ((uint64_t)st.st_size / 16 < per_file) break;
     }
-    if (written > num_labels) return fail_state(m, B200POST_ERR_CONFIG_MISMATCH, "DataDir holds more labels than NumUnits * LabelsPerUnit");
+    if (written > hi - lo) return fail_state(m, B200POST_ERR_CONFIG_MISMATCH, "DataDir holds more labels than NumUnits * LabelsPerUnit");
+    // a range's labels are not VRF-scanned: without a nonce, the stored data must be searched once it is merged
+    // (with one, the labels are deterministic and the nonce stays right)
+    const bool range = lo != 0 || hi != num_labels;
+    if (range && !meta.has_nonce) meta.vrf_scan_pending = 1;
 
     m->opts = *o; m->data_dir = dir; m->opts.data_dir = m->data_dir.c_str();
     if (m->opts.self_check_every == 0) m->opts.self_check_every = 16;
     memcpy(m->node_id, node_id, 32);
     m->meta = meta; m->num_labels = num_labels; m->have_opts = true;
+    m->range_lo = lo; m->range_hi = hi;
     m->labels_written.store(written);
     if ((rc = save_metadata(dir, m->meta))) { m->state = B200POST_SETUP_ERROR; return rc; }
     m->state = B200POST_SETUP_PREPARED;
@@ -313,8 +360,10 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     auto finish = [&](int32_t state, int rc) { std::lock_guard<std::mutex> lk(m->mu); m->state = state; return rc; };
 
     const uint64_t num_labels = m->num_labels, per_file = m->opts.max_file_size / 16, batch = m->opts.compute_batch_size;
-    uint64_t written = m->labels_written.load();
-    const bool need_work = written < num_labels || !m->meta.has_nonce;
+    const uint64_t lo = m->range_lo, hi = m->range_hi;
+    const bool range = m->range();   // no VRF scan, no nonce, no past-the-end search: a range's arg-min is not the POST's
+    uint64_t written = lo + m->labels_written.load();   // the next label to write
+    const bool need_work = written < hi || (!range && (!m->meta.has_nonce || m->meta.vrf_scan_pending));
     if (need_work && m->opts.provider_id == B200POST_PROVIDER_UNSET) {
         set_error("no provider specified");
         return finish(B200POST_SETUP_ERROR, B200POST_ERR_NO_PROVIDER);
@@ -333,13 +382,14 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         return save_metadata(m->data_dir, m->meta);
     };
 
-    while (written < num_labels) {
+    while (written < hi) {
         if (cancel && *cancel) { set_error("cancelled"); return finish(B200POST_SETUP_STOPPED, B200POST_ERR_CANCELLED); }
         const uint64_t file_idx = written / per_file, in_file = written % per_file;
-        const uint64_t count = std::min<uint64_t>({batch, per_file - in_file, num_labels - written});
+        const uint64_t count = std::min<uint64_t>({batch, per_file - in_file, hi - written});
         buf.resize((size_t)count * 16);
         b200post_vrf_nonce nn;
-        int rc = compute(m, written, count, buf.data(), diff, &nn, cancel, commitment);
+        int rc = compute_labels(m->opts.provider_id, m->opts.scrypt_n, commitment, written, count, buf.data(), range ? nullptr : diff,
+                                &nn, cancel);
         if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
         if (rc) return finish(B200POST_SETUP_ERROR, rc);
         // ErrReferenceLabelMismatch contract (activation/post.go:299-312): every self_check_every batches one label of the
@@ -372,20 +422,25 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         }
         if (!ok || close(fd) != 0) { const int rcio = io_error("write " + path); if (ok) {} else close(fd); return finish(B200POST_SETUP_ERROR, rcio); }
         written += count;
-        m->labels_written.store(written);
+        m->labels_written.store(written - lo);
         if ((rc = note_nonce(nn))) return finish(B200POST_SETUP_ERROR, rc);
     }
-    // "keep searching past numLabels until a VRF nonce is found" (SURVEY.md §8f.1): outputs are discarded
-    uint64_t pos = std::max<uint64_t>(num_labels, m->meta.last_position);
-    while (!m->meta.has_nonce) {
-        if (cancel && *cancel) { set_error("cancelled"); return finish(B200POST_SETUP_STOPPED, B200POST_ERR_CANCELLED); }
-        b200post_vrf_nonce nn;
-        int rc = compute(m, pos, batch, nullptr, diff, &nn, cancel, commitment);
+    if (!range) {
+        int rc;
+        if (m->meta.vrf_scan_pending) {
+            // some files were written by range sessions and never scanned: the nonce comes from all stored labels,
+            // whatever this session's own scan recorded
+            b200post_vrf_search_opts so;
+            b200post_default_vrf_search_opts(&so);
+            so.provider_id = m->opts.provider_id; so.compute_batch_size = batch;
+            b200post_vrf_nonce nn;
+            rc = stored_vrf_search(m->data_dir, &m->meta, so, &nn, cancel);
+        } else {
+            // "keep searching past numLabels until a VRF nonce is found" (SURVEY.md §8f.1): outputs are discarded
+            rc = search_past_end(m->data_dir, &m->meta, num_labels, m->opts.provider_id, batch, commitment, diff, cancel);
+        }
         if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
         if (rc) return finish(B200POST_SETUP_ERROR, rc);
-        pos += batch;
-        m->meta.last_position = pos;
-        if ((rc = nn.found ? note_nonce(nn) : save_metadata(m->data_dir, m->meta))) return finish(B200POST_SETUP_ERROR, rc);
     }
     const int rc = save_metadata(m->data_dir, m->meta);
     if (rc) return finish(B200POST_SETUP_ERROR, rc);

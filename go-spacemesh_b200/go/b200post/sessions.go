@@ -106,10 +106,7 @@ func NewSetupManager(cfg SetupConfig) (*SetupManager, error) {
 	return m, nil
 }
 
-// PrepareInitializer: the commitment ATX is chosen by the caller (activation/post.go:373-435 stays in Go).
-func (m *SetupManager) PrepareInitializer(opts SetupOpts, nodeID, commitmentAtxID []byte) error {
-	dir := C.CString(opts.DataDir)
-	defer C.free(unsafe.Pointer(dir))
+func setupOpts(opts SetupOpts, dir *C.char) C.b200post_setup_opts {
 	var o C.b200post_setup_opts
 	C.b200post_default_setup_opts(&o)
 	o.data_dir = dir
@@ -125,8 +122,29 @@ func (m *SetupManager) PrepareInitializer(opts SetupOpts, nodeID, commitmentAtxI
 	default:
 		o.provider_id = C.int64_t(*opts.ProviderID)
 	}
+	return o
+}
+
+// PrepareInitializer: the commitment ATX is chosen by the caller (activation/post.go:373-435 stays in Go).
+func (m *SetupManager) PrepareInitializer(opts SetupOpts, nodeID, commitmentAtxID []byte) error {
+	dir := C.CString(opts.DataDir)
+	defer C.free(unsafe.Pointer(dir))
+	o := setupOpts(opts, dir)
 	return setupErr(checked(func() C.int {
 		return C.b200post_setup_prepare_initializer(m.h, &o, (*C.uint8_t)(unsafe.Pointer(&nodeID[0])), (*C.uint8_t)(unsafe.Pointer(&commitmentAtxID[0])))
+	}))
+}
+
+// PrepareFiles is PrepareInitializer restricted to postdata files [fromFile, toFile] (toFile -1 = the last file), for one
+// POST initialised on several machines (postcli -fromFile/-toFile).  Without a nonce in the metadata it marks the data
+// VrfScanPending: merge every range's files with one metadata file, then SearchVRFNonce (or run a full session).
+func (m *SetupManager) PrepareFiles(opts SetupOpts, nodeID, commitmentAtxID []byte, fromFile uint64, toFile int64) error {
+	dir := C.CString(opts.DataDir)
+	defer C.free(unsafe.Pointer(dir))
+	o := setupOpts(opts, dir)
+	return setupErr(checked(func() C.int {
+		return C.b200post_setup_prepare_files(m.h, &o, (*C.uint8_t)(unsafe.Pointer(&nodeID[0])), (*C.uint8_t)(unsafe.Pointer(&commitmentAtxID[0])),
+			C.uint64_t(fromFile), C.int64_t(toFile))
 	}))
 }
 
@@ -365,4 +383,57 @@ func VerifyPos(ctx context.Context, dataDir string, o VerifyPosOpts) (*VerifyPos
 		return r, setupErr(rc, msg)
 	}
 	return nil, setupErr(rc, msg)
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// The VRF nonce from stored labels (postcli -searchForNonce, recalled, unpinned)
+// ---------------------------------------------------------------------------------------------------------
+
+type VRFSearchOpts struct {
+	ProviderID       uint32  // CUDA ordinal or AllProviders (scan on the first GPU, past-the-end search on all)
+	ComputeBatchSize uint64  // batch of the past-the-end search; 0 = 2^20 (use the init's batch for the same nonce)
+	ChunkLabels      uint64  // labels per H2D chunk; 0 = 2^22
+	Progress         *uint64 // optional: labels scanned (read it with atomic.LoadUint64)
+}
+
+// SearchVRFNonce finds the VRF nonce of the complete POST in dataDir from its stored labels and writes Nonce,
+// NonceValue and LastPosition to the metadata as one uninterrupted init would have.  Damaged data returns
+// ErrLabelMismatch (the error text names the index) and leaves the metadata as it was.
+func SearchVRFNonce(ctx context.Context, dataDir string, o VRFSearchOpts) (nonce uint64, label [32]byte, err error) {
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var co C.b200post_vrf_search_opts
+	C.b200post_default_vrf_search_opts(&co)
+	if o.ProviderID == AllProviders {
+		co.provider_id = C.B200POST_PROVIDER_ALL
+	} else {
+		co.provider_id = C.int64_t(o.ProviderID)
+	}
+	co.compute_batch_size, co.chunk_labels = C.uint64_t(o.ComputeBatchSize), C.uint64_t(o.ChunkLabels)
+	if o.Progress != nil {
+		var pin runtime.Pinner
+		pin.Pin(o.Progress)
+		defer pin.Unpin()
+		co.progress = (*C.uint64_t)(unsafe.Pointer(o.Progress))
+	}
+	var cancel int32
+	done := make(chan struct{})
+	defer close(done)
+	go func() {
+		select {
+		case <-ctx.Done():
+			atomic.StoreInt32(&cancel, 1)
+		case <-done:
+		}
+	}()
+	var out C.b200post_vrf_nonce
+	rc, msg := checked(func() C.int { return C.b200post_search_vrf_nonce(dir, &co, &out, (*C.int)(unsafe.Pointer(&cancel))) })
+	if rc == C.B200POST_ERR_LABEL_MISMATCH {
+		return 0, label, fmt.Errorf("%w: %s", ErrLabelMismatch, msg)
+	}
+	if err := setupErr(rc, msg); err != nil {
+		return 0, label, err
+	}
+	C.memcpy(unsafe.Pointer(&label[0]), unsafe.Pointer(&out.label32[0]), 32)
+	return uint64(out.index), label, nil
 }

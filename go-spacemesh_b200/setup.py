@@ -9,7 +9,7 @@ from __future__ import annotations
 import ctypes
 from dataclasses import dataclass
 
-from . import B200PostError, ERR_CANCELLED, OK, lib
+from . import B200PostError, ERR_CANCELLED, OK, VrfNonce, lib
 
 (STATE_NOT_STARTED, STATE_PREPARED, STATE_IN_PROGRESS, STATE_STOPPED, STATE_COMPLETE, STATE_ERROR) = range(1, 7)
 ERR_STATE, ERR_NO_PROVIDER, ERR_IO, ERR_LABEL_MISMATCH, ERR_CONFIG_MISMATCH = 10, 11, 12, 13, 14
@@ -35,7 +35,8 @@ class _Metadata(ctypes.Structure):
     _fields_ = [("node_id", ctypes.c_uint8 * 32), ("commitment_atx_id", ctypes.c_uint8 * 32), ("labels_per_unit", ctypes.c_uint64),
                 ("num_units", ctypes.c_uint32), ("max_file_size", ctypes.c_uint64), ("scrypt_n", ctypes.c_uint64),
                 ("scrypt_r", ctypes.c_uint64), ("scrypt_p", ctypes.c_uint64), ("has_nonce", ctypes.c_uint32),
-                ("nonce", ctypes.c_uint64), ("nonce_value", ctypes.c_uint8 * 32), ("last_position", ctypes.c_uint64)]
+                ("nonce", ctypes.c_uint64), ("nonce_value", ctypes.c_uint8 * 32), ("last_position", ctypes.c_uint64),
+                ("vrf_scan_pending", ctypes.c_uint32)]
 
 
 class _VerifyPosOpts(ctypes.Structure):
@@ -47,6 +48,11 @@ class _VerifyPosResult(ctypes.Structure):
     _fields_ = [("files_checked", ctypes.c_uint64), ("labels_checked", ctypes.c_uint64), ("mismatches", ctypes.c_uint64),
                 ("seed", ctypes.c_uint64), ("nonce_ok", ctypes.c_uint32), ("argmin_checked", ctypes.c_uint32),
                 ("argmin_ok", ctypes.c_uint32), ("n_reported", ctypes.c_uint32), ("bad_index", ctypes.c_uint64 * 64)]
+
+
+class _VrfSearchOpts(ctypes.Structure):
+    _fields_ = [("provider_id", ctypes.c_int64), ("compute_batch_size", ctypes.c_uint64), ("chunk_labels", ctypes.c_uint64),
+                ("progress", ctypes.c_void_p)]
 
 
 @dataclass
@@ -111,6 +117,9 @@ def _bind():
     L.b200post_verify_pos.argtypes = [ctypes.c_char_p, ctypes.POINTER(_VerifyPosOpts), ctypes.POINTER(_VerifyPosResult), vp]
     L.b200post_verify_pos_sample.argtypes = [ctypes.c_uint64, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_double, vp,
                                              ctypes.c_uint64, ctypes.POINTER(ctypes.c_uint64)]
+    L.b200post_setup_prepare_files.argtypes = [vp, ctypes.POINTER(_SetupOpts), ctypes.c_char_p, ctypes.c_char_p, ctypes.c_uint64,
+                                               ctypes.c_int64]
+    L.b200post_search_vrf_nonce.argtypes = [ctypes.c_char_p, ctypes.POINTER(_VrfSearchOpts), ctypes.POINTER(VrfNonce), vp]
     L._setup_bound = True
     return L
 
@@ -127,7 +136,19 @@ def load_metadata(data_dir: str) -> dict:
     return dict(node_id=bytes(m.node_id), commitment_atx_id=bytes(m.commitment_atx_id), labels_per_unit=m.labels_per_unit,
                 num_units=m.num_units, max_file_size=m.max_file_size, scrypt_n=m.scrypt_n,
                 nonce=int(m.nonce) if m.has_nonce else None, nonce_value=bytes(m.nonce_value) if m.has_nonce else None,
-                last_position=m.last_position)
+                last_position=m.last_position, vrf_scan_pending=m.vrf_scan_pending)
+
+
+def search_vrf_nonce(data_dir: str, *, provider_id: int = 0, compute_batch_size: int = 0, chunk_labels: int = 0,
+                     progress: ctypes.c_uint64 | None = None, cancel: ctypes.c_int | None = None) -> tuple[int, bytes]:
+    """postcli -searchForNonce: the VRF nonce of the complete POST in data_dir from its stored labels, written to the
+    metadata as a single uninterrupted init would have written it.  Returns (nonce, label32); raises B200PostError
+    (ERR_LABEL_MISMATCH for damaged data, the index in its text; ERR_IO for missing data; ERR_CANCELLED)."""
+    o = _VrfSearchOpts(provider_id, compute_batch_size, chunk_labels, ctypes.addressof(progress) if progress is not None else None)
+    out = VrfNonce()
+    _err(_bind().b200post_search_vrf_nonce(data_dir.encode(), ctypes.byref(o), ctypes.byref(out),
+                                           ctypes.addressof(cancel) if cancel is not None else None))
+    return int(out.index), bytes(out.label32)
 
 
 def verify_pos(data_dir: str, *, fraction: float = 0.2, provider_id: int = 0, from_file: int = 0, to_file: int = -1,
@@ -157,6 +178,12 @@ def verify_pos_sample(seed: int, file: int, labels_in_file: int, fraction: float
     return out
 
 
+def _c_opts(opts: PostSetupOpts) -> _SetupOpts:
+    return _SetupOpts(opts.data_dir.encode(), opts.num_units, opts.max_file_size,
+                      PROVIDER_UNSET if opts.provider_id is None else opts.provider_id,
+                      opts.scrypt_n, opts.scrypt_r, opts.scrypt_p, opts.compute_batch_size, opts.self_check_every)
+
+
 class PostSetupManager:
     def __init__(self, cfg: PostConfig | None = None):
         L = _bind()
@@ -170,10 +197,12 @@ class PostSetupManager:
         _err(L.b200post_setup_manager_new(ctypes.byref(c), ctypes.byref(self._h)))
 
     def prepare_initializer(self, opts: PostSetupOpts, node_id: bytes, commitment_atx_id: bytes) -> None:
-        o = _SetupOpts(opts.data_dir.encode(), opts.num_units, opts.max_file_size,
-                       PROVIDER_UNSET if opts.provider_id is None else opts.provider_id,
-                       opts.scrypt_n, opts.scrypt_r, opts.scrypt_p, opts.compute_batch_size, opts.self_check_every)
-        _err(_bind().b200post_setup_prepare_initializer(self._h, ctypes.byref(o), node_id, commitment_atx_id))
+        _err(_bind().b200post_setup_prepare_initializer(self._h, ctypes.byref(_c_opts(opts)), node_id, commitment_atx_id))
+
+    def prepare_files(self, opts: PostSetupOpts, node_id: bytes, commitment_atx_id: bytes, from_file: int, to_file: int = -1) -> None:
+        """PrepareInitializer restricted to postdata files [from_file, to_file] (-1 = the last file): postcli -fromFile/-toFile."""
+        _err(_bind().b200post_setup_prepare_files(self._h, ctypes.byref(_c_opts(opts)), node_id, commitment_atx_id, from_file,
+                                                  to_file))
 
     def start_session(self, cancel: ctypes.c_int | None = None) -> None:
         """Blocking.  `cancel` = a ctypes.c_int another thread sets to 1 (ctx cancel); raises code ERR_CANCELLED."""

@@ -83,6 +83,9 @@ typedef struct b200post_post_metadata {      /* shared.PostMetadata as stored in
     uint64_t nonce;                          /* VRF nonce (label index)                                         */
     uint8_t nonce_value[32];                 /* its 32-byte label                                                */
     uint64_t last_position;                  /* how far the past-the-end nonce search got                       */
+    uint32_t vrf_scan_pending;               /* "VrfScanPending": some stored labels were written by a file-range
+                                                session and never VRF-scanned; the nonce must come from the stored
+                                                data (b200post_search_vrf_nonce, or a full session's final step)   */
 } b200post_post_metadata;
 
 typedef struct b200post_setup_manager b200post_setup_manager;
@@ -98,7 +101,21 @@ void b200post_setup_manager_free(b200post_setup_manager *mgr);
 /* PrepareInitializer: validates cfg+opts, loads or creates the metadata, finds the resume point. */
 int b200post_setup_prepare_initializer(b200post_setup_manager *mgr, const b200post_setup_opts *opts,
                                        const uint8_t node_id[32], const uint8_t commitment_atx_id[32]);
-/* StartSession: blocking initialisation; `cancel` (may be NULL) is the ctx.Done() analogue. */
+/*
+ * PrepareInitializer restricted to postdata files [from_file, to_file]; to_file = -1 means the POST's last file
+ * (postcli -fromFile / -toFile: one POST initialised on several machines).  prepare_initializer is (0, -1).
+ * from_file <= to_file < n_files = ceil(NumUnits * LabelsPerUnit / (MaxFileSize / 16)), else INVALID_ARGUMENT.
+ * A range short of the whole POST covers labels [from * perFile, min((to + 1) * perFile, numLabels)); it resumes from
+ * from_file (full files, then one partial file) and never opens, creates or writes a file outside the range; the
+ * status counts the range's labels.  It records no VRF nonce and runs no past-the-end search (a range's arg-min is not
+ * the POST's).  If the metadata has no nonce yet, prepare sets "VrfScanPending": copy the files of every range into
+ * one directory with any one metadata file, then b200post_search_vrf_nonce (or a full session) finds the nonce.  If
+ * the metadata already has a nonce (re-initialising a damaged or lost file), it is kept and no marker is set.
+ */
+int b200post_setup_prepare_files(b200post_setup_manager *mgr, const b200post_setup_opts *opts, const uint8_t node_id[32],
+                                 const uint8_t commitment_atx_id[32], uint64_t from_file, int64_t to_file);
+/* StartSession: blocking initialisation; `cancel` (may be NULL) is the ctx.Done() analogue.  A full session on data
+ * whose metadata has VrfScanPending runs b200post_search_vrf_nonce's stored-data search once every label is on disk. */
 int b200post_setup_start_session(b200post_setup_manager *mgr, const volatile int *cancel);
 /* Status: callable from any thread while a session runs (NumLabelsWritten is monotone). */
 int b200post_setup_get_status(b200post_setup_manager *mgr, b200post_setup_status *out);
@@ -148,6 +165,31 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
  * (may be NULL to ask for the size only) receives them when cap >= *n, else INVALID_ARGUMENT. */
 int b200post_verify_pos_sample(uint64_t seed, uint64_t file, uint64_t labels_in_file, double fraction,
                                uint64_t *out, uint64_t cap, uint64_t *n);
+
+/*
+ * The VRF nonce from stored labels (postcli -searchForNonce, recalled, unpinned): for a POST whose files were written
+ * by several file-range sessions, none of which saw every label.  The rule is the one an init applies: the nonce is
+ * the lowest label32 (big-endian), lowest index on ties, recorded only if strictly below floor(2^256 / numLabels);
+ * otherwise the past-the-end search runs from numLabels in compute_batch_size batches.
+ * The arg-min of label32 is decided by its first 16 bytes, which are what is stored: the files are streamed through
+ * the GPU (K8) at 16 B per label, and only the labels at the lowest stored prefix have their label32 recomputed.
+ * One of those whose recomputed first 16 bytes differ from the stored ones means damaged data: LABEL_MISMATCH with
+ * the index in the error text, metadata untouched.  A label damaged upwards is invisible to a scan that trusts the
+ * stored bytes: `b200postcli -verify -fraction 100` (b200post_verify_pos) is the check for that.
+ * Host errors first: no metadata -> ERR_IO; a missing or short file -> ERR_IO "incomplete"; then ERR_NO_DEVICE
+ * without a GPU (no CPU path).  On success Nonce / NonceValue / LastPosition are written as a single uninterrupted
+ * init would have written them, and VrfScanPending is cleared.
+ */
+typedef struct b200post_vrf_search_opts {
+    int64_t provider_id;           /* CUDA ordinal or B200POST_PROVIDER_ALL (scan on the first device, past-the-end search on all) */
+    uint64_t compute_batch_size;   /* batch of the past-the-end search; 0 = 2^20. The same batch as a single init gives the same nonce */
+    uint64_t chunk_labels;         /* labels per H2D chunk; 0 = 2^22 (64 MiB), as the prover; at most 2^26 */
+    volatile uint64_t *progress;   /* optional: labels scanned */
+} b200post_vrf_search_opts;
+/* provider 0, batch 2^20, chunk 2^22, no progress */
+void b200post_default_vrf_search_opts(b200post_vrf_search_opts *o);
+int b200post_search_vrf_nonce(const char *data_dir, const b200post_vrf_search_opts *o, b200post_vrf_nonce *out,
+                              const volatile int *cancel);
 
 #ifdef __cplusplus
 }
