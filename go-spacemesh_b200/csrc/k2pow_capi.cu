@@ -37,6 +37,30 @@ bool clamp_range(uint64_t start, uint64_t &count) {
     return true;
 }
 
+// One window of the prover's search: pows [next, next + per) of every group in `groups`, in one device call.  hit[i] =
+// the smallest valid pow of groups[i] in the window, or B200POST_K2POW_NOT_FOUND.
+int search_window(RandomxEngine *e, const std::string &key, const b200post_k2pow_params *p, const std::vector<uint32_t> &groups,
+                  uint64_t next, uint64_t per, std::vector<uint8_t> &in, std::vector<uint8_t> &out, std::vector<uint64_t> &hit) {
+    const size_t n = groups.size() * per;
+    in.resize(n * 48); out.resize(n * 32);
+    for (size_t gi = 0; gi < groups.size(); gi++)
+        for (uint64_t k = 0; k < per; k++) {
+            uint8_t *d = &in[(gi * per + k) * 48];
+            const uint64_t pow = next + k;
+            for (int b = 0; b < 7; b++) d[b] = (uint8_t)(pow >> (8 * b));
+            d[7] = (uint8_t)groups[gi];
+            memcpy(d + 8, p->challenge8, 8);
+            memcpy(d + 16, p->node_id, 32);
+        }
+    const int rc = e->hash_inputs(key, in.data(), 48, n, out.data());
+    if (rc != B200POST_OK) return rc;
+    hit.assign(groups.size(), B200POST_K2POW_NOT_FOUND);
+    for (size_t gi = 0; gi < groups.size(); gi++)
+        for (uint64_t k = 0; k < per && hit[gi] == B200POST_K2POW_NOT_FOUND; k++)
+            if (memcmp(&out[(gi * per + k) * 32], p->difficulty, 32) < 0) hit[gi] = next + k;
+    return B200POST_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -138,36 +162,79 @@ int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params 
     std::vector<uint32_t> pending(n_groups);
     for (uint32_t g = 0; g < n_groups; g++) pending[g] = g;
     std::vector<uint8_t> in, out;
+    std::vector<uint64_t> hit;
     uint64_t next = 0, total = 0;      // every pending group has tried nonces [0, next)
     while (!pending.empty() && next < max_nonces_per_group) {
         if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
         // one device batch shared by all groups still searching: `per` consecutive nonces each
         const uint64_t per = std::min<uint64_t>(std::max<uint64_t>(1, batch / pending.size()), max_nonces_per_group - next);
-        const size_t n = pending.size() * per;
-        in.resize(n * 48); out.resize(n * 32);
-        for (size_t gi = 0; gi < pending.size(); gi++)
-            for (uint64_t k = 0; k < per; k++) {
-                uint8_t *d = &in[(gi * per + k) * 48];
-                const uint64_t pow = next + k;
-                for (int b = 0; b < 7; b++) d[b] = (uint8_t)(pow >> (8 * b));
-                d[7] = (uint8_t)pending[gi];
-                memcpy(d + 8, p->challenge8, 8);
-                memcpy(d + 16, p->node_id, 32);
-            }
-        const int rc = e->hash_inputs(key, in.data(), 48, n, out.data());
+        const int rc = search_window(e, key, p, pending, next, per, in, out, hit);
         if (rc != B200POST_OK) return rc;
-        total += n;
+        total += pending.size() * per;
         std::vector<uint32_t> still;
-        for (size_t gi = 0; gi < pending.size(); gi++) {
-            uint64_t hit = B200POST_K2POW_NOT_FOUND;
-            for (uint64_t k = 0; k < per && hit == B200POST_K2POW_NOT_FOUND; k++)
-                if (memcmp(&out[(gi * per + k) * 32], p->difficulty, 32) < 0) hit = next + k;
-            if (hit == B200POST_K2POW_NOT_FOUND) still.push_back(pending[gi]); else pows[pending[gi]] = hit;
-        }
+        for (size_t gi = 0; gi < pending.size(); gi++)
+            if (hit[gi] == B200POST_K2POW_NOT_FOUND) still.push_back(pending[gi]); else pows[pending[gi]] = hit[gi];
         pending.swap(still);
         next += per;
     }
     if (hashes_done) *hashes_done = total;
+    return B200POST_OK;
+}
+
+int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
+                                       uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
+                                       uint64_t *hashes_done, const volatile int *cancel) {
+    if (!providers || n_providers <= 0 || !p || !pows || n_groups == 0 || n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    if (n_providers == 1) return b200post_k2pow_search_groups(providers[0], p, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
+    std::vector<RandomxEngine *> eng(n_providers);
+    for (int i = 0; i < n_providers; i++) {
+        eng[i] = randomx_engine_for(providers[i]);
+        if (!eng[i]) return providers[i] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    }
+    for (uint32_t g = 0; g < n_groups; g++) pows[g] = B200POST_K2POW_NOT_FOUND;
+    const std::string key = key_of(p->cache_key, p->cache_key_len);
+    const uint64_t cap = max_nonces_per_group == 0 || max_nonces_per_group > kNonceSpace ? kNonceSpace : max_nonces_per_group;
+    // Windows go out in ascending nonce order from one cursor, each to every group without a hit yet.  So every group
+    // has been handed out the contiguous nonces [0, cursor at its first reported hit), and once all threads have
+    // joined, the smallest hit reported for it is its smallest valid pow.
+    std::mutex mu;
+    uint64_t next = 0, total = 0;
+    std::vector<uint64_t> best(n_groups, B200POST_K2POW_NOT_FOUND);
+    std::vector<int> rcs(n_providers, B200POST_OK);
+    std::vector<std::string> errs(n_providers);
+    std::atomic<bool> stop{false};
+    std::vector<std::thread> th;
+    for (int i = 0; i < n_providers; i++)
+        th.emplace_back([&, i] {
+            uint64_t batch = 0;
+            eng[i]->batch_size(&batch);
+            std::vector<uint8_t> in, out;
+            std::vector<uint64_t> hit;
+            std::vector<uint32_t> groups;
+            while (!stop) {
+                if (cancel && *cancel) { set_error("cancelled"); rcs[i] = B200POST_ERR_CANCELLED; break; }
+                uint64_t lo, per;
+                {
+                    std::lock_guard<std::mutex> lk(mu);
+                    groups.clear();
+                    for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(g);
+                    if (groups.empty() || next >= cap) break;
+                    // one device batch: `per` consecutive nonces for each group still searching, as on one device
+                    per = std::min<uint64_t>(std::max<uint64_t>(1, batch / groups.size()), cap - next);
+                    lo = next;
+                    next += per;
+                }
+                if ((rcs[i] = search_window(eng[i], key, p, groups, lo, per, in, out, hit)) != B200POST_OK) break;
+                std::lock_guard<std::mutex> lk(mu);
+                total += groups.size() * per;
+                for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi]] = std::min(best[groups[gi]], hit[gi]);
+            }
+            if (rcs[i] != B200POST_OK) { errs[i] = last_error(); stop = true; }
+        });
+    for (auto &t : th) t.join();
+    if (hashes_done) *hashes_done = total;
+    for (int i = 0; i < n_providers; i++) if (rcs[i] != B200POST_OK) { set_error(errs[i]); return rcs[i]; }
+    for (uint32_t g = 0; g < n_groups; g++) pows[g] = best[g];
     return B200POST_OK;
 }
 

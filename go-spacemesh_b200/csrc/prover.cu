@@ -5,8 +5,14 @@
 // hit lists and stops when a nonce owns K2 of them.  Bandwidth view: 16 B in per label, ~nothing out; the
 // kernel is far faster than PCIe/NVMe can feed it, so the design goal is simply to keep copies and compute
 // overlapped.  Conventions: post-rs Prover8_56 from memory (ASSUMED, unpinned).
+//
+// Several devices (b200post_generate_proof_multi): the label range is split into contiguous shards, one host thread and
+// Scanner each; their hit lists merge in shard order (ShardedScan), so the proof is the one-device proof.
 #include <algorithm>
+#include <atomic>
+#include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -106,10 +112,24 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
     }
 }
 
+// nonce -> its first hit indices (at most K2), ascending; ordered, so ties resolve to the lower nonce
+using HitLists = std::map<uint32_t, std::vector<uint64_t>>;
+
+// The selection rule, for one scan and for the merge of several: among nonces with K2 hits, the lowest K2-th hit
+// index wins; ties go to the lower nonce.
+bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
+    bool have = false;
+    for (const auto &kv : lists) {
+        if (kv.second.size() < k2) continue;
+        if (!have || kv.second[k2 - 1] < (*indices)[k2 - 1]) { *nonce = kv.first; *indices = kv.second; have = true; }
+    }
+    return have;
+}
+
 // Streaming scan state: device buffers, keys, per-nonce hit lists.
 class Scanner {
 public:
-    ~Scanner() { if (dev_ >= 0) cudaSetDevice(dev_); }   // the members free themselves on the scan's device
+    ~Scanner() { if (dev_ >= 0) { cudaSetDevice(dev_); drain(); } }   // the members free themselves on the scan's device
     int init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
              uint64_t num_labels, uint64_t chunk) {
         DeviceEngine *e = engine_for(provider);
@@ -193,8 +213,9 @@ public:
         pending_[b] = true; count_[b] = count;
         return B200POST_OK;
     }
-    // wait for chunk b and fold its hits in; *found set when some nonce has K2 hits
-    int collect(int b, bool *found) {
+    // wait for chunk b and fold its hits in.  The fold (hit lists, full nonces, labels scanned) happens under
+    // `fold_mu` when given, so that other threads may read that state under the same mutex.
+    int collect(int b, std::mutex *fold_mu = nullptr) {
         if (!pending_[b]) return B200POST_OK;
         CUDA_TRY(cudaEventSynchronize(ev_[b].get()));
         pending_[b] = false;
@@ -202,28 +223,28 @@ public:
         if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
         std::vector<Hit> v(h_hits_[b].get(), h_hits_[b].get() + n);
         std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+        std::unique_lock<std::mutex> lk;
+        if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
         for (const Hit &h : v) {
             std::vector<uint64_t> &l = lists_[h.nonce];
-            if (l.size() < k2_) l.push_back(h.index);
+            if (l.size() < k2_ && (l.push_back(h.index), l.size() == k2_)) full_++;
         }
         scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
-        for (auto &kv : lists_) if (kv.second.size() >= k2_) *found = true;
         return B200POST_OK;
     }
-    // the winning nonce: lowest K2-th hit index, ties to the lower nonce
-    bool winner(uint32_t *nonce, std::vector<uint64_t> *indices) const {
-        bool have = false;
-        for (const auto &kv : lists_) {
-            if (kv.second.size() < k2_) continue;
-            if (!have || kv.second[k2_ - 1] < (*indices)[k2_ - 1]) { *nonce = kv.first; *indices = kv.second; have = true; }
-        }
-        return have;
+    // wait for whatever is still in flight, without folding it (error and cancel paths)
+    void drain() {
+        for (int b = 0; b < 2; b++) if (pending_[b]) { cudaEventSynchronize(ev_[b].get()); pending_[b] = false; }
     }
+    const HitLists &lists() const { return lists_; }
+    bool any_full() const { return full_ > 0; }          // some nonce has K2 hits
+    bool saturated() const { return full_ == nonces_; }  // every nonce has K2 hits: later labels change no first K2
     uint64_t scanned() const { return scanned_; }
+    int device() const { return dev_; }
 
 private:
     int dev_ = -1;
-    uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0;
+    uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0, full_ = 0;
     uint64_t lsb_ = 0, chunk_ = 0, scanned_ = 0;
     DeviceBuffer<uint8_t> d_rk_, d_lazy_;
     DeviceBuffer<AesTables> d_tables_;
@@ -240,17 +261,126 @@ private:
     uint32_t cand_cap_ = 0;
     bool pending_[2] = {false, false};
     uint32_t count_[2] = {0, 0};
-    std::map<uint32_t, std::vector<uint64_t>> lists_;   // ordered: ties resolve to the lower nonce
+    HitLists lists_;
 };
 
-int finish(const Scanner &sc, uint32_t nonces, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
+// One contiguous label range [lo, hi) of a scan, streamed through its own Scanner.
+struct Shard {
+    Scanner sc;
+    uint64_t lo = 0, hi = 0;
+    int rc = B200POST_OK;
+    std::string err;
+};
+
+// The labels [0, total) in contiguous shards of whole chunks, one per provider in list order, sized within one chunk of
+// each other (the earlier shards take the odd chunks; a shard may be empty).
+std::vector<std::pair<uint64_t, uint64_t>> split_shards(uint64_t total, uint64_t chunk, size_t n) {
+    const uint64_t chunks = (total + chunk - 1) / chunk, q = chunks / n, r = chunks % n;
+    std::vector<std::pair<uint64_t, uint64_t>> out(n);
+    for (size_t s = 0; s < n; s++) {
+        const uint64_t first = s * q + std::min<uint64_t>(s, r), end = first + q + (s < r ? 1 : 0);
+        out[s] = {std::min(total, first * chunk), std::min(total, end * chunk)};
+    }
+    return out;
+}
+
+// A scan split into shards, one host thread each.  Stop rule: let x be the end of the longest gap-free scanned prefix
+// of [0, total), where a saturated shard counts as whole.  Once the hits below x give some nonce K2 of them the proof is
+// decided (every hit below x is known, so no nonce whose K2-th hit lies past x can win) and every shard stops.  A shard
+// also stops on its own once it is saturated.  With one shard this is "stop once a nonce has K2 hits".
+class ShardedScan {
+public:
+    // fill(shard, first label, count, dst): those labels into the shard's pinned staging
+    using Fill = std::function<int(size_t, uint64_t, uint64_t, uint8_t *)>;
+
+    ShardedScan(size_t n, uint32_t nonces, uint32_t k2) : nonces_(nonces), k2_(k2) {
+        for (size_t s = 0; s < n; s++) shards_.emplace_back(new Shard);
+    }
+    Shard &shard(size_t s) { return *shards_[s]; }
+
+    // runs every shard (the calling thread alone when there is one) and returns the first failing shard's status, in
+    // list order, once every thread has joined
+    int run(const Fill &fill, uint64_t chunk, uint64_t base, const volatile int *cancel) {
+        if (shards_.size() == 1) return run_shard(0, fill, chunk, base, cancel);
+        std::vector<std::thread> th;
+        for (size_t s = 0; s < shards_.size(); s++)
+            th.emplace_back([&, s] {
+                Shard &sh = *shards_[s];
+                if ((sh.rc = run_shard(s, fill, chunk, base, cancel)) != B200POST_OK) { sh.err = last_error(); abort_ = true; }
+            });
+        for (auto &t : th) t.join();
+        for (auto &sh : shards_) if (sh->rc != B200POST_OK) { set_error(sh->err); return sh->rc; }
+        return B200POST_OK;
+    }
+
+    // per nonce, the shards' hit lists appended in shard order, first K2 kept; with the stop rule above, the winner of
+    // these lists is the winner of a scan over every label
+    HitLists merged() const {
+        HitLists m;
+        for (const auto &sh : shards_)
+            for (const auto &kv : sh->sc.lists()) {
+                std::vector<uint64_t> &l = m[kv.first];
+                for (size_t i = 0; i < kv.second.size() && l.size() < k2_; i++) l.push_back(kv.second[i]);
+            }
+        return m;
+    }
+    uint64_t scanned() const {
+        uint64_t t = 0;
+        for (const auto &sh : shards_) t += sh->sc.scanned();
+        return t;
+    }
+
+private:
+    int run_shard(size_t s, const Fill &fill, uint64_t chunk, uint64_t base, const volatile int *cancel) {
+        Shard &sh = *shards_[s];
+        Scanner &sc = sh.sc;
+        std::mutex *mu = shards_.size() > 1 ? &mu_ : nullptr;
+        int rc = B200POST_OK;
+        if (sh.lo == sh.hi) return rc;
+        if (cudaSetDevice(sc.device()) != cudaSuccess) { cudaGetLastError(); set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
+        int b = 0;
+        for (uint64_t pos = sh.lo; pos < sh.hi; b ^= 1) {
+            if (cancel && *cancel) { sc.drain(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
+            if (abort_) { sc.drain(); return B200POST_OK; }   // another shard failed: its status is the call's
+            if ((rc = sc.collect(b, mu))) { sc.drain(); return rc; }
+            if (should_stop(s)) break;
+            // fill the staging buffer (a chunk may span files)
+            const uint64_t n = std::min<uint64_t>(chunk, sh.hi - pos);
+            if ((rc = fill(s, pos, n, sc.staging(b))) || (rc = sc.submit(b, base + pos, (uint32_t)n))) { sc.drain(); return rc; }
+            pos += n;
+        }
+        for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, mu))) { sc.drain(); return rc; }   // older chunk first
+        return B200POST_OK;
+    }
+
+    bool should_stop(size_t s) {
+        if (shards_.size() == 1) return shards_[0]->sc.any_full();
+        std::lock_guard<std::mutex> lk(mu_);
+        if (shards_[s]->sc.saturated()) return true;
+        below_x_.assign(nonces_, 0);   // hits below x per nonce
+        for (const auto &sh : shards_) {
+            for (const auto &kv : sh->sc.lists())
+                if ((below_x_[kv.first] += kv.second.size()) >= k2_) return true;
+            if (sh->sc.scanned() < sh->hi - sh->lo && !sh->sc.saturated()) break;   // x lies in this shard
+        }
+        return false;
+    }
+
+    uint32_t nonces_, k2_;
+    std::vector<std::unique_ptr<Shard>> shards_;
+    std::mutex mu_;                  // guards every shard's hit lists and progress once the threads run
+    std::vector<uint64_t> below_x_;
+    std::atomic<bool> abort_{false};
+};
+
+int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
     uint32_t nonce = 0;
     std::vector<uint64_t> idx;
-    if (!sc.winner(&nonce, &idx)) { set_error("no proof found: no nonce reached K2 qualifying labels"); return B200POST_ERR_INVALID_PROOF; }
-    (void)nonces;
-    metrics().prove_labels_scanned_total += sc.scanned(); metrics().proofs_generated_total++;
+    if (!pick_winner(scan.merged(), k2, &nonce, &idx)) { set_error("no proof found: no nonce reached K2 qualifying labels"); return B200POST_ERR_INVALID_PROOF; }
+    const uint64_t scanned = scan.scanned();
+    metrics().prove_labels_scanned_total += scanned; metrics().proofs_generated_total++;
     memset(out, 0, sizeof *out);
-    out->nonce = nonce; out->pow = pows[nonce / 16]; out->labels_scanned = sc.scanned();
+    out->nonce = nonce; out->pow = pows[nonce / 16]; out->labels_scanned = scanned;
     out->indices_len = b200post_pack_indices(idx.data(), idx.size(), b200post_bits_per_index(num_labels), out->indices, sizeof out->indices);
     if (out->indices_len == 0) { set_error("packed indices exceed the 800-byte wire cap"); return B200POST_ERR_INVALID_ARGUMENT; }
     return B200POST_OK;
@@ -283,27 +413,31 @@ extern "C" {
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count, const uint8_t challenge[32],
                         uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2, uint64_t num_labels, b200post_proof_out *out) {
     if (!labels16 || !challenge || !pows || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    Scanner sc;
+    ShardedScan scan(1, nonces, k2);
+    Shard &sh = scan.shard(0);
     const uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(count, 1), 1u << 22);
-    int rc = sc.init(provider, challenge, nonces, pows, k1, k2, num_labels, chunk);
+    int rc = sh.sc.init(provider, challenge, nonces, pows, k1, k2, num_labels, chunk);
     if (rc) return rc;
-    bool found = false;
-    int b = 0;
-    for (uint64_t off = 0; off < count && !found; off += chunk, b ^= 1) {
-        if ((rc = sc.collect(b, &found))) return rc;
-        if (found) break;
-        const uint32_t n = (uint32_t)std::min<uint64_t>(chunk, count - off);
-        parallel_copy(sc.staging(b), labels16 + off * 16, (size_t)n * 16);   // pageable -> pinned staging, the scan's host-side bound
-        if ((rc = sc.submit(b, first_index + off, n))) return rc;
-    }
-    for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, &found))) return rc;   // older chunk first
-    return finish(sc, nonces, pows, num_labels, out);
+    sh.lo = 0; sh.hi = count;
+    rc = scan.run([&](size_t, uint64_t off, uint64_t n, uint8_t *dst) {
+        parallel_copy(dst, labels16 + off * 16, (size_t)n * 16);   // pageable -> pinned staging, the scan's host-side bound
+        return B200POST_OK;
+    }, chunk, first_index, nullptr);
+    if (rc) return rc;
+    return finish(scan, k2, pows, num_labels, out);
 }
 
 int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
                             const b200post_prove_opts *opts, b200post_proof_out *out, b200post_proof_metadata *meta_out,
                             const volatile int *cancel) {
-    if (!data_dir || !challenge || !cfg || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    const uint32_t provider = opts ? opts->provider : 0;
+    return b200post_generate_proof_multi(data_dir, challenge, cfg, opts, &provider, 1, out, meta_out, cancel);
+}
+
+int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                  const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                  b200post_proof_out *out, b200post_proof_metadata *meta_out, const volatile int *cancel) {
+    if (!data_dir || !challenge || !cfg || !out || !providers || n_providers <= 0) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     b200post_prove_opts o{};
     if (opts) o = *opts;
     if (o.nonces == 0) o.nonces = 16;
@@ -332,31 +466,27 @@ int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], c
             memcpy(kp.challenge8, challenge, 8);
             memcpy(kp.node_id, md.node_id, 32);
             memcpy(kp.difficulty, scaled, 32);
-            if ((rc = b200post_k2pow_search_groups(o.provider, &kp, o.nonces / 16, 0, pows.data(), nullptr, cancel))) return rc;
+            if ((rc = b200post_k2pow_search_groups_multi(providers, n_providers, &kp, o.nonces / 16, 0, pows.data(), nullptr, cancel))) return rc;
             for (uint64_t v : pows) if (v == B200POST_K2POW_NOT_FOUND) { set_error("k2pow: nonce space exhausted"); return B200POST_ERR_INVALID_PROOF; }
         }
     }
-    Scanner sc;
+    // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
     const uint64_t chunk = std::min<uint64_t>(o.chunk_labels, num_labels);
-    if ((rc = sc.init(o.provider, challenge, o.nonces, pows.data(), cfg->k1, cfg->k2, num_labels, chunk))) return rc;
+    ShardedScan scan((size_t)n_providers, o.nonces, cfg->k2);
+    const auto ranges = split_shards(num_labels, chunk, (size_t)n_providers);
+    for (int s = 0; s < n_providers; s++) {
+        Shard &sh = scan.shard((size_t)s);
+        if ((rc = sh.sc.init(providers[s], challenge, o.nonces, pows.data(), cfg->k1, cfg->k2, num_labels, chunk))) return rc;
+        sh.lo = ranges[(size_t)s].first; sh.hi = ranges[(size_t)s].second;
+    }
 
     const uint64_t per_file = md.max_file_size / 16;
     if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
-    bool found = false;
-    int b = 0;
-    PostDataReader reader(data_dir, per_file);
-    for (uint64_t pos = 0; pos < num_labels && !found; b ^= 1) {
-        if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
-        if ((rc = sc.collect(b, &found))) return rc;
-        if (found) break;
-        // fill the staging buffer from the files (a chunk may span files)
-        const uint64_t n = std::min<uint64_t>(chunk, num_labels - pos);
-        if ((rc = reader.read(pos, n, sc.staging(b)))) return rc;
-        if ((rc = sc.submit(b, pos, (uint32_t)n))) return rc;
-        pos += n;
-    }
-    for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, &found))) return rc;   // older chunk first
-    if ((rc = finish(sc, o.nonces, pows.data(), num_labels, out))) return rc;
+    std::vector<std::unique_ptr<PostDataReader>> readers;
+    for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
+    rc = scan.run([&](size_t s, uint64_t pos, uint64_t n, uint8_t *dst) { return readers[s]->read(pos, n, dst); }, chunk, 0, cancel);
+    if (rc) return rc;
+    if ((rc = finish(scan, cfg->k2, pows.data(), num_labels, out))) return rc;
     if (meta_out) {
         memcpy(meta_out->node_id, md.node_id, 32);
         memcpy(meta_out->commitment_atx_id, md.commitment_atx_id, 32);

@@ -128,6 +128,33 @@ func K2powSearchGroups(ctx context.Context, provider uint32, p *K2powParams, gro
 	return out, nil
 }
 
+// K2powSearchGroupsOn is K2powSearchGroups over several devices (repeats allowed): windows of nonces go to the devices
+// from one shared cursor, and the result is exactly the one-device result (the smallest valid pow of every group).
+func K2powSearchGroupsOn(ctx context.Context, providers []uint32, p *K2powParams, groups uint32, maxNoncesPerGroup uint64) ([]uint64, error) {
+	if len(providers) == 0 {
+		return nil, ErrNoProvider
+	}
+	if groups == 0 {
+		return nil, nil
+	}
+	cp, free := p.cParams()
+	defer free()
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	pows := (*C.uint64_t)(C.calloc(C.size_t(groups), 8))
+	defer C.free(unsafe.Pointer(pows))
+	if err := statusErr(checked(func() C.int {
+		return C.b200post_k2pow_search_groups_multi(provs, C.int(len(providers)), cp, C.uint32_t(groups), C.uint64_t(maxNoncesPerGroup), pows, nil, flag)
+	})); err != nil {
+		return nil, err
+	}
+	out := make([]uint64, groups)
+	copy(out, unsafe.Slice((*uint64)(unsafe.Pointer(pows)), groups))
+	return out, nil
+}
+
 // K2powVerify is the verifier's check of one proof's pow (the batched verifier does the same for a whole batch in one
 // device launch; this entry point is for callers that hold a single pow).
 func K2powVerify(provider uint32, p *K2powParams, pow uint64) (bool, error) {

@@ -319,6 +319,33 @@ func GenerateProof(provider uint32, dataDir string, challenge []byte, cfg SetupC
 	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
 }
 
+// GenerateProofOn is GenerateProof over several devices (repeats allowed): the k2pow windows and contiguous shards of
+// the label scan are spread over the list, and the proof is byte-identical to the one-device proof.  ctx cancels the
+// call (polled between k2pow windows and per scan chunk).  A read error in any shard fails the call, even past the
+// point where a one-device scan would already have found its proof.
+func GenerateProofOn(ctx context.Context, providers []uint32, dataDir string, challenge []byte, cfg SetupConfig, nonces uint32) (*Proof, error) {
+	if len(providers) == 0 {
+		return nil, ErrNoProvider
+	}
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces)}
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	var out C.b200post_proof_out
+	if err := statusErr(checked(func() C.int {
+		return C.b200post_generate_proof_multi(dir, (*C.uint8_t)(unsafe.Pointer(&challenge[0])), &c, &o, provs, C.int(len(providers)), &out, nil, flag)
+	})); err != nil {
+		return nil, err
+	}
+	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Checking stored POST data (postcli -verify; verifying.VerifyPos, recalled, unpinned)
 // ---------------------------------------------------------------------------------------------------------

@@ -35,6 +35,8 @@ def _bind():
         L.b200post_k2pow_search_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u64, u64,
                                                   ctypes.POINTER(u64), ctypes.POINTER(u64), vp]
         L.b200post_k2pow_search_groups.argtypes = [u32, ctypes.POINTER(_Params), u32, u64, vp, ctypes.POINTER(u64), vp]
+        L.b200post_k2pow_search_groups_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u32, u64, vp,
+                                                         ctypes.POINTER(u64), vp]
         L.b200post_k2pow_verify.argtypes = [u32, ctypes.POINTER(_Params), u64, ctypes.POINTER(ctypes.c_int)]
         L.b200post_randomx_dataset_read.argtypes = [u32, ctypes.c_char_p, sz, u64, u64, vp]
         L.b200post_randomx_last_timing.argtypes = [u32, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
@@ -100,14 +102,23 @@ def search(nonce_group: int, challenge8: bytes, node_id: bytes, difficulty: byte
 
 
 def search_groups(challenge8: bytes, node_id: bytes, difficulty: bytes, n_groups: int, max_nonces_per_group: int = 0, *,
-                  key: bytes | None = None, provider: int = 0):
+                  key: bytes | None = None, provider: int = 0, providers: list[int] | None = None, cancel=None):
     """The prover's search: the smallest valid pow of each nonce group 0..n_groups-1 (None where there is none below
-    max_nonces_per_group; 0 = the whole nonce space).  -> (pows, hashes computed)."""
+    max_nonces_per_group; 0 = the whole nonce space).  providers: several devices (repeats allowed), same pows.
+    -> (pows, hashes computed)."""
     p = _params(0, challenge8, node_id, difficulty, key)
-    pows = np.zeros(n_groups, dtype=np.uint64)
+    pows = np.zeros(max(n_groups, 1), dtype=np.uint64)
     done = ctypes.c_uint64(0)
-    _check(_bind().b200post_k2pow_search_groups(provider, ctypes.byref(p), n_groups, max_nonces_per_group, pows.ctypes.data,
-                                                ctypes.byref(done), None))
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    if providers is not None:
+        arr = (ctypes.c_uint32 * len(providers))(*providers)
+        _check(_bind().b200post_k2pow_search_groups_multi(arr if len(providers) else None, len(providers), ctypes.byref(p),
+                                                          n_groups, max_nonces_per_group, pows.ctypes.data, ctypes.byref(done),
+                                                          cptr))
+    else:
+        _check(_bind().b200post_k2pow_search_groups(provider, ctypes.byref(p), n_groups, max_nonces_per_group,
+                                                    pows.ctypes.data, ctypes.byref(done), cptr))
+    pows = pows[:n_groups]
     return [None if int(v) == NOT_FOUND else int(v) for v in pows], done.value
 
 

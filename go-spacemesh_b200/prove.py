@@ -10,7 +10,7 @@ import ctypes
 
 import numpy as np
 
-from . import B200PostError, OK, lib
+from . import B200PostError, ERR_NO_DEVICE, OK, lib, providers as _providers
 from .setup import PostConfig, _PostConfig, _bind as _bind_setup
 from .verify import Proof, ProofMetadata, _Meta
 
@@ -35,6 +35,9 @@ def _bind():
         return L
     L.b200post_generate_proof.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
                                           ctypes.POINTER(_ProofOut), ctypes.POINTER(_Meta), ctypes.c_void_p]
+    L.b200post_generate_proof_multi.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
+                                                ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_ProofOut),
+                                                ctypes.POINTER(_Meta), ctypes.c_void_p]
     L.b200post_prove_scan.argtypes = [ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_char_p, ctypes.c_uint32,
                                       ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.POINTER(_ProofOut)]
     L._prove_bound = True
@@ -56,20 +59,38 @@ def _err(rc):
         raise B200PostError(rc, lib().b200post_last_error().decode(errors="replace"))
 
 
-def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int = 0, nonces: int = 16,
-                   chunk_labels: int = 0, pow="builtin"):
+def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int | None = None, nonces: int = 16,
+                   chunk_labels: int = 0, pow="builtin", providers=None, cancel=None):
     """PostClient.Proof(ctx, challenge) -> (Post, PostInfo-like metadata); also returns labels scanned.
     pow: "builtin" (k2pow search on the device, the library default), "skip" (pow = 0, explicit) or a callable
-    (ctx, nonce_group, challenge8, difficulty32, node_id32, pow_out) -> 0."""
+    (ctx, nonce_group, challenge8, difficulty32, node_id32, pow_out) -> 0.
+    providers: a list of device ids (repeats allowed) or "all" proves on several devices with the one-device result;
+    it replaces `provider` (default 0), and giving both is an error.  cancel: an optional ctypes.c_int, polled per
+    chunk."""
     L = _bind()
+    if provider is not None and providers is not None:
+        raise ValueError("give `provider` or `providers`, not both")
+    if isinstance(providers, str):
+        if providers != "all":
+            raise ValueError(f"providers must be a list of device ids or 'all', not {providers!r}")
+        providers = [p["id"] for p in _providers()]
+        if not providers:
+            raise B200PostError(ERR_NO_DEVICE, "providers='all': libb200post reports no CUDA device")
     if callable(pow):
         cb, mode = POW_PROVE_FN(pow), 1
     else:
         cb, mode = ctypes.cast(None, POW_PROVE_FN), {"builtin": 0, "skip": 2, "callback-missing": 1}[pow]
-    opts = _ProveOpts(provider, nonces, chunk_labels, cb, None, mode, None, 0)
+    opts = _ProveOpts(provider or 0, nonces, chunk_labels, cb, None, mode, None, 0)
     out, meta, c = _ProofOut(), _Meta(), _c_cfg(cfg)
-    _err(L.b200post_generate_proof(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts), ctypes.byref(out),
-                                   ctypes.byref(meta), None))
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    if providers is None:
+        _err(L.b200post_generate_proof(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts), ctypes.byref(out),
+                                       ctypes.byref(meta), cptr))
+    else:
+        arr = (ctypes.c_uint32 * len(providers))(*providers)
+        _err(L.b200post_generate_proof_multi(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts),
+                                             arr if len(providers) else None, len(providers), ctypes.byref(out),
+                                             ctypes.byref(meta), cptr))
     proof = Proof(int(out.nonce), bytes(out.indices[: out.indices_len]), int(out.pow))
     pm = ProofMetadata(bytes(meta.node_id), bytes(meta.commitment_atx_id), bytes(meta.challenge), int(meta.num_units),
                        int(meta.labels_per_unit))

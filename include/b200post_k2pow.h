@@ -83,6 +83,17 @@ int b200post_k2pow_search_multi(const uint32_t *providers, int n_providers, cons
 int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params *p, uint32_t n_groups, uint64_t max_nonces_per_group,
                                  uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel);
 
+/* The same search on several devices (n_providers >= 1; repeats allowed, their windows then share the device), with the
+ * same result: pows[g] is the smallest valid pow of group g below the cap whatever the number of devices and the order
+ * they finish in.  One host thread per list entry takes windows (consecutive nonces of every group that has no hit yet,
+ * a device batch in all) from a shared cursor; a group's pow is final once every window below its lowest hit has
+ * finished, and no window is handed out for a group that has a hit.  *hashes_done = the sum over devices.  `cancel` is
+ * polled between windows.  The first failing entry's status (list order) is returned once every thread has joined.
+ * One provider = b200post_k2pow_search_groups. */
+int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
+                                       uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
+                                       uint64_t *hashes_done, const volatile int *cancel);
+
 /* The verifier's check: *valid = 1 iff RandomX(input(pow)) < p->difficulty. */
 int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uint64_t pow, int *valid);
 

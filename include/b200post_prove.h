@@ -63,6 +63,25 @@ int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], c
                             const b200post_prove_opts *opts, b200post_proof_out *out, b200post_proof_metadata *meta_out,
                             const volatile int *cancel);
 
+/* The same proof on several devices (b200post_generate_proof is its one-provider case).  opts->provider is ignored;
+ * `providers` (n_providers >= 1 entries, repeats allowed: such shards share the device) takes its place.
+ *   k2pow (BUILTIN): b200post_k2pow_search_groups_multi over the same list.  CALLBACK and SKIP as for one device.
+ *   scan: [0, numLabels) is split into contiguous shards of whole chunks, one per list entry in list order, sized
+ *         within one chunk of each other (a shard may be empty); each shard runs on its own host thread with its own
+ *         buffers and reader and keeps, per nonce, its first K2 hits.  The lists merge in shard order (first K2 kept)
+ *         and the one-device selection rule picks the winner, so (nonce, indices, pow) are byte-identical to one
+ *         device's for the same inputs, chunk size and pows.
+ *   stop: once the hits below the end of the gap-free scanned prefix give a nonce K2 of them, every shard stops; a
+ *         shard also stops once every nonce has K2 hits inside it.
+ *   labels_scanned = the sum over shards (the metric grows by the same); `cancel` is polled per chunk in every shard.
+ * Errors: arguments, then metadata (B200POST_ERR_IO), then B200POST_ERR_NO_DEVICE / UNSUPPORTED (CPU id), as for one
+ * device.  A read or device error in ANY shard fails the call once every thread has joined (the first failing shard in
+ * list order gives the status and text).  Unlike one device, a shard can reach damaged or missing data past the point
+ * where a one-device scan would already have stopped with a proof. */
+int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                  const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                  b200post_proof_out *out, b200post_proof_metadata *meta_out, const volatile int *cancel);
+
 /* The scan alone over labels already in host memory: labels16 = count x 16 bytes holding label indices
  * [first_index, first_index + count).  pows = one u64 per nonce group (nonces/16 of them). */
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count,
