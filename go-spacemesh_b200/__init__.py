@@ -225,6 +225,47 @@ def verify_vrf_nonce(nonce: int, node_id: bytes, commitment_atx_id: bytes, num_u
     return bool(valid.value)
 
 
+class VrfCheck(ctypes.Structure):
+    """b200post_vrf_check: shared.VRFNonceMetadata + nonce (activation/validation.go:261-285)."""
+    _fields_ = [("node_id", ctypes.c_uint8 * 32), ("commitment_atx_id", ctypes.c_uint8 * 32), ("nonce", ctypes.c_uint64),
+                ("labels_per_unit", ctypes.c_uint64), ("scrypt_n", ctypes.c_uint64), ("num_units", ctypes.c_uint32),
+                ("prioritized", ctypes.c_uint32)]
+
+
+def vrf_check(node_id: bytes, commitment_atx_id: bytes, nonce: int, num_units: int, labels_per_unit: int, n: int = 8192, *,
+              prioritized: bool = False) -> VrfCheck:
+    c = VrfCheck(nonce=nonce, labels_per_unit=labels_per_unit, scrypt_n=n, num_units=num_units, prioritized=int(prioritized))
+    ctypes.memmove(c.node_id, node_id, 32)
+    ctypes.memmove(c.commitment_atx_id, commitment_atx_id, 32)
+    return c
+
+
+def verify_vrf_nonces(checks, *, provider: int = 0, providers: list[int] | None = None) -> list[tuple[int, bool, bytes]]:
+    """Many VRF-nonce checks in one GPU batch (with `providers`: split over those devices).  `checks` holds VrfCheck
+    structs or (node_id, commitment_atx_id, nonce, num_units, labels_per_unit, n) tuples.  Returns per check
+    (status, valid, label32): valid = label32 < floor(2^256 / numLabels), the UNPINNED rule of verify_vrf_nonce;
+    label32 = the label at the nonce, for the network's own rule.  A malformed check has status ERR_INVALID_ARGUMENT."""
+    checks = [c if isinstance(c, VrfCheck) else vrf_check(*c) for c in checks]
+    n = len(checks)
+    arr = (VrfCheck * max(n, 1))(*checks)
+    st, ok = (ctypes.c_int * max(n, 1))(), (ctypes.c_int * max(n, 1))()
+    labels = ctypes.create_string_buffer(32 * max(n, 1))
+    L = lib()
+    if providers is not None:
+        ids = (ctypes.c_uint32 * max(len(providers), 1))(*providers)
+        L.b200post_verify_vrf_nonces_multi.argtypes = [ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.c_size_t,
+                                                       ctypes.POINTER(VrfCheck), ctypes.POINTER(ctypes.c_int),
+                                                       ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
+        rc = L.b200post_verify_vrf_nonces_multi(ids, len(providers), n, arr, st, ok, labels)
+    else:
+        L.b200post_verify_vrf_nonces.argtypes = [ctypes.c_uint32, ctypes.c_size_t, ctypes.POINTER(VrfCheck),
+                                                 ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), ctypes.c_void_p]
+        rc = L.b200post_verify_vrf_nonces(provider, n, arr, st, ok, labels)
+    _check(rc)
+    raw = labels.raw
+    return [(int(st[i]), bool(ok[i]), raw[32 * i:32 * i + 32]) for i in range(n)]
+
+
 def vrf_nonce_label(nonce: int, node_id: bytes, commitment_atx_id: bytes, n: int, *, provider: int = 0) -> bytes:
     """label32 at index `nonce` of the identity's POST — the policy-free half of VerifyVRFNonce."""
     out = ctypes.create_string_buffer(32)

@@ -7,6 +7,7 @@
 #include <vector>
 
 #include "../../include/b200post.h"
+#include "../../include/b200post_verify.h"
 #include "../../include/post_compat.h"
 #include "engine.h"
 #include "host_hash.h"
@@ -191,33 +192,44 @@ void b200post_commitment(const uint8_t node_id[32], const uint8_t commitment_atx
 
 void b200post_vrf_difficulty(uint64_t num_labels, uint8_t out[32]) { vrf_difficulty(num_labels, out); }
 
+// The one-check case of b200post_verify_vrf_nonces (one path for every VRF-nonce check).  The check's own arguments are
+// judged here first, so that they keep their codes before the provider and device checks of the batch call.
+static int vrf_check_one(uint32_t provider, uint64_t nonce, const uint8_t node_id[32], const uint8_t commitment_atx_id[32],
+                         uint32_t num_units, uint64_t labels_per_unit, uint64_t n, int *valid, uint8_t label32[32]) {
+    if (!valid_n(n)) { set_error("invalid argument (N not a power of two in [2, 2^20])"); return B200POST_ERR_INVALID_ARGUMENT; }
+    b200post_vrf_check c;
+    memset(&c, 0, sizeof c);
+    memcpy(c.node_id, node_id, 32);
+    memcpy(c.commitment_atx_id, commitment_atx_id, 32);
+    c.nonce = nonce; c.num_units = num_units; c.labels_per_unit = labels_per_unit; c.scrypt_n = n;
+    int status = B200POST_OK;
+    const int rc = b200post_verify_vrf_nonces(provider, 1, &c, &status, valid, label32);
+    return rc ? rc : status;
+}
+
 int b200post_verify_vrf_nonce(uint32_t provider, uint64_t nonce, const uint8_t node_id[32],
                               const uint8_t commitment_atx_id[32], uint32_t num_units, uint64_t labels_per_unit,
                               uint64_t n, int *valid) {
     if (!node_id || !commitment_atx_id || !valid) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     *valid = 0;
-    uint8_t commitment[32], diff[32];
-    commitment_bytes(node_id, commitment_atx_id, commitment);
     const unsigned __int128 total = (unsigned __int128)num_units * labels_per_unit;
     if (total == 0 || total > ~0ull) { set_error("num_units * labels_per_unit out of range"); return B200POST_ERR_INVALID_ARGUMENT; }
-    vrf_difficulty((uint64_t)total, diff);
-    b200post_vrf_nonce r;
-    const int rc = b200post_labels_range(provider, commitment, n, nonce, 1, nullptr, diff, &r, nullptr);
+    int ok = 0;
+    const int rc = vrf_check_one(provider, nonce, node_id, commitment_atx_id, num_units, labels_per_unit, n, &ok, nullptr);
     if (rc) return rc;
-    *valid = (r.found && r.index == nonce) ? 1 : 0;
+    *valid = ok;
     return B200POST_OK;
 }
 
 int b200post_vrf_nonce_label(uint32_t provider, uint64_t nonce, const uint8_t node_id[32], const uint8_t commitment_atx_id[32],
                              uint64_t n, uint8_t label32[32]) {
     if (!node_id || !commitment_atx_id || !label32) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    uint8_t commitment[32], all[32];
-    commitment_bytes(node_id, commitment_atx_id, commitment);
-    memset(all, 0xff, 32);
-    b200post_vrf_nonce r;
-    const int rc = b200post_labels_range(provider, commitment, n, nonce, 1, nullptr, all, &r, nullptr);
+    int ok = 0;
+    uint8_t l32[32];
+    // the label does not depend on numLabels: one label suffices for a well-formed check
+    const int rc = vrf_check_one(provider, nonce, node_id, commitment_atx_id, 1, 1, n, &ok, l32);
     if (rc) return rc;
-    if (!r.found) memset(label32, 0xff, 32); else memcpy(label32, r.label32, 32);   // found is 0 only for the all-ones label
+    memcpy(label32, l32, 32);
     return B200POST_OK;
 }
 

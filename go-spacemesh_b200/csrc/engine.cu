@@ -221,6 +221,10 @@ int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n
         CUDA_TRY(cudaMemsetAsync(l.d_cnt.get(), 0, 4, stream_.get()));
         CUDA_TRY(launch_pbkdf2_final_compare(lj, l.X.get(), alloc_slots_, n_slots, l.d_exp.get(), l.d_bits.get(), l.d_cnt.get(),
                                            job.d_diff, d_cta_cand_.get(), stream_.get()));
+    } else if (job.out_hi_dev) {
+        // K3w: both halves of every label32 stay in HBM (gathers of VRF-nonce checks)
+        CUDA_TRY(launch_pbkdf2_final_wide(lj, l.X.get(), alloc_slots_, n_slots, job.out_dev + off * 16, job.out_hi_dev + off * 16,
+                                          stream_.get()));
     } else {
         uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : l.d_out.get();
         CUDA_TRY(launch_pbkdf2_final(lj, l.X.get(), alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_.get(), stream_.get()));
@@ -463,10 +467,12 @@ int DeviceEngine::labels_gather(size_t n_items, const uint8_t *commitments, cons
 }
 
 int DeviceEngine::labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
-                                        const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev) {
+                                        const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev,
+                                        uint8_t *out_hi_dev) {
+    if (out_hi_dev && (!out_dev || out_host)) { set_error("out_hi_dev needs out_dev (and no out_host)"); return B200POST_ERR_INVALID_ARGUMENT; }
     Job job;
     job.gather = true; job.commit_index = commit_index; job.indices = indices; job.total = n_items; job.N = N;
-    job.out_host = out_host; job.out_dev = out_dev;
+    job.out_host = out_host; job.out_dev = out_dev; job.out_hi_dev = out_hi_dev;
     return call(job, [&]() -> int {
         CUDA_TRY(d_ctab_.grow(n_commit * 32));
         CUDA_TRY(cudaMemcpyAsync(d_ctab_.get(), commitments, n_commit * 32, cudaMemcpyHostToDevice, stream_.get()));

@@ -61,9 +61,11 @@ public:
     int labels_gather(size_t n_items, const uint8_t *commitments, const uint64_t *indices, uint64_t N, uint8_t *out_host,
                       uint8_t *out_dev = nullptr);
     // same with the commitments given once (n_commit x 32 bytes) and a per-item row index into them: the verify
-    // path recomputes ~37 labels per identity, so the commitment H2D shrinks by that factor
+    // path recomputes ~37 labels per identity, so the commitment H2D shrinks by that factor.  out_hi_dev (optional, only
+    // with out_dev): device buffer of n_items*16 bytes that gets bytes 16-31 of every label32 (K3w instead of K3)
     int labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
-                              const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev);
+                              const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev,
+                              uint8_t *out_hi_dev = nullptr);
     // compare jobs (K3c): recompute labels and compare them with expect_host (16 bytes per item, in job order) instead of
     // returning them.  Range form: labels [start, start + count), VRF scan as in labels_range.  Indexed form: the labels
     // at `indices` under one commitment.  *cmp is reset by the call; on CANCELLED it holds what was compared so far.
@@ -95,6 +97,7 @@ private:
         VrfResult *vrf = nullptr;
         uint64_t start = 0, total = 0, N = 0;
         uint8_t *out_host = nullptr, *out_dev = nullptr;
+        uint8_t *out_hi_dev = nullptr;          // gather: bytes 16-31 of each label32 (device, with out_dev; K3w)
         const uint32_t *d_diff = nullptr;
         const volatile int *cancel = nullptr;
     };

@@ -393,15 +393,6 @@ __global__ void __launch_bounds__(TPB) romix_pipe_kernel(const PipeParams p) {
 // =================================================================================================
 constexpr int FINAL_TPB = 128;
 
-// lexicographic (label_be[0..7], index) "a < b"
-__device__ __forceinline__ bool cand_less(const uint32_t (&a)[8], uint64_t ai, const uint32_t (&b)[8], uint64_t bi) {
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        if (a[k] != b[k]) return a[k] < b[k];
-    }
-    return ai < bi;
-}
-
 // warp arg-min of (best, best_i) over the lanes with has != 0, by shuffles; every lane ends with the warp's winner
 __device__ __forceinline__ void warp_argmin(uint32_t (&best)[8], uint64_t &best_i, uint32_t &has) {
 #pragma unroll
@@ -494,6 +485,42 @@ __global__ void __launch_bounds__(FINAL_TPB) pbkdf2_final_kernel(LabelJob job, c
     }
     if (vrf_be == nullptr) return;
     cta_vrf_candidate(valid, lab, index, vrf_be, warp_best, cta_cand);
+}
+
+// K3w: K3's label with all 32 bytes kept, for gathers whose items need the whole label32 (VRF-nonce checks).  Bytes
+// 0-15 go to out16 exactly as K3 stores them, bytes 16-31 to out_hi16 at the same item position; each half leaves by
+// its own TMA bulk store.  No VRF-candidate path: a gather has none.
+__global__ void __launch_bounds__(FINAL_TPB) pbkdf2_final_wide_kernel(LabelJob job, const uint4 *__restrict__ X, uint32_t x_stride,
+                                                                      uint32_t n_slots, uint8_t *__restrict__ out16,
+                                                                      uint8_t *__restrict__ out_hi16) {
+    __shared__ __align__(128) uint4 stage_lo[FINAL_TPB];
+    __shared__ __align__(128) uint4 stage_hi[FINAL_TPB];
+    const uint32_t slot = blockIdx.x * FINAL_TPB + threadIdx.x;
+    const bool valid = slot < job.n_valid;
+    uint32_t lab[8];
+    if (slot < n_slots) {
+        uint32_t c[8];
+        load_commit(job, valid ? slot : 0, c);
+        uint32_t lo[16], hi[16];
+#pragma unroll
+        for (int k = 0; k < 8; k++) set_chunk(lo, hi, k, X[(size_t)k * x_stride + slot]);
+        label_final(c, slot_index(job, slot), lo, hi, lab);
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; k++) lab[k] = 0xffffffffu;
+    }
+    stage_lo[threadIdx.x] = make_uint4(bswap32(lab[0]), bswap32(lab[1]), bswap32(lab[2]), bswap32(lab[3]));
+    stage_hi[threadIdx.x] = make_uint4(bswap32(lab[4]), bswap32(lab[5]), bswap32(lab[6]), bswap32(lab[7]));
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t cta_first = blockIdx.x * FINAL_TPB;
+    if (threadIdx.x == 0 && cta_first < job.n_valid) {
+        const uint32_t n_here = min((uint32_t)FINAL_TPB, job.n_valid - cta_first);
+        bulk_s2g(out16 + (size_t)cta_first * 16, smem_u32(stage_lo), n_here * 16);
+        bulk_s2g(out_hi16 + (size_t)cta_first * 16, smem_u32(stage_hi), n_here * 16);
+        bulk_commit();
+        bulk_wait_all<0>();
+    }
 }
 
 // K3c: K3's label, compared with the expected 16 bytes instead of stored (checking stored POST data).  The CTA's
@@ -607,6 +634,13 @@ cudaError_t launch_pbkdf2_final(const LabelJob &job, const uint4 *X, uint32_t x_
     if (n_slots == 0) return cudaSuccess;
     pbkdf2_final_kernel<<<pbkdf2_final_ctas(n_slots), FINAL_TPB, 0, s>>>(job, X, x_stride, n_slots, out16,
                                                                          vrf_difficulty_be, cta_cand);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_pbkdf2_final_wide(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots, uint8_t *out16,
+                                     uint8_t *out_hi16, cudaStream_t s) {
+    if (n_slots == 0) return cudaSuccess;
+    pbkdf2_final_wide_kernel<<<pbkdf2_final_ctas(n_slots), FINAL_TPB, 0, s>>>(job, X, x_stride, n_slots, out16, out_hi16);
     return cudaGetLastError();
 }
 

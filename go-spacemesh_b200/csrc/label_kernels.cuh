@@ -7,7 +7,9 @@
 //   K2 romix_kernel<VARIANT>   X <- ROMix(X) with the ChaCha20/8 BlockMix, the 99.5 % kernel (scrypt step 2)
 //   K3 pbkdf2_final_kernel     X -> label32 (PBKDF2 again); 16-byte labels out via TMA bulk store; VRF candidates
 //   K3c pbkdf2_final_compare_kernel   K3's label compared with expected stored bytes (TMA bulk load): mismatch bitmap + count
+//   K3w pbkdf2_final_wide_kernel      K3's label with both 16-byte halves stored (two TMA bulk stores): VRF-nonce checks
 //   K4 vrf_merge_kernel        per-CTA VRF candidates -> running minimum
+//   K9 vrf_judge_kernel        (vrf_verify.cu) label32 of each VRF-nonce check vs its own threshold: verdict + label32
 //
 // Reference anchors: activation/post.go:295 (Initialize -> labels over a contiguous range),
 // activation/post_verifier.go:159 (Verify -> labels at scattered indices),
@@ -82,7 +84,14 @@ cudaError_t launch_pbkdf2_final(const LabelJob &job, const uint4 *X, uint32_t x_
 cudaError_t launch_pbkdf2_final_compare(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots,
                                         const uint8_t *expect16, uint32_t *mismatch_bits, uint32_t *mismatch_count,
                                         const uint32_t *vrf_difficulty_be, VrfCandidate *cta_cand, cudaStream_t s);
+// K3w: as K3 without the VRF path; out16 gets bytes 0-15 of each label32, out_hi16 bytes 16-31 (both n_valid x 16, device)
+cudaError_t launch_pbkdf2_final_wide(const LabelJob &job, const uint4 *X, uint32_t x_stride, uint32_t n_slots, uint8_t *out16,
+                                     uint8_t *out_hi16, cudaStream_t s);
 cudaError_t launch_vrf_merge(const VrfCandidate *cta_cand, uint32_t n_cta, VrfCandidate *running, cudaStream_t s);
+// K9: item i's label32 = lo16[first + i] || hi16[first + i] (device, K3w's outputs) against threshold_be[i] (8 big-endian
+// words): valid[i] = label32 < threshold (strict), label32_out[i] = the 32 label bytes.  One thread per item.
+cudaError_t launch_vrf_judge(const uint4 *lo16, const uint4 *hi16, uint32_t first, uint32_t n_items, const uint4 *threshold_be,
+                             uint8_t *valid, uint4 *label32_out, cudaStream_t s);
 uint32_t pbkdf2_final_ctas(uint32_t n_slots);
 // bytes of dynamic shared memory the ROMix variant needs per CTA
 size_t romix_smem_bytes(int variant, int tpb);

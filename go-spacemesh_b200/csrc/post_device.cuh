@@ -309,4 +309,16 @@ PD_HD void sha256_iv(uint32_t (&st)[8]) {
     st[4] = 0x510e527f; st[5] = 0x9b05688c; st[6] = 0x1f83d9ab; st[7] = 0x5be0cd19;
 }
 
+// ------------------------------------------------------------------------------------------------
+// VRF order: lexicographic (label_be[0..7], index) "a < b", label32 as eight big-endian words.  With equal indices
+// (0, 0) it is the strict "label32 < threshold" of the VRF-nonce rule (K3's candidates, K4, K9).
+// ------------------------------------------------------------------------------------------------
+PD_HD bool cand_less(const uint32_t (&a)[8], uint64_t ai, const uint32_t (&b)[8], uint64_t bi) {
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        if (a[k] != b[k]) return a[k] < b[k];
+    }
+    return ai < bi;
+}
+
 }  // namespace b200post

@@ -46,10 +46,13 @@ struct Blake3Rng {
     }
 };
 
+// One queue entry: a proof, or (vrf != nullptr) a VRF-nonce check.  Both kinds share the queues and the batch; a
+// VRF check is one label (the one at its nonce), judged by K9 instead of K5, and never reaches the k2pow step.
 struct Job {
-    const b200post_proof *proof;
-    const b200post_proof_metadata *meta;
-    const b200post_verify_params *params;
+    const b200post_proof *proof = nullptr;
+    const b200post_proof_metadata *meta = nullptr;
+    const b200post_verify_params *params = nullptr;
+    const b200post_vrf_check *vrf = nullptr;
     b200post_verify_options opt;
     int status = B200POST_OK;
     uint64_t bad_index = 0;
@@ -66,6 +69,11 @@ struct Job {
     uint64_t diff_lsb = 0;
     uint32_t out_byte = 0;
     size_t first_item = 0;
+    // VRF check: threshold floor(2^256 / numLabels) as big-endian words (filled by prepare()), and the results
+    uint32_t vrf_threshold[8];
+    int vrf_valid = 0;
+    uint8_t label32[32] = {0};
+    uint64_t scrypt_n() const { return vrf ? vrf->scrypt_n : params->scrypt_n; }
 };
 
 }  // namespace
@@ -141,8 +149,24 @@ int b200post_verify_batch_multi(const uint32_t *providers, int n_providers, size
 namespace b200post {
 namespace {
 
+// A VRF check's host part: its numLabels, threshold and commitment; the one label to recompute is at the nonce.  The
+// nonce is not range-checked: a nonce >= numLabels is what the past-the-end search produces.
+void prepare_vrf(Job &j) {
+    const b200post_vrf_check &c = *j.vrf;
+    j.status = B200POST_OK;
+    const unsigned __int128 nl = (unsigned __int128)c.num_units * c.labels_per_unit;
+    if (nl == 0 || nl > ~0ull) { j.status = B200POST_ERR_INVALID_ARGUMENT; return; }
+    uint8_t diff[32];
+    vrf_difficulty((uint64_t)nl, diff);
+    for (int k = 0; k < 8; k++)
+        j.vrf_threshold[k] = ((uint32_t)diff[4 * k] << 24) | ((uint32_t)diff[4 * k + 1] << 16) | ((uint32_t)diff[4 * k + 2] << 8) | diff[4 * k + 3];
+    commitment_bytes(c.node_id, c.commitment_atx_id, j.commitment);
+    j.check.assign(1, c.nonce);
+}
+
 // Per-proof checks that need no labels; fills job.check with the label indices to recompute.
 void prepare(Job &j, const b200post_verifier_opts &vo) {
+    if (j.vrf) { prepare_vrf(j); return; }
     const b200post_proof &p = *j.proof;
     const b200post_proof_metadata &m = *j.meta;
     const b200post_verify_params &q = *j.params;
@@ -280,6 +304,20 @@ struct JudgeScratch {
     DeviceBuffer<uint32_t> item_job, first_bad;
     DeviceBuffer<DevJob> jobs;
     DeviceBuffer<AesTables> tables;
+    // VRF checks: the high label halves of the gather (K3w), and per check the threshold, K9's verdict and label32
+    DeviceBuffer<uint4> labels_hi, vrf_threshold, vrf_label;
+    DeviceBuffer<uint8_t> vrf_valid;
+    int reserve_vrf(size_t n_items, size_t n_vrf) {
+        if (n_items > labels_hi.size()) CUDA_TRY(labels_hi.resize(n_items + n_items / 4));
+        if (n_vrf > vrf_valid.size()) {   // vrf_valid is allocated last: its size is the capacity of all three
+            vrf_valid.reset();
+            const size_t c = n_vrf + n_vrf / 4;
+            CUDA_TRY(vrf_threshold.resize(2 * c));
+            CUDA_TRY(vrf_label.resize(2 * c));
+            CUDA_TRY(vrf_valid.resize(c));
+        }
+        return B200POST_OK;
+    }
     int reserve(size_t n_items, size_t n_jobs, const AesTables &host_tables) {
         if (!tables.get()) {
             CUDA_TRY(tables.resize(1));
@@ -309,17 +347,24 @@ JudgeScratch &judge_scratch(uint32_t provider) {
     return *s;
 }
 
-// `indices` holds every checked label index of the batch, job after job (Job::first_item); each job's commitment is
-// uploaded once and items refer to it by row (DeviceEngine::labels_gather_indexed).
-int gather_and_judge(uint32_t provider, std::vector<Job *> &jobs, uint64_t n, const std::vector<uint64_t> &indices,
-                     std::vector<uint32_t> &first_bad) {
+// `indices` holds every checked label index of the batch, proof after proof, then one per VRF check (Job::first_item);
+// each job's commitment is uploaded once and items refer to it by row (DeviceEngine::labels_gather_indexed): the
+// proofs' rows first, so that a proof item's row is also its DevJob.  K5 judges the proof items; when VRF checks are
+// present the gather keeps both label halves (K3w) and K9 judges the checks, whose results land in their jobs.
+int gather_and_judge(uint32_t provider, const std::vector<Job *> &live, const std::vector<Job *> &vrfs, uint64_t n,
+                     const std::vector<uint64_t> &indices, std::vector<uint32_t> &first_bad) {
     DeviceEngine *e = engine_for(provider);
     if (!e) return B200POST_ERR_NO_DEVICE;
-    std::vector<Job *> live;
-    for (Job *j : jobs) if (j->status == B200POST_OK && j->params->scrypt_n == n) live.push_back(j);
     std::vector<DevJob> dj(live.size());
-    std::vector<uint8_t> commitments(live.size() * 32);
+    std::vector<uint8_t> commitments((live.size() + vrfs.size()) * 32);
     std::vector<uint32_t> item_job(indices.size());
+    std::vector<uint32_t> thresholds(vrfs.size() * 8);
+    for (size_t v = 0; v < vrfs.size(); v++) {
+        const size_t row = live.size() + v;
+        memcpy(&commitments[row * 32], vrfs[v]->commitment, 32);
+        item_job[vrfs[v]->first_item] = (uint32_t)row;
+        memcpy(&thresholds[v * 8], vrfs[v]->vrf_threshold, 32);
+    }
     parallel_for(live.size(), [&](size_t i) {
         Job *j = live[i];
         DevJob &d = dj[i];
@@ -339,21 +384,39 @@ int gather_and_judge(uint32_t provider, std::vector<Job *> &jobs, uint64_t n, co
     std::call_once(once, [] { aes_build_tables(host_tables); });
 
     const uint32_t n_items = (uint32_t)indices.size();
+    const uint32_t n_vrf = (uint32_t)vrfs.size(), n_proof_items = n_items - n_vrf;
     CUDA_TRY(cudaSetDevice(e->device()));
     JudgeScratch &s = judge_scratch(provider);
     std::lock_guard<std::mutex> lk(s.mu);
     int rc = s.reserve(n_items, dj.size(), host_tables);
+    if (rc == B200POST_OK && n_vrf) rc = s.reserve_vrf(n_items, n_vrf);
     if (rc != B200POST_OK) return rc;
     CUDA_TRY(cudaMemcpy(s.item_job.get(), item_job.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemcpy(s.jobs.get(), dj.data(), dj.size() * sizeof(DevJob), cudaMemcpyHostToDevice));
     CUDA_TRY(cudaMemset(s.first_bad.get(), 0xff, dj.size() * 4));
-    rc = e->labels_gather_indexed(indices.size(), dj.size(), commitments.data(), item_job.data(), indices.data(), n, nullptr,
-                                  reinterpret_cast<uint8_t *>(s.labels.get()));
+    if (n_vrf) CUDA_TRY(cudaMemcpy(s.vrf_threshold.get(), thresholds.data(), thresholds.size() * 4, cudaMemcpyHostToDevice));
+    rc = e->labels_gather_indexed(indices.size(), live.size() + n_vrf, commitments.data(), item_job.data(), indices.data(), n, nullptr,
+                                  reinterpret_cast<uint8_t *>(s.labels.get()),
+                                  n_vrf ? reinterpret_cast<uint8_t *>(s.labels_hi.get()) : nullptr);
     if (rc != B200POST_OK) return rc;
-    verify_judge_kernel<<<(n_items + 255) / 256, 256, AES_SMEM_BYTES>>>(s.labels.get(), s.item_job.get(), s.jobs.get(), n_items,
-                                                                        s.tables.get(), s.first_bad.get());
-    g_launches += 1;
-    CUDA_TRY(cudaGetLastError());
+    if (n_proof_items) {
+        verify_judge_kernel<<<(n_proof_items + 255) / 256, 256, AES_SMEM_BYTES>>>(s.labels.get(), s.item_job.get(), s.jobs.get(),
+                                                                                  n_proof_items, s.tables.get(), s.first_bad.get());
+        g_launches += 1;
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (n_vrf) {
+        CUDA_TRY(launch_vrf_judge(s.labels.get(), s.labels_hi.get(), n_proof_items, n_vrf, s.vrf_threshold.get(), s.vrf_valid.get(),
+                                  s.vrf_label.get(), 0));
+        g_launches += 1;
+        std::vector<uint8_t> valid(n_vrf), label32((size_t)n_vrf * 32);
+        CUDA_TRY(cudaMemcpy(valid.data(), s.vrf_valid.get(), n_vrf, cudaMemcpyDeviceToHost));
+        CUDA_TRY(cudaMemcpy(label32.data(), s.vrf_label.get(), label32.size(), cudaMemcpyDeviceToHost));
+        for (uint32_t v = 0; v < n_vrf; v++) {
+            vrfs[v]->vrf_valid = valid[v];
+            memcpy(vrfs[v]->label32, &label32[(size_t)v * 32], 32);
+        }
+    }
     CUDA_TRY(cudaMemcpy(first_bad.data(), s.first_bad.get(), dj.size() * 4, cudaMemcpyDeviceToHost));
     return B200POST_OK;
 }
@@ -365,9 +428,10 @@ int process(uint32_t provider, std::vector<Job *> &jobs, const b200post_verifier
     else parallel_for(jobs.size(), [&](size_t i) { prepare(*jobs[i], vo); });
     if (vo.pow_mode == B200POST_POW_BUILTIN) {
         // the k2pow check of verifying.ProofVerifier.Verify (activation/post_verifier.go:150-160): one RandomX hash per
-        // proof, all proofs of the batch in one device batch
+        // proof, all proofs of the batch in one device batch.  VRF checks have no pow: a batch of only VRF checks never
+        // touches the RandomX engine (nor builds its dataset).
         std::vector<Job *> live;
-        for (Job *j : jobs) if (j->status == B200POST_OK) live.push_back(j);
+        for (Job *j : jobs) if (j->status == B200POST_OK && !j->vrf) live.push_back(j);
         if (!live.empty()) {
             std::vector<uint8_t> in(live.size() * 48), out(live.size() * 32);
             for (size_t i = 0; i < live.size(); i++) memcpy(&in[i * 48], live[i]->pow_input, 48);
@@ -387,23 +451,32 @@ int process(uint32_t provider, std::vector<Job *> &jobs, const b200post_verifier
         metrics().verify_gather_judge_us_total += (uint64_t)std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now() - from).count(); } } stage{t1};
     std::vector<uint64_t> ns;
     for (Job *j : jobs)
-        if (j->status == B200POST_OK && std::find(ns.begin(), ns.end(), j->params->scrypt_n) == ns.end()) ns.push_back(j->params->scrypt_n);
+        if (j->status == B200POST_OK && std::find(ns.begin(), ns.end(), j->scrypt_n()) == ns.end()) ns.push_back(j->scrypt_n());
     for (uint64_t n : ns) {
-        std::vector<uint64_t> indices;
+        // one gather per N: the proofs' labels, then one label per VRF check
+        std::vector<Job *> live, vrfs;
         size_t total = 0;
-        for (Job *j : jobs) if (j->status == B200POST_OK && j->params->scrypt_n == n) total += j->check.size();
-        indices.reserve(total);
         for (Job *j : jobs) {
-            if (j->status != B200POST_OK || j->params->scrypt_n != n) continue;
+            if (j->status != B200POST_OK || j->scrypt_n() != n) continue;
+            (j->vrf ? vrfs : live).push_back(j);
+            total += j->check.size();
+        }
+        std::vector<uint64_t> indices;
+        indices.reserve(total);
+        for (Job *j : live) {
             j->first_item = indices.size();
             indices.insert(indices.end(), j->check.begin(), j->check.end());
         }
+        for (Job *j : vrfs) {
+            j->first_item = indices.size();
+            indices.push_back(j->check[0]);
+        }
         int rc = B200POST_ERR_INVALID_ARGUMENT;
         std::vector<uint32_t> first_bad;
-        if (n >= 2 && n <= (1ull << 20) && (n & (n - 1)) == 0) rc = gather_and_judge(provider, jobs, n, indices, first_bad);
+        if (n >= 2 && n <= (1ull << 20) && (n & (n - 1)) == 0) rc = gather_and_judge(provider, live, vrfs, n, indices, first_bad);
+        for (Job *j : vrfs) if (rc != B200POST_OK) j->status = rc;
         size_t k = 0;
-        for (Job *j : jobs) {
-            if (j->status != B200POST_OK || j->params->scrypt_n != n) continue;
+        for (Job *j : live) {
             if (rc != B200POST_OK) j->status = rc;
             else if (first_bad[k] != 0xffffffffu) {
                 // verifying.ErrInvalidIndex{Index}: the POSITION in the proof's K2 list (activation/handler_v1.go:248 stores it as
@@ -454,7 +527,8 @@ struct b200post_verifier {
             lk.unlock();
             process(provider, batch, opts);
             lk.lock();
-            batches++; proofs += batch.size();
+            batches++;
+            for (Job *j : batch) proofs += j->vrf ? 0 : 1;   // VRF checks are not proofs
             metrics().verify_batches_total++;
             for (Job *j : batch) j->done = true;
             cv_done.notify_all();
@@ -523,6 +597,27 @@ int b200post_verifier_verify(b200post_verifier *v, const b200post_proof *proof, 
     return j.status;
 }
 
+int b200post_verifier_verify_vrf_nonce(b200post_verifier *v, const b200post_vrf_check *c, int *valid, uint8_t label32[32]) {
+    if (!v || !c || !valid) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    *valid = 0;
+    Job j;
+    j.vrf = c;
+    memset(&j.opt, 0, sizeof j.opt);
+    {
+        std::unique_lock<std::mutex> lk(v->mu);
+        if (v->closed) { set_error("verifier is closed"); return B200POST_ERR_CLOSED; }
+        (c->prioritized ? v->prioritized : v->normal).push_back(&j);
+        v->cv_work.notify_one();
+        v->cv_done.wait(lk, [&] { return j.done; });
+    }
+    if (j.status == B200POST_ERR_CLOSED) set_error("verifier is closed");
+    else if (j.status == B200POST_ERR_INVALID_ARGUMENT) set_error("malformed VRF check (num_units * labels_per_unit or scrypt N)");
+    if (j.status != B200POST_OK) return j.status;
+    *valid = j.vrf_valid;
+    if (label32) memcpy(label32, j.label32, 32);
+    return B200POST_OK;
+}
+
 int b200post_verifier_close(b200post_verifier *v) {
     if (!v) return B200POST_ERR_INVALID_ARGUMENT;
     {
@@ -574,6 +669,57 @@ int b200post_verify_batch(uint32_t provider, size_t n, const b200post_proof *pro
         statuses[i] = jobs[i].status;
         if (invalid_indices) invalid_indices[i] = jobs[i].bad_index;
     }
+    return B200POST_OK;
+}
+
+int b200post_verify_vrf_nonces(uint32_t provider, size_t n, const b200post_vrf_check *checks, int *statuses, int *valid,
+                               uint8_t *labels32) {
+    if (n && (!checks || !statuses || !valid)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    if (!engine_for(provider)) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (n == 0) return B200POST_OK;
+    std::vector<Job> jobs(n);
+    std::vector<Job *> ptrs(n);
+    for (size_t i = 0; i < n; i++) {
+        jobs[i].vrf = &checks[i];
+        memset(&jobs[i].opt, 0, sizeof jobs[i].opt);
+        ptrs[i] = &jobs[i];
+    }
+    b200post_verifier_opts vo{};
+    vo.pow_mode = B200POST_POW_SKIP;   // VRF checks have no pow; nothing reads it
+    process(provider, ptrs, vo);
+    metrics().verify_batches_total++;
+    for (size_t i = 0; i < n; i++) {
+        statuses[i] = jobs[i].status;
+        valid[i] = jobs[i].status == B200POST_OK ? jobs[i].vrf_valid : 0;
+        if (labels32) {
+            if (jobs[i].status == B200POST_OK) memcpy(labels32 + 32 * i, jobs[i].label32, 32);
+            else memset(labels32 + 32 * i, 0, 32);
+        }
+    }
+    return B200POST_OK;
+}
+
+int b200post_verify_vrf_nonces_multi(const uint32_t *providers, int n_providers, size_t n, const b200post_vrf_check *checks,
+                                     int *statuses, int *valid, uint8_t *labels32) {
+    if (!providers || n_providers <= 0 || (n && (!checks || !statuses || !valid))) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    for (int d = 0; d < n_providers; d++)
+        if (!engine_for(providers[d])) return providers[d] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (n_providers == 1 || n < 2) return b200post_verify_vrf_nonces(providers[0], n, checks, statuses, valid, labels32);
+    const size_t parts = std::min<size_t>((size_t)n_providers, n);
+    std::vector<int> rcs(parts, B200POST_OK);
+    std::vector<std::string> errs(parts);
+    std::vector<std::thread> th;
+    for (size_t d = 0; d < parts; d++) {
+        const size_t lo = n * d / parts, hi = n * (d + 1) / parts;
+        th.emplace_back([=, &rcs, &errs] {
+            rcs[d] = b200post_verify_vrf_nonces(providers[d], hi - lo, checks + lo, statuses + lo, valid + lo,
+                                                labels32 ? labels32 + 32 * lo : nullptr);
+            if (rcs[d] != B200POST_OK) errs[d] = b200post_last_error();   // the error text is thread-local
+        });
+    }
+    for (auto &t : th) t.join();
+    for (size_t d = 0; d < parts; d++)
+        if (rcs[d] != B200POST_OK) { set_error(errs[d]); return rcs[d]; }
     return B200POST_OK;
 }
 

@@ -297,6 +297,97 @@ func (v *Verifier) Verify(p *Proof, m *ProofMetadata, k1, k2 uint32, powDifficul
 
 func (v *Verifier) Close() error { C.b200post_verifier_close(v.h); return nil }
 
+// VRFCheck is shared.VRFNonceMetadata plus the nonce (activation/validation.go:261-285).
+type VRFCheck struct {
+	NodeId, CommitmentAtxId []byte
+	Nonce                   uint64
+	NumUnits                uint32
+	LabelsPerUnit           uint64
+	ScryptN                 uint64
+	Prioritized             bool // PrioritizedCall(); used by Verifier.VerifyVRFNonce
+}
+
+// VRFResult is one check's outcome.  Valid is label32 < floor(2^256 / numLabels): the UNPINNED rule of
+// b200post_verify_vrf_nonce, which real network data contradicts as a universal rule (include/b200post.h).  Label is
+// the label32 at the nonce, for the rule the network uses.  Err is set for a malformed check only.
+type VRFResult struct {
+	Valid bool
+	Label [32]byte
+	Err   error
+}
+
+func (c *VRFCheck) cCheck() (cc C.b200post_vrf_check, err error) {
+	if len(c.NodeId) != 32 || len(c.CommitmentAtxId) != 32 {
+		return cc, errors.New("b200post: node id and commitment ATX id must be 32 bytes")
+	}
+	C.memcpy(unsafe.Pointer(&cc.node_id[0]), unsafe.Pointer(&c.NodeId[0]), 32)
+	C.memcpy(unsafe.Pointer(&cc.commitment_atx_id[0]), unsafe.Pointer(&c.CommitmentAtxId[0]), 32)
+	cc.nonce, cc.num_units, cc.labels_per_unit, cc.scrypt_n = C.uint64_t(c.Nonce), C.uint32_t(c.NumUnits), C.uint64_t(c.LabelsPerUnit), C.uint64_t(c.ScryptN)
+	if c.Prioritized {
+		cc.prioritized = 1
+	}
+	return cc, nil
+}
+
+// VerifyVRFNonce = Validator.VRFNonce / VRFNonceV2 through the verifier's dispatcher: blocking, safe for concurrent
+// use, coalesced with concurrent proofs into one GPU gather.  See VRFResult for what valid and label mean.
+func (v *Verifier) VerifyVRFNonce(c *VRFCheck) (valid bool, label [32]byte, err error) {
+	cc, err := c.cCheck()
+	if err != nil {
+		return false, label, err
+	}
+	var ok C.int
+	var cl [32]C.uint8_t
+	rc, msg := checked(func() C.int { return C.b200post_verifier_verify_vrf_nonce(v.h, &cc, &ok, &cl[0]) })
+	switch rc {
+	case C.B200POST_OK:
+		for i := range label {
+			label[i] = byte(cl[i])
+		}
+		return ok != 0, label, nil
+	case C.B200POST_ERR_CLOSED:
+		return false, label, ErrVerifierClosed
+	default:
+		return false, label, statusErr(rc, msg)
+	}
+}
+
+// VerifyVRFNonces runs many checks in one GPU batch on the calling goroutine, split over `providers` in contiguous
+// runs (one device: []uint32{id}).  Results are in the order of `checks`; a malformed check (numLabels 0 or above
+// 2^64-1, scrypt N not a power of two in [2, 2^20]) gets its own Err and leaves the others alone.
+func VerifyVRFNonces(providers []uint32, checks []VRFCheck) ([]VRFResult, error) {
+	if len(providers) == 0 {
+		return nil, errors.New("b200post: no providers")
+	}
+	n := len(checks)
+	out := make([]VRFResult, n)
+	cs := make([]C.b200post_vrf_check, n+1) // C structs without Go pointers; one spare so that &cs[0] exists for n == 0
+	for i := range checks {
+		cc, err := checks[i].cCheck()
+		if err != nil {
+			return nil, err
+		}
+		cs[i] = cc
+	}
+	statuses, valid := make([]C.int, n+1), make([]C.int, n+1)
+	labels := make([]byte, 32*(n+1))
+	rc, msg := checked(func() C.int {
+		return C.b200post_verify_vrf_nonces_multi((*C.uint32_t)(unsafe.Pointer(&providers[0])), C.int(len(providers)), C.size_t(n),
+			&cs[0], &statuses[0], &valid[0], (*C.uint8_t)(unsafe.Pointer(&labels[0])))
+	})
+	if err := statusErr(rc, msg); err != nil {
+		return nil, err
+	}
+	for i := range out {
+		out[i].Valid = valid[i] != 0
+		copy(out[i].Label[:], labels[32*i:32*i+32])
+		if statuses[i] != C.B200POST_OK {
+			out[i].Err = statusErr(statuses[i], "malformed VRF check (num_units * labels_per_unit or scrypt N)")
+		}
+	}
+	return out, nil
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Proof generation scan (the AES half of PostClient.Proof, activation/interface.go:204-207)
 // ---------------------------------------------------------------------------------------------------------

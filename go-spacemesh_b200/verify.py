@@ -11,7 +11,7 @@ from __future__ import annotations
 import ctypes
 from dataclasses import dataclass, field
 
-from . import B200PostError, ERR_CLOSED, ERR_EMPTY_PROOF, ERR_INVALID_PROOF, OK, lib
+from . import B200PostError, ERR_CLOSED, ERR_EMPTY_PROOF, ERR_INVALID_PROOF, OK, VrfCheck, lib, vrf_check
 
 MODE_ALL, MODE_SUBSET, MODE_SELECTED_INDEX = 0, 1, 2
 
@@ -111,6 +111,7 @@ def _bind():
     L.b200post_verifier_new_multi.argtypes = [ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_VerifierOpts), ctypes.POINTER(vp)]
     L.b200post_verifier_verify.argtypes = [vp, ctypes.POINTER(_Proof), ctypes.POINTER(_Meta), ctypes.POINTER(_Params),
                                            ctypes.POINTER(_Options), ctypes.POINTER(ctypes.c_uint64)]
+    L.b200post_verifier_verify_vrf_nonce.argtypes = [vp, ctypes.POINTER(VrfCheck), ctypes.POINTER(ctypes.c_int), vp]
     L.b200post_verifier_close.argtypes = [vp]
     L.b200post_verifier_free.argtypes = [vp]
     L.b200post_verifier_free.restype = None
@@ -211,6 +212,18 @@ class PostVerifier:
         rc = _bind().b200post_verifier_verify(self._h, ctypes.byref(cp), ctypes.byref(cm), ctypes.byref(cq),
                                               ctypes.byref(co), ctypes.byref(bad))
         _raise(rc, bad.value)
+
+    def verify_vrf_nonce(self, node_id: bytes, atx: bytes, nonce: int, num_units: int, labels_per_unit: int, n: int = 8192, *,
+                         prioritized: bool = False) -> tuple[bool, bytes]:
+        """Validator.VRFNonce / VRFNonceV2 through this verifier's dispatcher, coalesced with concurrent proofs.
+        Returns (valid, label32): valid = label32 < floor(2^256 / numLabels), the UNPINNED rule of verify_vrf_nonce;
+        label32 = the label at the nonce, for the network's own rule."""
+        c = vrf_check(node_id, atx, nonce, num_units, labels_per_unit, n, prioritized=prioritized)
+        ok = ctypes.c_int(0)
+        label = ctypes.create_string_buffer(32)
+        rc = _bind().b200post_verifier_verify_vrf_nonce(self._h, ctypes.byref(c), ctypes.byref(ok), label)
+        _raise(rc, 0)
+        return bool(ok.value), label.raw
 
     def stats(self) -> tuple[int, int]:
         b, p = ctypes.c_uint64(0), ctypes.c_uint64(0)

@@ -140,7 +140,9 @@ void b200post_vrf_difficulty(uint64_t num_labels, uint8_t out[32]);
  * universal rule: 16 of its 42 recorded, network-accepted nonces are the arg-min of their POST yet lie above that
  * threshold (tests/golden/checkpoint_vrf.json, tests/test_gpu_labels.py lists them).  Do not wire this into
  * Validator.VRFNonce (activation/validation.go:261-282) before checking the rule against libpost; until then use
- * b200post_vrf_nonce_label and apply the rule the network uses. */
+ * b200post_vrf_nonce_label and apply the rule the network uses.
+ * This call and b200post_vrf_nonce_label below are the one-check case of b200post_verify_vrf_nonces (include/b200post_verify.h), which checks many nonces in
+ * one GPU batch and returns the label32 with each verdict. */
 int b200post_verify_vrf_nonce(uint32_t provider, uint64_t nonce, const uint8_t node_id[32],
                               const uint8_t commitment_atx_id[32], uint32_t num_units,
                               uint64_t labels_per_unit, uint64_t n, int *valid);

@@ -124,6 +124,45 @@ int b200post_verify_batch_multi(const uint32_t *providers, int n_providers, size
                                 const b200post_verify_options *options /* n or NULL */, const b200post_verifier_opts *opts,
                                 int *statuses, uint64_t *invalid_indices);
 
+/* ---------------------------------------------------------------------------------------------------------------
+ * VRF-nonce checks in batches.  Validator.VRFNonce / VRFNonceV2 (activation/validation.go:261-285, called by
+ * activation/handler_v2.go on every non-initial V2 ATX and by handler_v1.go on initial ATXs) recompute ONE label per
+ * check: the label at the nonce.  These calls put many checks into one GPU gather, and the verifier handle coalesces
+ * them with concurrent proofs (one gather per scrypt N; the checks' labels follow the proofs' labels).
+ *
+ * PARITY: *valid / valid[i] is label32 < floor(2^256 / numLabels), strict — the UNPINNED rule of
+ * b200post_verify_vrf_nonce, which real network data contradicts as a universal rule (see include/b200post.h).  The
+ * label32 at the nonce comes back with it, so that a caller can apply the rule the network uses.
+ *
+ * A check never reaches the k2pow step, is not counted as a proof (b200post_verifier_stats' proofs, the verify
+ * metrics), and counts as one entry toward max_batch_proofs.  Per-check argument errors (num_units * labels_per_unit
+ * 0 or above 2^64-1, scrypt N not a power of two in [2, 2^20]) give that check B200POST_ERR_INVALID_ARGUMENT and leave
+ * the others alone.  The nonce is not range-checked: a nonce >= numLabels is what the past-the-end search produces.
+ * --------------------------------------------------------------------------------------------------------------- */
+typedef struct b200post_vrf_check {        /* shared.VRFNonceMetadata + nonce: activation/validation.go:261-285 */
+    uint8_t node_id[32];
+    uint8_t commitment_atx_id[32];
+    uint64_t nonce;
+    uint64_t labels_per_unit;
+    uint64_t scrypt_n;                     /* r = p = 1 */
+    uint32_t num_units;
+    uint32_t prioritized;                  /* verifier only: PrioritizedCall */
+} b200post_vrf_check;
+
+/* Validator.VRFNonce / VRFNonceV2 through the verifier's dispatcher: blocking, safe for concurrent use, coalesced with
+ * concurrent proofs.  B200POST_OK with *valid = label32 < floor(2^256 / numLabels) (the UNPINNED rule of
+ * b200post_verify_vrf_nonce), label32 (may be NULL) = the label at the nonce; INVALID_ARGUMENT, CLOSED or an engine error. */
+int b200post_verifier_verify_vrf_nonce(b200post_verifier *v, const b200post_vrf_check *c, int *valid, uint8_t label32[32]);
+
+/* n checks in one GPU batch on the calling thread; statuses[i] per item, valid[i] 0/1, labels32 = n x 32 bytes or NULL.
+ * Call-level checks, in this order: NULL pointers with n > 0 -> INVALID_ARGUMENT, the CPU provider id -> UNSUPPORTED,
+ * no such device -> NO_DEVICE (no fallback), n == 0 -> OK.  A failed item gets valid 0 and a zero label32. */
+int b200post_verify_vrf_nonces(uint32_t provider, size_t n, const b200post_vrf_check *checks, int *statuses, int *valid,
+                               uint8_t *labels32);
+/* the same split over devices: contiguous runs, one host thread each, results in the caller's order */
+int b200post_verify_vrf_nonces_multi(const uint32_t *providers, int n_providers, size_t n, const b200post_vrf_check *checks,
+                                     int *statuses, int *valid, uint8_t *labels32);
+
 /* Helpers shared with the Go side (all ASSUMED post-rs conventions, see PARITY NOTE). */
 uint32_t b200post_bits_per_index(uint64_t num_labels);                       /* floor(log2(num_labels)) + 1       */
 uint64_t b200post_proving_difficulty(uint32_t k1, uint64_t num_labels);      /* floor(2^64 * k1 / num_labels)      */
