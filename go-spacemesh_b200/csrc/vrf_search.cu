@@ -5,8 +5,8 @@
 // The arg-min of label32 (big-endian) is decided by its first 16 bytes, and those are exactly what postdata_N.bin
 // holds.  So instead of recomputing every label (ROMix speed), the files are streamed through the GPU at 16 B per label
 // (storage speed): a reader thread fills pinned staging one chunk ahead, the H2D copy runs on its own stream, and per
-// chunk K8 reduces the chunk to one small record (lowest prefix, its lowest position, and up to 64 positions holding
-// it).  The host folds the records; only the positions at the final lowest prefix have their label32 recomputed.
+// chunk K8 reduces the chunk to one small record (lowest prefix, its two lowest positions, how many hold it).  The host
+// folds the records; only the two lowest positions at the final lowest prefix have their label32 recomputed.
 #include <algorithm>
 #include <cstring>
 #include <future>
@@ -25,7 +25,6 @@
 namespace b200post {
 namespace {
 
-constexpr uint32_t kMaxTies = 64;
 constexpr uint64_t kMaxChunk = 1ull << 26;   // 1 GiB of staging per buffer
 constexpr int kTpb = 256;
 
@@ -37,7 +36,7 @@ struct ChunkMin {
     uint64_t hi, lo;          // the smallest stored 16-byte prefix of the chunk
     uint32_t index;           // its lowest position in the chunk
     uint32_t n_ties;          // positions holding that prefix, all of them counted
-    uint32_t ties[kMaxTies];  // up to kMaxTies of those positions, in no particular order
+    uint32_t next;            // the lowest of them above index (~0u: none)
 };
 
 struct CtaMin { uint64_t hi, lo; uint32_t index, pad; };
@@ -75,15 +74,16 @@ __device__ __forceinline__ void cta_argmin(uint64_t &h, uint64_t &l, uint32_t &i
 }
 
 // K8a: arg-min of the chunk's stored prefixes (lowest position on ties).  Each thread keeps its own minimum over a
-// grid-stride walk (positions ascend per thread, so a strict comparison keeps the lowest); each CTA writes one
-// partial; the last CTA to finish reduces the partials into the chunk's record and re-arms the counter.
+// grid-stride walk (positions ascend per thread, so a strict comparison keeps the lowest; a thread's first label is
+// always taken, so an all-ones prefix gets its real position, not the empty ~0u); each CTA writes one partial; the
+// last CTA to finish reduces the partials into the chunk's record and re-arms the counter.
 __global__ void __launch_bounds__(kTpb) stored_min_kernel(const uint4 *__restrict__ labels, uint32_t count, CtaMin *__restrict__ partial,
                                                          uint32_t *__restrict__ done, ChunkMin *__restrict__ rec) {
     uint64_t h = ~0ull, l = ~0ull;
     uint32_t idx = ~0u;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
         const Key k = load_key(__ldcs(labels + i));
-        if (k.hi < h || (k.hi == h && k.lo < l)) { h = k.hi; l = k.lo; idx = i; }
+        if (idx == ~0u || k.hi < h || (k.hi == h && k.lo < l)) { h = k.hi; l = k.lo; idx = i; }
     }
     cta_argmin(h, l, idx);
     __shared__ bool last;
@@ -103,20 +103,22 @@ __global__ void __launch_bounds__(kTpb) stored_min_kernel(const uint4 *__restric
     }
     cta_argmin(h, l, idx);
     if (threadIdx.x == 0) {
-        rec->hi = h; rec->lo = l; rec->index = idx; rec->n_ties = 0;
+        rec->hi = h; rec->lo = l; rec->index = idx; rec->n_ties = 0; rec->next = ~0u;
         *done = 0;
     }
 }
 
-// K8b: a second pass over the same device-resident chunk collects the positions whose prefix equals the minimum
-// (two distinct real labels cannot share 128 bits, so more than one means damaged data)
+// K8b: a second pass over the same device-resident chunk counts the positions whose prefix equals the minimum and keeps
+// the lowest above K8a's index (two distinct real labels cannot share 128 bits, so more than one means damaged data:
+// index is damaged, or index holds the real label and next is the lowest copy of it)
 __global__ void __launch_bounds__(kTpb) stored_tie_kernel(const uint4 *__restrict__ labels, uint32_t count, ChunkMin *__restrict__ rec) {
     const uint64_t mh = rec->hi, ml = rec->lo;
+    const uint32_t first = rec->index;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < count; i += gridDim.x * blockDim.x) {
         const Key k = load_key(__ldcs(labels + i));
         if (k.hi == mh && k.lo == ml) {
-            const uint32_t slot = atomicAdd(&rec->n_ties, 1u);
-            if (slot < kMaxTies) rec->ties[slot] = i;
+            atomicAdd(&rec->n_ties, 1u);
+            if (i != first) atomicMin(&rec->next, i);
         }
     }
 }
@@ -194,17 +196,21 @@ private:
     Event copied_[2], scanned_[2];
 };
 
-// the running minimum across chunks and files
+// the running minimum across chunks and files; next is the lowest position at the prefix above index (~0: none)
 struct Running {
     bool any = false;
-    uint64_t hi = 0, lo = 0, index = 0, n_ties = 0;
-    std::vector<uint64_t> ties;
+    uint64_t hi = 0, lo = 0, index = 0, next = ~0ull, n_ties = 0;
     void fold(const ChunkMin &r, uint64_t first) {
         const bool less = !any || r.hi < hi || (r.hi == hi && r.lo < lo);
-        if (less) { any = true; hi = r.hi; lo = r.lo; index = first + r.index; n_ties = 0; ties.clear(); }
-        else if (r.hi != hi || r.lo != lo) return;
+        if (less) {
+            any = true; hi = r.hi; lo = r.lo; index = first + r.index; n_ties = 0;
+            next = r.next == ~0u ? ~0ull : first + r.next;
+        } else if (r.hi != hi || r.lo != lo) {
+            return;
+        } else {
+            next = std::min(next, first + r.index);   // chunks arrive in ascending order: above index
+        }
         n_ties += r.n_ties;
-        for (uint32_t j = 0; j < std::min<uint32_t>(r.n_ties, kMaxTies) && ties.size() < kMaxTies; j++) ties.push_back(first + r.ties[j]);
     }
 };
 
@@ -278,13 +284,12 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
         if (o.progress) __atomic_fetch_add(o.progress, count_of(n_chunks - 1), __ATOMIC_RELAXED);
     }
 
-    // ---- the label32 of every position at the lowest prefix, recomputed; a stored prefix it does not reproduce is damage
+    // ---- the label32 of the two lowest positions at the lowest prefix, recomputed; a stored prefix it does not reproduce
+    // is damage.  index first: if it is damaged it is the lowest damaged position, else next is the lowest copy of it.
     uint8_t prefix[16];
     for (int j = 0; j < 8; j++) { prefix[j] = (uint8_t)(best.hi >> (56 - 8 * j)); prefix[8 + j] = (uint8_t)(best.lo >> (56 - 8 * j)); }
-    std::vector<uint64_t> pos = best.ties;
-    pos.push_back(best.index);
-    std::sort(pos.begin(), pos.end());
-    pos.erase(std::unique(pos.begin(), pos.end()), pos.end());
+    std::vector<uint64_t> pos{best.index};
+    if (best.next != ~0ull) pos.push_back(best.next);
     uint8_t commitment[32], all[32], best32[32];
     commitment_bytes(md->node_id, md->commitment_atx_id, commitment);
     memset(all, 0xff, 32);

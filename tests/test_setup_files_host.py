@@ -151,6 +151,57 @@ def stored_argmin_rule(orc, stored: np.ndarray, commitment: bytes, n: int, num_l
     return (i, l32) if l32 < orc.py_vrf_difficulty(num_labels) else None
 
 
+def _py_stored_argmin(stored: np.ndarray):
+    keys = [bytes(r) for r in stored]
+    low = min(keys)
+    ties = [i for i, k in enumerate(keys) if k == low]
+    return ties[0], ties
+
+
+def _planted(rng, n, rows):
+    """n random rows whose first byte is at least 1, with `rows` (16-byte strings) planted at distinct random positions."""
+    a = rng.integers(0, 256, (n, 16), dtype=np.uint8)
+    a[:, 0] |= 1
+    for p, r in zip(rng.choice(n, len(rows), replace=False), rows):
+        a[p] = np.frombuffer(r, dtype=np.uint8)
+    return a
+
+
+def test_np_stored_argmin_matches_a_bytes_min(orc):
+    """np_stored_argmin (the GPU stored-scan tests' reference) against Python's min over bytes, with the orderings a
+    word-wise compare gets wrong planted among random rows."""
+    rng = np.random.default_rng(7)
+    z = bytes(16)
+
+    def b(**at):   # zero row with byte i set to at[f"b{i}"]
+        r = bytearray(16)
+        for k, v in at.items():
+            r[int(k[1:])] = v
+        return bytes(r)
+    cases = {
+        "same first 8 bytes": [b(b3=1, b9=5), b(b3=1, b9=4), b(b3=1, b15=9)],
+        "same first 15 bytes": [b(b2=7, b15=3), b(b2=7, b15=2), b(b2=7, b15=4)],
+        "byte order in the high word": [b(b2=1), b(b3=1), b(b7=1)],
+        "byte order in the low word": [b(b1=1, b10=1), b(b1=1, b11=1), b(b1=1, b15=0x80)],
+        "smaller low half, larger high half": [b(b7=2), b(b7=1, b8=0xff, b15=0xff), b(b7=2, b8=1)],
+        "exact ties": [b(b5=3)] * 5 + [b(b5=4)],
+        "all-ones minimum": [],
+        "zero rows": [z] * 3 + [b(b15=1)],
+    }
+    for name, rows in cases.items():
+        for trial in range(4):
+            a = _planted(rng, 3000 + trial, rows)
+            if name == "all-ones minimum":
+                a[:] = 0xff
+            got_first, got_ties = orc.np_stored_argmin(a)
+            want_first, want_ties = _py_stored_argmin(a)
+            assert got_first == want_first and got_ties.tolist() == want_ties, name
+    for trial in range(20):                                              # random 0/1 bytes: long shared prefixes and ties
+        a = rng.integers(0, 2, (1 + 97 * trial, 16), dtype=np.uint8)
+        got_first, got_ties = orc.np_stored_argmin(a)
+        assert (got_first, got_ties.tolist()) == _py_stored_argmin(a)
+
+
 def test_stored_argmin_rule_matches_the_oracle_scan(orc):
     """Small N = 2 POSTs; seeds chosen so that both outcomes occur (P(min >= threshold) is about 1/e)."""
     seen = set()
