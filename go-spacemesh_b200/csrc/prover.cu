@@ -8,12 +8,17 @@
 //
 // Several devices (b200post_generate_proof_multi): the label range is split into contiguous shards, one host thread and
 // Scanner each; their hit lists merge in shard order (ShardedScan), so the proof is the one-device proof.
+//
+// Damaged stored data (b200post_generate_proof_checked): the kernels also return each hit's stored bytes (StoredHit), and
+// the stop rule's tentative winner has its first K2 hits recomputed and compared on the device before the scan may stop
+// on it; damaged hits are dropped (DESIGN.md §5).
 #include <algorithm>
 #include <atomic>
 #include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
+#include <set>
 #include <string>
 #include <thread>
 #include <vector>
@@ -30,14 +35,22 @@ namespace b200post {
 namespace {
 
 struct Hit { uint32_t nonce; uint32_t pad; uint64_t index; };
+// b200post_generate_proof_checked's record: the hit and the 16 stored bytes the kernel judged
+struct StoredHit { uint32_t nonce; uint32_t pad; uint64_t index; uint4 label; };
+
+__device__ __forceinline__ Hit make_hit(const Hit *, uint32_t nonce, uint64_t index, uint4) { return Hit{nonce, 0, index}; }
+__device__ __forceinline__ StoredHit make_hit(const StoredHit *, uint32_t nonce, uint64_t index, uint4 label) {
+    return StoredHit{nonce, 0, index, label};
+}
 
 // K6a: rk = per nonce group 11 round keys.  Every (label, group) costs one AES; ciphertext bytes below the
 // difficulty MSB are hits, bytes EQUAL to it (1 in 256) need the nonce's "lazy" cipher: those are queued as
 // (label offset, nonce) candidates and resolved densely by K6b — evaluating them in place would run a whole
-// AES with one or two active lanes for most warps.
+// AES with one or two active lanes for most warps.  Rec = Hit, or StoredHit to keep the label bytes with the hit.
+template <class Rec>
 __global__ void __launch_bounds__(256) prove_scan_kernel(const uint4 *__restrict__ labels, uint64_t first_index, uint32_t count,
                                                          const uint4 *__restrict__ rk, uint32_t n_groups, uint32_t diff_msb,
-                                                         const AesTables *__restrict__ tables, Hit *__restrict__ hits,
+                                                         const AesTables *__restrict__ tables, Rec *__restrict__ hits,
                                                          uint32_t hit_cap, uint32_t *__restrict__ n_hits,
                                                          uint2 *__restrict__ cands, uint32_t cand_cap, uint32_t *__restrict__ n_cands) {
     extern __shared__ uint32_t aes_sm[];
@@ -84,7 +97,7 @@ __global__ void __launch_bounds__(256) prove_scan_kernel(const uint4 *__restrict
                         slot++;
                     } else {
                         const uint32_t pos = atomicAdd(n_hits, 1u);
-                        if (pos < hit_cap) hits[pos] = Hit{nonce, 0, first_index + i};
+                        if (pos < hit_cap) hits[pos] = make_hit(hits, nonce, first_index + i, label);
                     }
                 }
             }
@@ -93,10 +106,11 @@ __global__ void __launch_bounds__(256) prove_scan_kernel(const uint4 *__restrict
 }
 
 // K6b: one thread per candidate: the nonce's lazy cipher decides with the low 56 bits.
+template <class Rec>
 __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict__ labels, uint64_t first_index,
                                                          const uint2 *__restrict__ cands, const uint32_t *__restrict__ n_cands,
                                                          uint32_t cand_cap, const uint4 *__restrict__ lazy_rk, uint64_t diff_lsb,
-                                                         const AesTables *__restrict__ tables, Hit *__restrict__ hits,
+                                                         const AesTables *__restrict__ tables, Rec *__restrict__ hits,
                                                          uint32_t hit_cap, uint32_t *__restrict__ n_hits) {
     extern __shared__ uint32_t aes_sm[];
     aes_load_smem(aes_sm, tables);
@@ -104,11 +118,12 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
     const uint32_t n = min(*n_cands, cand_cap);
     for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n; c += gridDim.x * blockDim.x) {
         const uint2 cd = cands[c];
-        const uint4 lz = aes128_encrypt(tl, lazy_rk + 11 * cd.y, labels[cd.x]);
+        const uint4 label = labels[cd.x];
+        const uint4 lz = aes128_encrypt(tl, lazy_rk + 11 * cd.y, label);
         const uint64_t lsb = ((uint64_t)lz.x | ((uint64_t)lz.y << 32)) & 0x00ffffffffffffffull;
         if (lsb >= diff_lsb) continue;
         const uint32_t pos = atomicAdd(n_hits, 1u);
-        if (pos < hit_cap) hits[pos] = Hit{cd.y, 0, first_index + cd.x};
+        if (pos < hit_cap) hits[pos] = make_hit(hits, cd.y, first_index + cd.x, label);
     }
 }
 
@@ -126,19 +141,26 @@ bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vecto
     return have;
 }
 
-// Streaming scan state: device buffers, keys, per-nonce hit lists.
+// A hit the checked scan keeps: its stored bytes, and whether they have been recomputed and found equal (good) or
+// not yet looked at (pending).  A damaged hit is removed from its list.
+struct KeptHit { uint64_t index; uint8_t label[16]; bool good; };
+using KeptLists = std::map<uint32_t, std::vector<KeptHit>>;   // nonce -> every kept hit, ascending index
+
+// Streaming scan state: device buffers, keys, per-nonce hit lists.  With keep_stored (the checked proof) the kernels
+// write StoredHit records and every hit is kept with its bytes (kept()); otherwise the first K2 per nonce (lists()).
 class Scanner {
 public:
     ~Scanner() { if (dev_ >= 0) { cudaSetDevice(dev_); drain(); } }   // the members free themselves on the scan's device
     int init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
-             uint64_t num_labels, uint64_t chunk) {
+             uint64_t num_labels, uint64_t chunk, bool keep_stored = false) {
         DeviceEngine *e = engine_for(provider);
         if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
         if (nonces == 0 || nonces % 16 || nonces > 4096 || k1 == 0 || k2 == 0 || num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
             set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
             return B200POST_ERR_INVALID_ARGUMENT;
         }
-        dev_ = e->device(); nonces_ = nonces; k2_ = k2; chunk_ = chunk;
+        engine_ = e; dev_ = e->device(); nonces_ = nonces; k2_ = k2; chunk_ = chunk;
+        stored_ = keep_stored; rec_ = stored_ ? sizeof(StoredHit) : sizeof(Hit);
         const uint64_t diff = b200post_proving_difficulty(k1, num_labels);
         msb_ = (uint32_t)(diff >> 56); lsb_ = diff & 0x00ffffffffffffffull;
         // hits per chunk are ~ chunk * nonces * K1/numLabels; leave generous slack, cap the buffer at 64 MiB
@@ -172,9 +194,9 @@ public:
             CUDA_TRY(ev_[b].create(cudaEventDisableTiming));
             CUDA_TRY(d_labels_[b].resize(chunk * 16));
             CUDA_TRY(h_labels_[b].resize(chunk * 16));
-            CUDA_TRY(d_hits_[b].resize(hit_cap_));
+            CUDA_TRY(d_hits_[b].resize((size_t)hit_cap_ * rec_));
             CUDA_TRY(d_nhits_[b].resize(1));
-            CUDA_TRY(h_hits_[b].resize(hit_cap_));
+            CUDA_TRY(h_hits_[b].resize((size_t)hit_cap_ * rec_));
             CUDA_TRY(h_nhits_[b].resize(1));
             CUDA_TRY(h_ncands_[b].resize(1));
         }
@@ -198,17 +220,13 @@ public:
         CUDA_TRY(cudaMemsetAsync(d_ncands_.get(), 0, 8, st_[b].get()));
         cudaStream_t st = st_[b].get();
         const uint4 *labels = reinterpret_cast<const uint4 *>(d_labels_[b].get());
-        prove_scan_kernel<<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
-                                                              msb_, d_tables_.get(), d_hits_[b].get(), hit_cap_, d_nhits_[b].get(),
-                                                              d_cands_.get(), cand_cap_, d_ncands_.get());
-        prove_lazy_kernel<<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
-                                                              reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
-                                                              d_hits_[b].get(), hit_cap_, d_nhits_[b].get());
+        if (stored_) launch(st, labels, first, count, reinterpret_cast<StoredHit *>(d_hits_[b].get()), d_nhits_[b].get());
+        else launch(st, labels, first, count, reinterpret_cast<Hit *>(d_hits_[b].get()), d_nhits_[b].get());
         g_launches += 2;
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaMemcpyAsync(h_ncands_[b].get(), d_ncands_.get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
         CUDA_TRY(cudaMemcpyAsync(h_nhits_[b].get(), d_nhits_[b].get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
-        CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * sizeof(Hit), cudaMemcpyDeviceToHost, st_[b].get()));
+        CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * rec_, cudaMemcpyDeviceToHost, st_[b].get()));
         CUDA_TRY(cudaEventRecord(ev_[b].get(), st_[b].get()));
         pending_[b] = true; count_[b] = count;
         return B200POST_OK;
@@ -221,7 +239,9 @@ public:
         pending_[b] = false;
         const uint32_t n = *h_nhits_[b].get();
         if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
-        std::vector<Hit> v(h_hits_[b].get(), h_hits_[b].get() + n);
+        if (stored_) return fold_stored(b, n, fold_mu);
+        const Hit *rec = reinterpret_cast<const Hit *>(h_hits_[b].get());
+        std::vector<Hit> v(rec, rec + n);
         std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
         std::unique_lock<std::mutex> lk;
         if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
@@ -232,28 +252,70 @@ public:
         scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
         return B200POST_OK;
     }
+    int fold_stored(int b, uint32_t n, std::mutex *fold_mu) {
+        const StoredHit *rec = reinterpret_cast<const StoredHit *>(h_hits_[b].get());
+        std::vector<StoredHit> v(rec, rec + n);
+        std::sort(v.begin(), v.end(), [](const StoredHit &x, const StoredHit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+        std::unique_lock<std::mutex> lk;
+        if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
+        for (const StoredHit &h : v) {
+            KeptHit k{h.index, {}, false};
+            memcpy(k.label, &h.label, 16);
+            kept_[h.nonce].push_back(k);
+        }
+        scanned_ += count_[b];
+        return B200POST_OK;
+    }
     // wait for whatever is still in flight, without folding it (error and cancel paths)
     void drain() {
         for (int b = 0; b < 2; b++) if (pending_[b]) { cudaEventSynchronize(ev_[b].get()); pending_[b] = false; }
     }
     const HitLists &lists() const { return lists_; }
+    const KeptLists &kept() const { return kept_; }
+    KeptLists &kept() { return kept_; }
     bool any_full() const { return full_ > 0; }          // some nonce has K2 hits
-    bool saturated() const { return full_ == nonces_; }  // every nonce has K2 hits: later labels change no first K2
+    // every nonce has K2 hits (kept: K2 good ones): later labels change no nonce's first K2 (usable) hits
+    bool saturated() const { return stored_ ? count_kept(true) == nonces_ : full_ == nonces_; }
+    // nonces with at least K2 kept hits (good ones only, or good and pending)
+    uint32_t count_kept(bool good_only) const {
+        uint32_t full = 0;
+        for (const auto &kv : kept_) {
+            size_t c = 0;
+            for (const KeptHit &k : kv.second) if ((c += !good_only || k.good) >= k2_) break;
+            full += c >= k2_;
+        }
+        return full;
+    }
+    uint32_t nonces() const { return nonces_; }
     uint64_t scanned() const { return scanned_; }
     int device() const { return dev_; }
+    DeviceEngine *engine() const { return engine_; }
 
 private:
+    template <class Rec>
+    void launch(cudaStream_t st, const uint4 *labels, uint64_t first, uint32_t count, Rec *hits, uint32_t *n_hits) {
+        prove_scan_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
+                                                                   msb_, d_tables_.get(), hits, hit_cap_, n_hits, d_cands_.get(), cand_cap_,
+                                                                   d_ncands_.get());
+        prove_lazy_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
+                                                                   reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
+                                                                   hits, hit_cap_, n_hits);
+    }
+
+    DeviceEngine *engine_ = nullptr;
     int dev_ = -1;
     uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0, full_ = 0;
     uint64_t lsb_ = 0, chunk_ = 0, scanned_ = 0;
+    bool stored_ = false;
+    size_t rec_ = sizeof(Hit);   // bytes per hit record (Hit or StoredHit)
     DeviceBuffer<uint8_t> d_rk_, d_lazy_;
     DeviceBuffer<AesTables> d_tables_;
     Stream st_[2];
     Event ev_[2];
     DeviceBuffer<uint8_t> d_labels_[2];
     PinnedBuffer<uint8_t> h_labels_[2];
-    DeviceBuffer<Hit> d_hits_[2];
-    PinnedBuffer<Hit> h_hits_[2];
+    DeviceBuffer<uint8_t> d_hits_[2];   // hit_cap_ records of rec_ bytes
+    PinnedBuffer<uint8_t> h_hits_[2];
     DeviceBuffer<uint32_t> d_nhits_[2];
     PinnedBuffer<uint32_t> h_nhits_[2], h_ncands_[2];
     DeviceBuffer<uint2> d_cands_;
@@ -262,6 +324,7 @@ private:
     bool pending_[2] = {false, false};
     uint32_t count_[2] = {0, 0};
     HitLists lists_;
+    KeptLists kept_;
 };
 
 // One contiguous label range [lo, hi) of a scan, streamed through its own Scanner.
@@ -330,11 +393,140 @@ public:
         return t;
     }
 
+    // ---- the checked proof (b200post_generate_proof_checked): every hit is kept with its stored bytes, and the stop
+    // rule's tentative winner has its first K2 hits recomputed under `commitment` before the scan may stop on it
+    void enable_check(const uint8_t commitment[32], uint64_t N, const volatile int *cancel) {
+        checked_ = true;
+        memcpy(commitment_, commitment, 32);
+        N_ = N; cancel_ = cancel;
+    }
+    // After run(): recheck rounds over everything kept until the winner's first K2 hits are all good (the winner and its
+    // indices) or no nonce has K2 usable hits (false, *rc OK).  Needs no round when the scan stopped on a decision.
+    bool decide(uint32_t *nonce, std::vector<uint64_t> *indices, int *rc) {
+        *rc = B200POST_OK;
+        for (;;) {
+            std::vector<Item> items;
+            const Plan p = plan_winner(&items, nonce, indices);
+            if (p != RECHECK) return p == DECIDED;
+            if ((*rc = round(shards_[0]->sc.engine(), items))) return false;
+        }
+    }
+    uint64_t rechecked() const { return rechecked_; }
+    uint32_t rounds() const { return rounds_; }
+    const std::set<uint64_t> &damaged() const { return damaged_; }
+
 private:
+    struct Item { size_t shard; uint32_t nonce; uint64_t index; uint8_t label[16]; };
+    enum Plan { NONE, DECIDED, RECHECK };
+
+    // Under mu_ (or with the threads joined).  The stop rule over kept (good and pending) hits below x: NONE if no nonce
+    // has K2 of them; DECIDED with the winner when the winner's first K2 are all good; RECHECK with the pending ones.
+    Plan plan_winner(std::vector<Item> *items, uint32_t *nonce, std::vector<uint64_t> *indices) const {
+        struct Ref { size_t shard; const KeptHit *k; };
+        std::map<uint32_t, std::vector<Ref>> m;   // per nonce, its first K2 kept hits below x in shard order
+        for (size_t s = 0; s < shards_.size(); s++) {
+            const Scanner &sc = shards_[s]->sc;
+            for (const auto &kv : sc.kept()) {
+                std::vector<Ref> &l = m[kv.first];
+                for (size_t i = 0; i < kv.second.size() && l.size() < k2_; i++) l.push_back({s, &kv.second[i]});
+            }
+            if (sc.scanned() < shards_[s]->hi - shards_[s]->lo && !sc.saturated()) break;   // x lies in this shard
+        }
+        const std::pair<const uint32_t, std::vector<Ref>> *win = nullptr;
+        for (const auto &kv : m)
+            if (kv.second.size() >= k2_ && (!win || kv.second[k2_ - 1].k->index < win->second[k2_ - 1].k->index)) win = &kv;
+        if (!win) return NONE;
+        for (const Ref &r : win->second) {
+            if (r.k->good) continue;
+            Item it{r.shard, win->first, r.k->index, {}};
+            memcpy(it.label, r.k->label, 16);
+            items->push_back(it);
+        }
+        if (!items->empty()) return RECHECK;
+        *nonce = win->first;
+        indices->clear();
+        for (const Ref &r : win->second) indices->push_back(r.k->index);
+        return DECIDED;
+    }
+    // Under mu_: when every nonce has K2 kept hits in shard s but not K2 good ones, the pending ones among each nonce's
+    // first K2 in the shard (the shard's own saturation stop counts good hits only).
+    bool plan_saturation(size_t s, std::vector<Item> *items) const {
+        const Scanner &sc = shards_[s]->sc;
+        if (sc.count_kept(false) != sc.nonces()) return false;
+        for (const auto &kv : sc.kept())
+            for (size_t i = 0; i < kv.second.size() && i < k2_; i++) {
+                const KeptHit &k = kv.second[i];
+                if (k.good) continue;
+                Item it{s, kv.first, k.index, {}};
+                memcpy(it.label, k.label, 16);
+                items->push_back(it);
+            }
+        return !items->empty();
+    }
+    // One recheck round on `e` (outside mu_): the items' labels recomputed and compared with their stored bytes, then,
+    // under mu_ when threads run, good ones marked and damaged ones dropped.  A compare reports at most
+    // CompareResult::kMaxReported positions, so it is repeated past the last reported one until every mismatch is known.
+    int round(DeviceEngine *e, const std::vector<Item> &items) {
+        const size_t n = items.size();
+        std::vector<uint64_t> idx(n);
+        std::vector<uint8_t> expect(n * 16), bad(n, 0);
+        for (size_t i = 0; i < n; i++) { idx[i] = items[i].index; memcpy(&expect[i * 16], items[i].label, 16); }
+        for (size_t from = 0; from < n;) {
+            CompareResult cmp;
+            const int rc = e->labels_compare_indexed(commitment_, n - from, idx.data() + from, N_, expect.data() + from * 16, &cmp, cancel_);
+            if (rc) return rc;
+            for (uint64_t p : cmp.first) bad[from + p] = 1;
+            if (cmp.mismatches <= cmp.first.size()) break;
+            from += cmp.first.back() + 1;
+        }
+        std::unique_lock<std::mutex> lk(mu_);
+        for (size_t i = 0; i < n; i++) {
+            std::vector<KeptHit> &l = shards_[items[i].shard]->sc.kept()[items[i].nonce];
+            auto it = std::lower_bound(l.begin(), l.end(), items[i].index, [](const KeptHit &k, uint64_t v) { return k.index < v; });
+            if (it == l.end() || it->index != items[i].index) continue;
+            if (bad[i]) { l.erase(it); damaged_.insert(items[i].index); }
+            else it->good = true;
+        }
+        rechecked_ += n; rounds_++;
+        return B200POST_OK;
+    }
+    // The checked stop rule for shard s, run by its thread after each chunk: stop once a decision is taken or the shard is
+    // saturated by good hits.  When the multi-device stop rule fires (or the shard would saturate) this thread runs recheck
+    // rounds until that settles, while the other shards keep scanning.  One winner round runs at a time; a saturation
+    // round touches only its own shard's hits.
+    bool should_stop_checked(size_t s, int *rc) {
+        for (;;) {
+            std::vector<Item> items;
+            bool winner_round = false;
+            {
+                std::lock_guard<std::mutex> lk(mu_);
+                if (decided_ || shards_[s]->sc.saturated()) return true;
+                if (!round_busy_) {
+                    uint32_t nonce;
+                    std::vector<uint64_t> idx;
+                    const Plan p = plan_winner(&items, &nonce, &idx);
+                    if (p == DECIDED) { decided_ = true; return true; }
+                    winner_round = round_busy_ = p == RECHECK;
+                }
+                if (!winner_round && !plan_saturation(s, &items)) return false;
+            }
+            *rc = round(shards_[s]->sc.engine(), items);
+            if (winner_round) { std::lock_guard<std::mutex> lk(mu_); round_busy_ = false; }
+            if (*rc) return true;
+        }
+    }
+
+    bool checked_ = false, decided_ = false, round_busy_ = false;   // the last two under mu_
+    uint8_t commitment_[32] = {0};
+    uint64_t N_ = 0;
+    const volatile int *cancel_ = nullptr;
+    uint64_t rechecked_ = 0;                 // under mu_
+    uint32_t rounds_ = 0;
+    std::set<uint64_t> damaged_;
     int run_shard(size_t s, const Fill &fill, uint64_t chunk, uint64_t base, const volatile int *cancel) {
         Shard &sh = *shards_[s];
         Scanner &sc = sh.sc;
-        std::mutex *mu = shards_.size() > 1 ? &mu_ : nullptr;
+        std::mutex *mu = shards_.size() > 1 || checked_ ? &mu_ : nullptr;
         int rc = B200POST_OK;
         if (sh.lo == sh.hi) return rc;
         if (cudaSetDevice(sc.device()) != cudaSuccess) { cudaGetLastError(); set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
@@ -343,7 +535,9 @@ private:
             if (cancel && *cancel) { sc.drain(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
             if (abort_) { sc.drain(); return B200POST_OK; }   // another shard failed: its status is the call's
             if ((rc = sc.collect(b, mu))) { sc.drain(); return rc; }
-            if (should_stop(s)) break;
+            const bool stop = checked_ ? should_stop_checked(s, &rc) : should_stop(s);
+            if (rc) { sc.drain(); return rc; }
+            if (stop) break;
             // fill the staging buffer (a chunk may span files)
             const uint64_t n = std::min<uint64_t>(chunk, sh.hi - pos);
             if ((rc = fill(s, pos, n, sc.staging(b))) || (rc = sc.submit(b, base + pos, (uint32_t)n))) { sc.drain(); return rc; }
@@ -373,10 +567,8 @@ private:
     std::atomic<bool> abort_{false};
 };
 
-int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
-    uint32_t nonce = 0;
-    std::vector<uint64_t> idx;
-    if (!pick_winner(scan.merged(), k2, &nonce, &idx)) { set_error("no proof found: no nonce reached K2 qualifying labels"); return B200POST_ERR_INVALID_PROOF; }
+int write_proof(const ShardedScan &scan, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint64_t num_labels,
+                b200post_proof_out *out) {
     const uint64_t scanned = scan.scanned();
     metrics().prove_labels_scanned_total += scanned; metrics().proofs_generated_total++;
     memset(out, 0, sizeof *out);
@@ -384,6 +576,33 @@ int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t 
     out->indices_len = b200post_pack_indices(idx.data(), idx.size(), b200post_bits_per_index(num_labels), out->indices, sizeof out->indices);
     if (out->indices_len == 0) { set_error("packed indices exceed the 800-byte wire cap"); return B200POST_ERR_INVALID_ARGUMENT; }
     return B200POST_OK;
+}
+
+const char *const kNoProof = "no proof found: no nonce reached K2 qualifying labels";
+
+int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
+    uint32_t nonce = 0;
+    std::vector<uint64_t> idx;
+    if (!pick_winner(scan.merged(), k2, &nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
+    return write_proof(scan, nonce, idx, pows, num_labels, out);
+}
+
+// The checked proof's decision step: recheck rounds until the winner over usable hits is known, then the report.
+int finish_checked(ShardedScan &scan, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out, b200post_prove_check *check) {
+    uint32_t nonce = 0;
+    std::vector<uint64_t> idx;
+    int rc = B200POST_OK;
+    const bool have = scan.decide(&nonce, &idx, &rc);
+    check->labels_rechecked = scan.rechecked(); check->damaged = scan.damaged().size(); check->rounds = scan.rounds();
+    for (uint64_t i : scan.damaged()) {   // ascending
+        if (check->n_reported == 64) break;
+        check->damaged_index[check->n_reported++] = i;
+    }
+    metrics().prove_labels_rechecked_total += check->labels_rechecked;
+    metrics().prove_damaged_labels_total += check->damaged;
+    if (rc) return rc;
+    if (!have) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
+    return write_proof(scan, nonce, idx, pows, num_labels, out);
 }
 
 }  // namespace
@@ -406,6 +625,12 @@ void parallel_copy(uint8_t *dst, const uint8_t *src, size_t bytes) {
     }
     for (auto &x : th) x.join();
 }
+}  // namespace
+
+namespace {
+int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
+             const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
+             b200post_prove_check *check, const volatile int *cancel);
 }  // namespace
 
 extern "C" {
@@ -438,6 +663,26 @@ int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[
                                   const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
                                   b200post_proof_out *out, b200post_proof_metadata *meta_out, const volatile int *cancel) {
     if (!data_dir || !challenge || !cfg || !out || !providers || n_providers <= 0) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    return generate(data_dir, challenge, cfg, opts, providers, n_providers, out, meta_out, nullptr, cancel);
+}
+
+int b200post_generate_proof_checked(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                    const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                    b200post_proof_out *out, b200post_proof_metadata *meta_out, b200post_prove_check *check,
+                                    const volatile int *cancel) {
+    if (!data_dir || !challenge || !cfg || !out || !providers || n_providers <= 0 || !check) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    memset(check, 0, sizeof *check);
+    return generate(data_dir, challenge, cfg, opts, providers, n_providers, out, meta_out, check, cancel);
+}
+
+}  // extern "C"
+
+namespace {
+// b200post_generate_proof_multi (check == nullptr) and b200post_generate_proof_checked: they differ only in the scan's
+// hit records and the decision step (ShardedScan::enable_check, finish_checked) and the final verifier gate
+int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
+             const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
+             b200post_prove_check *check, const volatile int *cancel) {
     b200post_prove_opts o{};
     if (opts) o = *opts;
     if (o.nonces == 0) o.nonces = 16;
@@ -447,6 +692,10 @@ int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[
     if (rc) return rc;
     const uint64_t num_labels = (uint64_t)md.num_units * md.labels_per_unit;
     if (num_labels == 0 || o.nonces % 16 || o.nonces > 4096) { set_error("invalid metadata or nonce count"); return B200POST_ERR_INVALID_ARGUMENT; }
+    if (check && (md.scrypt_n < 2 || md.scrypt_n > (1ull << 20) || (md.scrypt_n & (md.scrypt_n - 1)))) {
+        set_error("corrupt metadata: Scrypt.N out of range");
+        return B200POST_ERR_IO;
+    }
     // k2pow per nonce group (RandomX upstream) through the caller's hook
     std::vector<uint64_t> pows(o.nonces / 16, 0);
     if (o.pow_mode > B200POST_POW_SKIP || (o.pow_mode == B200POST_POW_CALLBACK && !o.pow_prove)) {
@@ -473,10 +722,15 @@ int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[
     // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
     const uint64_t chunk = std::min<uint64_t>(o.chunk_labels, num_labels);
     ShardedScan scan((size_t)n_providers, o.nonces, cfg->k2);
+    if (check) {
+        uint8_t commitment[32];
+        commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
+        scan.enable_check(commitment, md.scrypt_n, cancel);
+    }
     const auto ranges = split_shards(num_labels, chunk, (size_t)n_providers);
     for (int s = 0; s < n_providers; s++) {
         Shard &sh = scan.shard((size_t)s);
-        if ((rc = sh.sc.init(providers[s], challenge, o.nonces, pows.data(), cfg->k1, cfg->k2, num_labels, chunk))) return rc;
+        if ((rc = sh.sc.init(providers[s], challenge, o.nonces, pows.data(), cfg->k1, cfg->k2, num_labels, chunk, check != nullptr))) return rc;
         sh.lo = ranges[(size_t)s].first; sh.hi = ranges[(size_t)s].second;
     }
 
@@ -486,14 +740,32 @@ int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[
     for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
     rc = scan.run([&](size_t s, uint64_t pos, uint64_t n, uint8_t *dst) { return readers[s]->read(pos, n, dst); }, chunk, 0, cancel);
     if (rc) return rc;
-    if ((rc = finish(scan, cfg->k2, pows.data(), num_labels, out))) return rc;
-    if (meta_out) {
-        memcpy(meta_out->node_id, md.node_id, 32);
-        memcpy(meta_out->commitment_atx_id, md.commitment_atx_id, 32);
-        memcpy(meta_out->challenge, challenge, 32);
-        meta_out->num_units = md.num_units; meta_out->labels_per_unit = md.labels_per_unit;
+    if ((rc = check ? finish_checked(scan, pows.data(), num_labels, out, check) : finish(scan, cfg->k2, pows.data(), num_labels, out))) return rc;
+    b200post_proof_metadata meta;
+    memcpy(meta.node_id, md.node_id, 32);
+    memcpy(meta.commitment_atx_id, md.commitment_atx_id, 32);
+    memcpy(meta.challenge, challenge, 32);
+    meta.num_units = md.num_units; meta.labels_per_unit = md.labels_per_unit;
+    if (check) {
+        // the gate: a proof this library's own verifier rejects is never handed out
+        b200post_verify_params vp{};
+        vp.k1 = cfg->k1; vp.k2 = cfg->k2; vp.scrypt_n = md.scrypt_n;
+        memcpy(vp.pow_difficulty, cfg->pow_difficulty, 32);
+        b200post_verifier_opts vo{};
+        vo.pow_mode = o.pow_mode == B200POST_POW_BUILTIN ? B200POST_POW_BUILTIN : B200POST_POW_SKIP;
+        vo.pow_cache_key = o.pow_cache_key; vo.pow_cache_key_len = o.pow_cache_key_len;
+        const b200post_proof proof{out->nonce, out->indices, out->indices_len, out->pow};
+        int status = B200POST_OK;
+        uint64_t bad = 0;
+        if ((rc = b200post_verify_batch(providers[0], 1, &proof, &meta, &vp, nullptr, &vo, &status, &bad))) return rc;
+        if (status != B200POST_OK) {
+            memset(out, 0, sizeof *out);
+            set_error(bad == ~0ull ? "the proof failed the verifier's k2pow check" : "the proof failed the verifier at position " + std::to_string(bad));
+            return B200POST_ERR_INVALID_PROOF;
+        }
+        check->proof_verified = 1;
     }
+    if (meta_out) *meta_out = meta;
     return B200POST_OK;
 }
-
-}  // extern "C"
+}  // namespace

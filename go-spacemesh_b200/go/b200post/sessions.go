@@ -437,6 +437,49 @@ func GenerateProofOn(ctx context.Context, providers []uint32, dataDir string, ch
 	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
 }
 
+// ProveCheck is what GenerateProofChecked found: scan hits recomputed, distinct damaged label indices among them (a
+// lower bound on the damage), the lowest 64 of those ascending, and whether the proof passed the library's verifier.
+type ProveCheck struct {
+	LabelsRechecked uint64
+	Damaged         uint64
+	DamagedIndex    []uint64
+	ProofVerified   bool
+	Rounds          uint32
+}
+
+// GenerateProofChecked is GenerateProofOn over stored data that may be damaged (b200post_generate_proof_checked): a
+// stored label is a hit only when it also equals its recomputed label, and the proof passes the library's verifier
+// before it is returned.  On clean data the proof equals GenerateProofOn's.  Damage is not an error: a non-empty
+// report means the data needs `b200postcli -verify -fraction 100` and the damaged file a repair.
+func GenerateProofChecked(ctx context.Context, providers []uint32, dataDir string, challenge []byte, cfg SetupConfig, nonces uint32) (*Proof, *ProveCheck, error) {
+	if len(providers) == 0 {
+		return nil, nil, ErrNoProvider
+	}
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces)}
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	var out C.b200post_proof_out
+	var chk C.b200post_prove_check
+	if err := statusErr(checked(func() C.int {
+		return C.b200post_generate_proof_checked(dir, (*C.uint8_t)(unsafe.Pointer(&challenge[0])), &c, &o, provs, C.int(len(providers)), &out, nil, &chk, flag)
+	})); err != nil {
+		return nil, nil, err
+	}
+	rep := &ProveCheck{LabelsRechecked: uint64(chk.labels_rechecked), Damaged: uint64(chk.damaged), ProofVerified: chk.proof_verified != 0,
+		Rounds: uint32(chk.rounds)}
+	for i := 0; i < int(chk.n_reported); i++ {
+		rep.DamagedIndex = append(rep.DamagedIndex, uint64(chk.damaged_index[i]))
+	}
+	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, rep, nil
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Checking stored POST data (postcli -verify; verifying.VerifyPos, recalled, unpinned)
 // ---------------------------------------------------------------------------------------------------------

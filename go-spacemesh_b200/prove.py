@@ -7,6 +7,7 @@ PostVerifier.verify.  The k2pow (RandomX upstream) is a caller-supplied hook; co
 from __future__ import annotations
 
 import ctypes
+from dataclasses import dataclass, field
 
 import numpy as np
 
@@ -29,6 +30,23 @@ class _ProofOut(ctypes.Structure):
                 ("indices", ctypes.c_uint8 * 800), ("labels_scanned", ctypes.c_uint64)]
 
 
+class _ProveCheck(ctypes.Structure):
+    _fields_ = [("labels_rechecked", ctypes.c_uint64), ("damaged", ctypes.c_uint64), ("n_reported", ctypes.c_uint32),
+                ("damaged_index", ctypes.c_uint64 * 64), ("proof_verified", ctypes.c_uint32), ("rounds", ctypes.c_uint32)]
+
+
+@dataclass
+class ProveCheck:
+    """What generate_proof_checked found: hits rechecked against their recomputed labels, the distinct damaged label
+    indices among them (a lower bound on the POST's damage), the lowest 64 of those ascending, whether the proof passed
+    the library's verifier, and the recheck rounds run."""
+    labels_rechecked: int
+    damaged: int
+    damaged_index: list = field(default_factory=list)
+    proof_verified: bool = False
+    rounds: int = 0
+
+
 def _bind():
     L = lib()
     if getattr(L, "_prove_bound", False):
@@ -40,6 +58,9 @@ def _bind():
                                                 ctypes.POINTER(_Meta), ctypes.c_void_p]
     L.b200post_prove_scan.argtypes = [ctypes.c_uint32, ctypes.c_void_p, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_char_p, ctypes.c_uint32,
                                       ctypes.POINTER(ctypes.c_uint64), ctypes.c_uint32, ctypes.c_uint32, ctypes.c_uint64, ctypes.POINTER(_ProofOut)]
+    L.b200post_generate_proof_checked.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
+                                                  ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_ProofOut),
+                                                  ctypes.POINTER(_Meta), ctypes.POINTER(_ProveCheck), ctypes.c_void_p]
     L._prove_bound = True
     return L
 
@@ -59,15 +80,7 @@ def _err(rc):
         raise B200PostError(rc, lib().b200post_last_error().decode(errors="replace"))
 
 
-def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int | None = None, nonces: int = 16,
-                   chunk_labels: int = 0, pow="builtin", providers=None, cancel=None):
-    """PostClient.Proof(ctx, challenge) -> (Post, PostInfo-like metadata); also returns labels scanned.
-    pow: "builtin" (k2pow search on the device, the library default), "skip" (pow = 0, explicit) or a callable
-    (ctx, nonce_group, challenge8, difficulty32, node_id32, pow_out) -> 0.
-    providers: a list of device ids (repeats allowed) or "all" proves on several devices with the one-device result;
-    it replaces `provider` (default 0), and giving both is an error.  cancel: an optional ctypes.c_int, polled per
-    chunk."""
-    L = _bind()
+def _opts(provider, providers, nonces, chunk_labels, pow):
     if provider is not None and providers is not None:
         raise ValueError("give `provider` or `providers`, not both")
     if isinstance(providers, str):
@@ -80,7 +93,46 @@ def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider
         cb, mode = POW_PROVE_FN(pow), 1
     else:
         cb, mode = ctypes.cast(None, POW_PROVE_FN), {"builtin": 0, "skip": 2, "callback-missing": 1}[pow]
-    opts = _ProveOpts(provider or 0, nonces, chunk_labels, cb, None, mode, None, 0)
+    return _ProveOpts(provider or 0, nonces, chunk_labels, cb, None, mode, None, 0), providers
+
+
+def _results(out, meta):
+    proof = Proof(int(out.nonce), bytes(out.indices[: out.indices_len]), int(out.pow))
+    pm = ProofMetadata(bytes(meta.node_id), bytes(meta.commitment_atx_id), bytes(meta.challenge), int(meta.num_units),
+                       int(meta.labels_per_unit))
+    return proof, pm, int(out.labels_scanned)
+
+
+def generate_proof_checked(data_dir: str, challenge: bytes, cfg: PostConfig, *, providers=(0,), nonces: int = 16,
+                           chunk_labels: int = 0, pow="builtin", cancel=None):
+    """generate_proof over stored data that may be damaged (b200post_generate_proof_checked): a stored label is a hit
+    only when it also equals its recomputed label, so a damaged label never enters the proof, and the proof passes the
+    library's verifier before it is returned.  On undamaged data the proof equals generate_proof's.
+    Returns (Proof, ProofMetadata, labels scanned, ProveCheck).  A non-empty report is damage in the stored POST data:
+    run `b200postcli -verify -fraction 100` to find all of it.  providers: a list of device ids or "all"."""
+    L = _bind()
+    opts, providers = _opts(None, list(providers) if not isinstance(providers, str) else providers, nonces, chunk_labels, pow)
+    out, meta, chk, c = _ProofOut(), _Meta(), _ProveCheck(), _c_cfg(cfg)
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    arr = (ctypes.c_uint32 * len(providers))(*providers)
+    _err(L.b200post_generate_proof_checked(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts),
+                                           arr if len(providers) else None, len(providers), ctypes.byref(out),
+                                           ctypes.byref(meta), ctypes.byref(chk), cptr))
+    report = ProveCheck(int(chk.labels_rechecked), int(chk.damaged), [int(v) for v in chk.damaged_index[: chk.n_reported]],
+                        bool(chk.proof_verified), int(chk.rounds))
+    return (*_results(out, meta), report)
+
+
+def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int | None = None, nonces: int = 16,
+                   chunk_labels: int = 0, pow="builtin", providers=None, cancel=None):
+    """PostClient.Proof(ctx, challenge) -> (Post, PostInfo-like metadata); also returns labels scanned.
+    pow: "builtin" (k2pow search on the device, the library default), "skip" (pow = 0, explicit) or a callable
+    (ctx, nonce_group, challenge8, difficulty32, node_id32, pow_out) -> 0.
+    providers: a list of device ids (repeats allowed) or "all" proves on several devices with the one-device result;
+    it replaces `provider` (default 0), and giving both is an error.  cancel: an optional ctypes.c_int, polled per
+    chunk."""
+    L = _bind()
+    opts, providers = _opts(provider, providers, nonces, chunk_labels, pow)
     out, meta, c = _ProofOut(), _Meta(), _c_cfg(cfg)
     cptr = ctypes.addressof(cancel) if cancel is not None else None
     if providers is None:
@@ -91,10 +143,7 @@ def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider
         _err(L.b200post_generate_proof_multi(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts),
                                              arr if len(providers) else None, len(providers), ctypes.byref(out),
                                              ctypes.byref(meta), cptr))
-    proof = Proof(int(out.nonce), bytes(out.indices[: out.indices_len]), int(out.pow))
-    pm = ProofMetadata(bytes(meta.node_id), bytes(meta.commitment_atx_id), bytes(meta.challenge), int(meta.num_units),
-                       int(meta.labels_per_unit))
-    return proof, pm, int(out.labels_scanned)
+    return _results(out, meta)
 
 
 def prove_scan(labels: np.ndarray, challenge: bytes, nonces: int, pows, k1: int, k2: int, num_labels: int, *,

@@ -82,6 +82,42 @@ int b200post_generate_proof_multi(const char *data_dir, const uint8_t challenge[
                                   const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
                                   b200post_proof_out *out, b200post_proof_metadata *meta_out, const volatile int *cancel);
 
+/* What b200post_generate_proof_checked found while proving. */
+typedef struct b200post_prove_check {
+    uint64_t labels_rechecked;         /* scan hits recomputed and compared with their stored bytes              */
+    uint64_t damaged;                  /* distinct label indices among them whose stored bytes differ: damage    */
+    uint32_t n_reported;
+    uint64_t damaged_index[64];        /* the lowest n_reported damaged label indices, ascending                  */
+    uint32_t proof_verified;           /* 1: the returned proof passed b200post_verify_batch                     */
+    uint32_t rounds;                   /* recheck rounds run                                                      */
+} b200post_prove_check;
+
+/* b200post_generate_proof_multi over stored data that may be damaged (bit rot, a bad drive, a truncated copy).
+ * A stored label counts as a hit of a nonce only when it passes the nonce's difficulty AND equals the label recomputed
+ * from blake3(NodeId || CommitmentAtxId) at its index under the metadata's scrypt N.  The proof is the one-device
+ * selection rule applied to those usable hits, so it depends on the stored data and the real labels only, not on the
+ * device list or the chunk size; on undamaged data (nonce, indices, pow) are byte-identical to
+ * b200post_generate_proof_multi's.
+ *   How: the scan keeps every hit with its 16 stored bytes.  Whenever the multi-device stop rule would fire, the
+ *   tentative winner (over unrejected hits below the end of the gap-free scanned prefix) has its not yet rechecked hits
+ *   among its first K2 recomputed on the device (K2s/K2p + K3c, the verify_pos path); damaged hits are dropped and the
+ *   decision is taken again.  The scan stops only when the winner's first K2 hits are all rechecked.  A shard's own
+ *   saturation stop likewise needs K2 rechecked hits for every nonce.
+ *   Gate: before returning, the proof goes through b200post_verify_batch on providers[0] (k2pow checked under
+ *   pow_mode BUILTIN, not under SKIP or CALLBACK); a rejection returns B200POST_ERR_INVALID_PROOF and no proof.
+ *   check: labels_rechecked, the damage found and the lowest 64 damaged indices.  The report is a LOWER BOUND on the
+ *   damage and may differ between device lists and chunk sizes; it never names an undamaged label, and it names every
+ *   damaged hit among the first K2 hits of every nonce that was ever the tentative winner.  Not seen: a damaged label
+ *   that falsely FAILS the difficulty (never a hit; harmless to the proof) and damage past the decision point.  The
+ *   full check of the stored data is b200postcli -verify -fraction 100 (b200post_verify_pos).
+ * Damage alone is not an error: B200POST_OK with a valid proof and a non-zero report.  Arguments (check NULL included),
+ * host checks and their order, cancellation and read errors are those of b200post_generate_proof_multi; metadata with
+ * an invalid scrypt N is B200POST_ERR_IO.  A one-device call is a list of one. */
+int b200post_generate_proof_checked(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                    const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                    b200post_proof_out *out, b200post_proof_metadata *meta_out, b200post_prove_check *check,
+                                    const volatile int *cancel);
+
 /* The scan alone over labels already in host memory: labels16 = count x 16 bytes holding label indices
  * [first_index, first_index + count).  pows = one u64 per nonce group (nonces/16 of them). */
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count,
