@@ -17,6 +17,11 @@
 //   b200postcli -printNumFiles -numUnits N -labelsPerUnit L [-maxFileSize S]   how many files the POST has
 //   b200postcli -searchForNonce -datadir D [-provider 0|all] [-computeBatchSize B]
 // The last one finds the VRF nonce of the merged files from their stored labels and writes it to the metadata.
+//
+// The initial proof (the proof for the zero challenge a node asks for right after initialisation) from the labels as
+// the session computes them, so that the node's post-service need not read the whole POST back:
+//   b200postcli <init flags> -initialProof [-nonces 288] [-k1 26] [-k2 37] [-powDifficulty <64 hex digits>]
+// writes initial_post.json into the data dir (k2pow on the session's devices).  Not with -fromFile / -toFile.
 // Exit codes: 0 ok, 1 error or damaged data, 2 usage, 130 stopped.
 #include <signal.h>
 
@@ -28,7 +33,7 @@
 #include <string>
 #include <thread>
 
-#include "../../include/b200post_setup.h"
+#include "../../include/b200post_prove.h"
 
 static volatile int g_cancel = 0;
 static void on_signal(int) { g_cancel = 1; }
@@ -133,7 +138,9 @@ static int run_search(const std::string &datadir, const std::string &provider, u
 int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
-    bool print_providers = false, verify = false, print_num_files = false, search = false, range = false;
+    bool print_providers = false, verify = false, print_num_files = false, search = false, range = false, initial = false;
+    uint32_t nonces = 288, k1 = 0, k2 = 0;
+    std::string pow_difficulty;
     double fraction = 0.2;
     uint64_t from_file = 0, seed = 0;
     int64_t to_file = -1;
@@ -161,6 +168,11 @@ int main(int argc, char **argv) {
         else if (a == "printNumFiles") print_num_files = true;
         else if (a == "searchForNonce") search = true;
         else if (a == "seed") seed = strtoull(val().c_str(), nullptr, 10);
+        else if (a == "initialProof") initial = true;
+        else if (a == "nonces") nonces = (uint32_t)strtoul(val().c_str(), nullptr, 10);
+        else if (a == "k1") k1 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
+        else if (a == "k2") k2 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
+        else if (a == "powDifficulty") pow_difficulty = val();
         else { fprintf(stderr, "unknown flag -%s\n", a.c_str()); return 2; }
     }
     if (print_providers) {
@@ -184,6 +196,10 @@ int main(int argc, char **argv) {
     b200post_default_post_config(&cfg);
     if (labels_per_unit) cfg.labels_per_unit = labels_per_unit;
     cfg.min_num_units = 1; cfg.max_num_units = 1u << 20;
+    if (initial && range) { fprintf(stderr, "-initialProof needs the whole POST: it cannot be combined with -fromFile / -toFile\n"); return 2; }
+    if (k1) cfg.k1 = k1;
+    if (k2) cfg.k2 = cfg.k3 = k2;
+    if (!pow_difficulty.empty() && !unhex32(pow_difficulty, cfg.pow_difficulty)) { fprintf(stderr, "-powDifficulty must be a 32-byte hex string\n"); return 2; }
     b200post_setup_opts o;
     b200post_default_setup_opts(&o);
     o.data_dir = datadir.c_str(); o.num_units = (uint32_t)num_units; o.scrypt_n = scrypt_n; o.max_file_size = max_file_size;
@@ -197,6 +213,14 @@ int main(int argc, char **argv) {
     if (int rc = b200post_setup_prepare_files(mgr, &o, node_id, atx_id, from_file, to_file)) {
         fprintf(stderr, "prepare: %s (%d)\n", b200post_last_error(), rc);
         return range && rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;   // a file range outside the POST is a usage error
+    }
+    if (initial) {
+        b200post_prove_opts po{};
+        po.nonces = nonces; po.pow_mode = B200POST_POW_BUILTIN;
+        if (int rc = b200post_setup_request_initial_proof(mgr, &po)) {
+            fprintf(stderr, "initial proof: %s (%d)\n", b200post_last_error(), rc);
+            return rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;
+        }
     }
     signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
     const uint64_t per_file = o.max_file_size / 16, all = (uint64_t)o.num_units * cfg.labels_per_unit;
@@ -225,6 +249,13 @@ int main(int argc, char **argv) {
             printf("files %llu..%llu complete; copy every range's files and one metadata file into one directory, then search the VRF nonce "
                    "with -searchForNonce\n", (unsigned long long)from_file, (unsigned long long)(from_file + (total + per_file - 1) / per_file - 1));
         else if (md.has_nonce) printf("initialization complete; VRF nonce %llu\n", (unsigned long long)md.nonce);
+    }
+    if (initial) {
+        b200post_proof_out proof;
+        const int prc = b200post_setup_initial_proof(mgr, &proof, nullptr);
+        const std::string where = datadir + (datadir.empty() || datadir.back() == '/' ? "" : "/") + "initial_post.json";
+        if (prc == 0) printf("initial proof: nonce %u, written to %s\n", proof.nonce, where.c_str());
+        else printf("no initial proof: %s; the post-service proves from the stored data instead\n", b200post_last_error());
     }
     b200post_setup_manager_free(mgr);
     return 0;

@@ -12,6 +12,9 @@
 // Damaged stored data (b200post_generate_proof_checked): the kernels also return each hit's stored bytes (StoredHit), and
 // the stop rule's tentative winner has its first K2 hits recomputed and compared on the device before the scan may stop
 // on it; damaged hits are dropped (DESIGN.md §5).
+//
+// The scanner, the selection rule, the proof record, the pow step and the verifier gate are declared in prove_internal.h:
+// the setup session's initial proof (initial_proof.cu) runs the same scan over the labels as it writes them.
 #include <algorithm>
 #include <atomic>
 #include <functional>
@@ -30,6 +33,7 @@
 #include "metrics.h"
 #include "postdata_io.h"
 #include "proof_common.h"
+#include "prove_internal.h"
 
 namespace b200post {
 namespace {
@@ -127,11 +131,8 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
     }
 }
 
-// nonce -> its first hit indices (at most K2), ascending; ordered, so ties resolve to the lower nonce
-using HitLists = std::map<uint32_t, std::vector<uint64_t>>;
+}  // namespace
 
-// The selection rule, for one scan and for the merge of several: among nonces with K2 hits, the lowest K2-th hit
-// index wins; ties go to the lower nonce.
 bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
     bool have = false;
     for (const auto &kv : lists) {
@@ -141,191 +142,152 @@ bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vecto
     return have;
 }
 
-// A hit the checked scan keeps: its stored bytes, and whether they have been recomputed and found equal (good) or
-// not yet looked at (pending).  A damaged hit is removed from its list.
-struct KeptHit { uint64_t index; uint8_t label[16]; bool good; };
-using KeptLists = std::map<uint32_t, std::vector<KeptHit>>;   // nonce -> every kept hit, ascending index
+int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
+                  uint64_t num_labels, uint64_t chunk, bool keep_stored) {
+    DeviceEngine *e = engine_for(provider);
+    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (nonces == 0 || nonces % 16 || nonces > 4096 || k1 == 0 || k2 == 0 || num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
+        set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
+        return B200POST_ERR_INVALID_ARGUMENT;
+    }
+    engine_ = e; dev_ = e->device(); nonces_ = nonces; k2_ = k2; chunk_ = chunk;
+    stored_ = keep_stored; rec_ = stored_ ? sizeof(StoredHit) : sizeof(Hit);
+    const uint64_t diff = b200post_proving_difficulty(k1, num_labels);
+    msb_ = (uint32_t)(diff >> 56); lsb_ = diff & 0x00ffffffffffffffull;
+    // hits per chunk are ~ chunk * nonces * K1/numLabels; leave generous slack, cap the buffer at 64 MiB
+    const double expect = (double)chunk * nonces * ((double)k1 / (double)num_labels);
+    hit_cap_ = (uint32_t)std::min<double>(std::max<double>(4.0 * expect + 65536.0, 65536.0), 4.0 * 1024 * 1024);
+    CUDA_TRY(cudaSetDevice(dev_));
+    std::vector<uint8_t> rk((size_t)(nonces / 16) * 176), lazy((size_t)nonces * 176);
+    for (uint32_t g = 0; g < nonces / 16; g++) {
+        uint8_t key[16];
+        cipher_key(challenge, g, pows[g], nullptr, key);
+        const Aes128 a(key);
+        memcpy(rk.data() + (size_t)g * 176, a.rk, 176);
+    }
+    for (uint32_t n = 0; n < nonces; n++) {
+        uint8_t key[16];
+        cipher_key(challenge, n / 16, pows[n / 16], &n, key);
+        const Aes128 a(key);
+        memcpy(lazy.data() + (size_t)n * 176, a.rk, 176);
+    }
+    static AesTables host_tables;
+    static std::once_flag once;
+    std::call_once(once, [] { aes_build_tables(host_tables); });
+    CUDA_TRY(d_rk_.resize(rk.size()));
+    CUDA_TRY(d_lazy_.resize(lazy.size()));
+    CUDA_TRY(d_tables_.resize(1));
+    CUDA_TRY(cudaMemcpy(d_rk_.get(), rk.data(), rk.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(d_lazy_.get(), lazy.data(), lazy.size(), cudaMemcpyHostToDevice));
+    CUDA_TRY(cudaMemcpy(d_tables_.get(), &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice));
+    for (int b = 0; b < 2; b++) {
+        CUDA_TRY(st_[b].create(cudaStreamNonBlocking));
+        CUDA_TRY(ev_[b].create(cudaEventDisableTiming));
+        CUDA_TRY(d_labels_[b].resize(chunk * 16));
+        CUDA_TRY(h_labels_[b].resize(chunk * 16));
+        CUDA_TRY(d_hits_[b].resize((size_t)hit_cap_ * rec_));
+        CUDA_TRY(d_nhits_[b].resize(1));
+        CUDA_TRY(h_hits_[b].resize((size_t)hit_cap_ * rec_));
+        CUDA_TRY(h_nhits_[b].resize(1));
+        CUDA_TRY(h_ncands_[b].resize(1));
+    }
+    // lazy-cipher candidates: one ciphertext byte in 256 equals the MSB; 2x slack, shared by both buffers
+    // (chunks are processed in stream order on alternating streams, so the queue is fenced by events below)
+    cand_cap_ = (uint32_t)std::min<uint64_t>((chunk * nonces) / 128 + 65536, 1u << 27);
+    CUDA_TRY(d_cands_.resize(cand_cap_));
+    CUDA_TRY(d_ncands_.resize(2));
+    cudaDeviceProp p;
+    CUDA_TRY(cudaGetDeviceProperties(&p, dev_));
+    grid_ = (uint32_t)p.multiProcessorCount * 6;   // 6 CTAs x 32 KiB of lane-replicated AES table per SM
+    return B200POST_OK;
+}
 
-// Streaming scan state: device buffers, keys, per-nonce hit lists.  With keep_stored (the checked proof) the kernels
-// write StoredHit records and every hit is kept with its bytes (kept()); otherwise the first K2 per nonce (lists()).
-class Scanner {
-public:
-    ~Scanner() { if (dev_ >= 0) { cudaSetDevice(dev_); drain(); } }   // the members free themselves on the scan's device
-    int init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
-             uint64_t num_labels, uint64_t chunk, bool keep_stored = false) {
-        DeviceEngine *e = engine_for(provider);
-        if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
-        if (nonces == 0 || nonces % 16 || nonces > 4096 || k1 == 0 || k2 == 0 || num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
-            set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
-            return B200POST_ERR_INVALID_ARGUMENT;
-        }
-        engine_ = e; dev_ = e->device(); nonces_ = nonces; k2_ = k2; chunk_ = chunk;
-        stored_ = keep_stored; rec_ = stored_ ? sizeof(StoredHit) : sizeof(Hit);
-        const uint64_t diff = b200post_proving_difficulty(k1, num_labels);
-        msb_ = (uint32_t)(diff >> 56); lsb_ = diff & 0x00ffffffffffffffull;
-        // hits per chunk are ~ chunk * nonces * K1/numLabels; leave generous slack, cap the buffer at 64 MiB
-        const double expect = (double)chunk * nonces * ((double)k1 / (double)num_labels);
-        hit_cap_ = (uint32_t)std::min<double>(std::max<double>(4.0 * expect + 65536.0, 65536.0), 4.0 * 1024 * 1024);
-        CUDA_TRY(cudaSetDevice(dev_));
-        std::vector<uint8_t> rk((size_t)(nonces / 16) * 176), lazy((size_t)nonces * 176);
-        for (uint32_t g = 0; g < nonces / 16; g++) {
-            uint8_t key[16];
-            cipher_key(challenge, g, pows[g], nullptr, key);
-            const Aes128 a(key);
-            memcpy(rk.data() + (size_t)g * 176, a.rk, 176);
-        }
-        for (uint32_t n = 0; n < nonces; n++) {
-            uint8_t key[16];
-            cipher_key(challenge, n / 16, pows[n / 16], &n, key);
-            const Aes128 a(key);
-            memcpy(lazy.data() + (size_t)n * 176, a.rk, 176);
-        }
-        static AesTables host_tables;
-        static std::once_flag once;
-        std::call_once(once, [] { aes_build_tables(host_tables); });
-        CUDA_TRY(d_rk_.resize(rk.size()));
-        CUDA_TRY(d_lazy_.resize(lazy.size()));
-        CUDA_TRY(d_tables_.resize(1));
-        CUDA_TRY(cudaMemcpy(d_rk_.get(), rk.data(), rk.size(), cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(d_lazy_.get(), lazy.data(), lazy.size(), cudaMemcpyHostToDevice));
-        CUDA_TRY(cudaMemcpy(d_tables_.get(), &host_tables, sizeof(AesTables), cudaMemcpyHostToDevice));
-        for (int b = 0; b < 2; b++) {
-            CUDA_TRY(st_[b].create(cudaStreamNonBlocking));
-            CUDA_TRY(ev_[b].create(cudaEventDisableTiming));
-            CUDA_TRY(d_labels_[b].resize(chunk * 16));
-            CUDA_TRY(h_labels_[b].resize(chunk * 16));
-            CUDA_TRY(d_hits_[b].resize((size_t)hit_cap_ * rec_));
-            CUDA_TRY(d_nhits_[b].resize(1));
-            CUDA_TRY(h_hits_[b].resize((size_t)hit_cap_ * rec_));
-            CUDA_TRY(h_nhits_[b].resize(1));
-            CUDA_TRY(h_ncands_[b].resize(1));
-        }
-        // lazy-cipher candidates: one ciphertext byte in 256 equals the MSB; 2x slack, shared by both buffers
-        // (chunks are processed in stream order on alternating streams, so the queue is fenced by events below)
-        cand_cap_ = (uint32_t)std::min<uint64_t>((chunk * nonces) / 128 + 65536, 1u << 27);
-        CUDA_TRY(d_cands_.resize(cand_cap_));
-        CUDA_TRY(d_ncands_.resize(2));
-        cudaDeviceProp p;
-        CUDA_TRY(cudaGetDeviceProperties(&p, dev_));
-        grid_ = (uint32_t)p.multiProcessorCount * 6;   // 6 CTAs x 32 KiB of lane-replicated AES table per SM
-        return B200POST_OK;
-    }
-    uint8_t *staging(int b) { return h_labels_[b].get(); }
-    // enqueue chunk in staging(b): labels [first, first+count)
-    int submit(int b, uint64_t first, uint32_t count) {
-        CUDA_TRY(cudaMemcpyAsync(d_labels_[b].get(), h_labels_[b].get(), (size_t)count * 16, cudaMemcpyHostToDevice, st_[b].get()));
-        CUDA_TRY(cudaMemsetAsync(d_nhits_[b].get(), 0, 4, st_[b].get()));
-        // the single candidate queue is reused by consecutive chunks: wait for the other stream's lazy pass
-        if (pending_[b ^ 1]) CUDA_TRY(cudaStreamWaitEvent(st_[b].get(), ev_[b ^ 1].get(), 0));
-        CUDA_TRY(cudaMemsetAsync(d_ncands_.get(), 0, 8, st_[b].get()));
-        cudaStream_t st = st_[b].get();
-        const uint4 *labels = reinterpret_cast<const uint4 *>(d_labels_[b].get());
-        if (stored_) launch(st, labels, first, count, reinterpret_cast<StoredHit *>(d_hits_[b].get()), d_nhits_[b].get());
-        else launch(st, labels, first, count, reinterpret_cast<Hit *>(d_hits_[b].get()), d_nhits_[b].get());
-        g_launches += 2;
-        CUDA_TRY(cudaGetLastError());
-        CUDA_TRY(cudaMemcpyAsync(h_ncands_[b].get(), d_ncands_.get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
-        CUDA_TRY(cudaMemcpyAsync(h_nhits_[b].get(), d_nhits_[b].get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
-        CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * rec_, cudaMemcpyDeviceToHost, st_[b].get()));
-        CUDA_TRY(cudaEventRecord(ev_[b].get(), st_[b].get()));
-        pending_[b] = true; count_[b] = count;
-        return B200POST_OK;
-    }
-    // wait for chunk b and fold its hits in.  The fold (hit lists, full nonces, labels scanned) happens under
-    // `fold_mu` when given, so that other threads may read that state under the same mutex.
-    int collect(int b, std::mutex *fold_mu = nullptr) {
-        if (!pending_[b]) return B200POST_OK;
-        CUDA_TRY(cudaEventSynchronize(ev_[b].get()));
-        pending_[b] = false;
-        const uint32_t n = *h_nhits_[b].get();
-        if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
-        if (stored_) return fold_stored(b, n, fold_mu);
-        const Hit *rec = reinterpret_cast<const Hit *>(h_hits_[b].get());
-        std::vector<Hit> v(rec, rec + n);
-        std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
-        std::unique_lock<std::mutex> lk;
-        if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
-        for (const Hit &h : v) {
-            std::vector<uint64_t> &l = lists_[h.nonce];
-            if (l.size() < k2_ && (l.push_back(h.index), l.size() == k2_)) full_++;
-        }
-        scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
-        return B200POST_OK;
-    }
-    int fold_stored(int b, uint32_t n, std::mutex *fold_mu) {
-        const StoredHit *rec = reinterpret_cast<const StoredHit *>(h_hits_[b].get());
-        std::vector<StoredHit> v(rec, rec + n);
-        std::sort(v.begin(), v.end(), [](const StoredHit &x, const StoredHit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
-        std::unique_lock<std::mutex> lk;
-        if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
-        for (const StoredHit &h : v) {
-            KeptHit k{h.index, {}, false};
-            memcpy(k.label, &h.label, 16);
-            kept_[h.nonce].push_back(k);
-        }
-        scanned_ += count_[b];
-        return B200POST_OK;
-    }
-    // wait for whatever is still in flight, without folding it (error and cancel paths)
-    void drain() {
-        for (int b = 0; b < 2; b++) if (pending_[b]) { cudaEventSynchronize(ev_[b].get()); pending_[b] = false; }
-    }
-    const HitLists &lists() const { return lists_; }
-    const KeptLists &kept() const { return kept_; }
-    KeptLists &kept() { return kept_; }
-    bool any_full() const { return full_ > 0; }          // some nonce has K2 hits
-    // every nonce has K2 hits (kept: K2 good ones): later labels change no nonce's first K2 (usable) hits
-    bool saturated() const { return stored_ ? count_kept(true) == nonces_ : full_ == nonces_; }
-    // nonces with at least K2 kept hits (good ones only, or good and pending)
-    uint32_t count_kept(bool good_only) const {
-        uint32_t full = 0;
-        for (const auto &kv : kept_) {
-            size_t c = 0;
-            for (const KeptHit &k : kv.second) if ((c += !good_only || k.good) >= k2_) break;
-            full += c >= k2_;
-        }
-        return full;
-    }
-    uint32_t nonces() const { return nonces_; }
-    uint64_t scanned() const { return scanned_; }
-    int device() const { return dev_; }
-    DeviceEngine *engine() const { return engine_; }
+template <class Rec>
+void Scanner::launch(cudaStream_t st, const uint4 *labels, uint64_t first, uint32_t count, Rec *hits, uint32_t *n_hits) {
+    prove_scan_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
+                                                               msb_, d_tables_.get(), hits, hit_cap_, n_hits, d_cands_.get(), cand_cap_,
+                                                               d_ncands_.get());
+    prove_lazy_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
+                                                               reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
+                                                               hits, hit_cap_, n_hits);
+}
 
-private:
-    template <class Rec>
-    void launch(cudaStream_t st, const uint4 *labels, uint64_t first, uint32_t count, Rec *hits, uint32_t *n_hits) {
-        prove_scan_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
-                                                                   msb_, d_tables_.get(), hits, hit_cap_, n_hits, d_cands_.get(), cand_cap_,
-                                                                   d_ncands_.get());
-        prove_lazy_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
-                                                                   reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
-                                                                   hits, hit_cap_, n_hits);
-    }
+int Scanner::submit(int b, uint64_t first, uint32_t count) {
+    CUDA_TRY(cudaMemcpyAsync(d_labels_[b].get(), h_labels_[b].get(), (size_t)count * 16, cudaMemcpyHostToDevice, st_[b].get()));
+    CUDA_TRY(cudaMemsetAsync(d_nhits_[b].get(), 0, 4, st_[b].get()));
+    // the single candidate queue is reused by consecutive chunks: wait for the other stream's lazy pass
+    if (pending_[b ^ 1]) CUDA_TRY(cudaStreamWaitEvent(st_[b].get(), ev_[b ^ 1].get(), 0));
+    CUDA_TRY(cudaMemsetAsync(d_ncands_.get(), 0, 8, st_[b].get()));
+    cudaStream_t st = st_[b].get();
+    const uint4 *labels = reinterpret_cast<const uint4 *>(d_labels_[b].get());
+    if (stored_) launch(st, labels, first, count, reinterpret_cast<StoredHit *>(d_hits_[b].get()), d_nhits_[b].get());
+    else launch(st, labels, first, count, reinterpret_cast<Hit *>(d_hits_[b].get()), d_nhits_[b].get());
+    g_launches += 2;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(h_ncands_[b].get(), d_ncands_.get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
+    CUDA_TRY(cudaMemcpyAsync(h_nhits_[b].get(), d_nhits_[b].get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
+    CUDA_TRY(cudaMemcpyAsync(h_hits_[b].get(), d_hits_[b].get(), (size_t)hit_cap_ * rec_, cudaMemcpyDeviceToHost, st_[b].get()));
+    CUDA_TRY(cudaEventRecord(ev_[b].get(), st_[b].get()));
+    pending_[b] = true; count_[b] = count;
+    return B200POST_OK;
+}
 
-    DeviceEngine *engine_ = nullptr;
-    int dev_ = -1;
-    uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0, full_ = 0;
-    uint64_t lsb_ = 0, chunk_ = 0, scanned_ = 0;
-    bool stored_ = false;
-    size_t rec_ = sizeof(Hit);   // bytes per hit record (Hit or StoredHit)
-    DeviceBuffer<uint8_t> d_rk_, d_lazy_;
-    DeviceBuffer<AesTables> d_tables_;
-    Stream st_[2];
-    Event ev_[2];
-    DeviceBuffer<uint8_t> d_labels_[2];
-    PinnedBuffer<uint8_t> h_labels_[2];
-    DeviceBuffer<uint8_t> d_hits_[2];   // hit_cap_ records of rec_ bytes
-    PinnedBuffer<uint8_t> h_hits_[2];
-    DeviceBuffer<uint32_t> d_nhits_[2];
-    PinnedBuffer<uint32_t> h_nhits_[2], h_ncands_[2];
-    DeviceBuffer<uint2> d_cands_;
-    DeviceBuffer<uint32_t> d_ncands_;
-    uint32_t cand_cap_ = 0;
-    bool pending_[2] = {false, false};
-    uint32_t count_[2] = {0, 0};
-    HitLists lists_;
-    KeptLists kept_;
-};
+int Scanner::collect(int b, std::mutex *fold_mu) {
+    if (!pending_[b]) return B200POST_OK;
+    CUDA_TRY(cudaEventSynchronize(ev_[b].get()));
+    pending_[b] = false;
+    const uint32_t n = *h_nhits_[b].get();
+    if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
+    if (stored_) return fold_stored(b, n, fold_mu);
+    const Hit *rec = reinterpret_cast<const Hit *>(h_hits_[b].get());
+    std::vector<Hit> v(rec, rec + n);
+    std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+    std::unique_lock<std::mutex> lk;
+    if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
+    for (const Hit &h : v) {
+        std::vector<uint64_t> &l = lists_[h.nonce];
+        if (l.size() < k2_ && (l.push_back(h.index), l.size() == k2_)) full_++;
+    }
+    scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
+    return B200POST_OK;
+}
+
+int Scanner::fold_stored(int b, uint32_t n, std::mutex *fold_mu) {
+    const StoredHit *rec = reinterpret_cast<const StoredHit *>(h_hits_[b].get());
+    std::vector<StoredHit> v(rec, rec + n);
+    std::sort(v.begin(), v.end(), [](const StoredHit &x, const StoredHit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+    std::unique_lock<std::mutex> lk;
+    if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
+    for (const StoredHit &h : v) {
+        KeptHit k{h.index, {}, false};
+        memcpy(k.label, &h.label, 16);
+        kept_[h.nonce].push_back(k);
+    }
+    scanned_ += count_[b];
+    return B200POST_OK;
+}
+
+void Scanner::drain() {
+    for (int b = 0; b < 2; b++) if (pending_[b]) { cudaEventSynchronize(ev_[b].get()); pending_[b] = false; }
+}
+
+void Scanner::restore(const HitLists &lists) {
+    lists_ = lists;
+    full_ = 0;
+    for (const auto &kv : lists_) full_ += kv.second.size() >= k2_;
+}
+
+uint32_t Scanner::count_kept(bool good_only) const {
+    uint32_t full = 0;
+    for (const auto &kv : kept_) {
+        size_t c = 0;
+        for (const KeptHit &k : kv.second) if ((c += !good_only || k.good) >= k2_) break;
+        full += c >= k2_;
+    }
+    return full;
+}
+
+namespace {
 
 // One contiguous label range [lo, hi) of a scan, streamed through its own Scanner.
 struct Shard {
@@ -567,9 +529,10 @@ private:
     std::atomic<bool> abort_{false};
 };
 
-int write_proof(const ShardedScan &scan, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint64_t num_labels,
+}  // namespace
+
+int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint64_t num_labels,
                 b200post_proof_out *out) {
-    const uint64_t scanned = scan.scanned();
     metrics().prove_labels_scanned_total += scanned; metrics().proofs_generated_total++;
     memset(out, 0, sizeof *out);
     out->nonce = nonce; out->pow = pows[nonce / 16]; out->labels_scanned = scanned;
@@ -580,11 +543,66 @@ int write_proof(const ShardedScan &scan, uint32_t nonce, const std::vector<uint6
 
 const char *const kNoProof = "no proof found: no nonce reached K2 qualifying labels";
 
+int check_pow_mode(const b200post_prove_opts &o) {
+    if (o.pow_mode > B200POST_POW_SKIP || (o.pow_mode == B200POST_POW_CALLBACK && !o.pow_prove)) {
+        set_error("pow_mode CALLBACK needs a pow_prove function; to prove without k2pow ask for B200POST_POW_SKIP explicitly");
+        return B200POST_ERR_UNSUPPORTED;
+    }
+    return B200POST_OK;
+}
+
+int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const uint8_t node_id[32], uint32_t num_units,
+              const uint8_t cfg_difficulty[32], const uint32_t *providers, int n_providers, std::vector<uint64_t> *pows,
+              const volatile int *cancel) {
+    pows->assign(o.nonces / 16, 0);
+    if (o.pow_mode == B200POST_POW_SKIP) return B200POST_OK;
+    uint8_t scaled[32];
+    div256_u32(cfg_difficulty, num_units, scaled);
+    if (o.pow_mode == B200POST_POW_CALLBACK) {
+        for (uint32_t g = 0; g < o.nonces / 16; g++)
+            if (o.pow_prove(o.pow_ctx, (uint8_t)g, challenge, scaled, node_id, &(*pows)[g]) != 0) { set_error("k2pow hook failed"); return B200POST_ERR_INVALID_ARGUMENT; }
+        return B200POST_OK;
+    }
+    // the k2pow step of NIPostBuilder.Proof (activation/nipost.go:171 -> post-service): RandomX nonce search on the device
+    b200post_k2pow_params kp{};
+    kp.cache_key = o.pow_cache_key; kp.cache_key_len = o.pow_cache_key_len;
+    memcpy(kp.challenge8, challenge, 8);
+    memcpy(kp.node_id, node_id, 32);
+    memcpy(kp.difficulty, scaled, 32);
+    const int rc = b200post_k2pow_search_groups_multi(providers, n_providers, &kp, o.nonces / 16, 0, pows->data(), nullptr, cancel);
+    if (rc) return rc;
+    for (uint64_t v : *pows) if (v == B200POST_K2POW_NOT_FOUND) { set_error("k2pow: nonce space exhausted"); return B200POST_ERR_INVALID_PROOF; }
+    return B200POST_OK;
+}
+
+int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o,
+               const b200post_proof_metadata &meta, b200post_proof_out *out) {
+    b200post_verify_params vp{};
+    vp.k1 = cfg.k1; vp.k2 = cfg.k2; vp.scrypt_n = scrypt_n;
+    memcpy(vp.pow_difficulty, cfg.pow_difficulty, 32);
+    b200post_verifier_opts vo{};
+    vo.pow_mode = o.pow_mode == B200POST_POW_BUILTIN ? B200POST_POW_BUILTIN : B200POST_POW_SKIP;
+    vo.pow_cache_key = o.pow_cache_key; vo.pow_cache_key_len = o.pow_cache_key_len;
+    const b200post_proof proof{out->nonce, out->indices, out->indices_len, out->pow};
+    int status = B200POST_OK;
+    uint64_t bad = 0;
+    const int rc = b200post_verify_batch(provider, 1, &proof, &meta, &vp, nullptr, &vo, &status, &bad);
+    if (rc) return rc;
+    if (status != B200POST_OK) {
+        memset(out, 0, sizeof *out);
+        set_error(bad == ~0ull ? "the proof failed the verifier's k2pow check" : "the proof failed the verifier at position " + std::to_string(bad));
+        return B200POST_ERR_INVALID_PROOF;
+    }
+    return B200POST_OK;
+}
+
+namespace {
+
 int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
     uint32_t nonce = 0;
     std::vector<uint64_t> idx;
     if (!pick_winner(scan.merged(), k2, &nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    return write_proof(scan, nonce, idx, pows, num_labels, out);
+    return write_proof(scan.scanned(), nonce, idx, pows, num_labels, out);
 }
 
 // The checked proof's decision step: recheck rounds until the winner over usable hits is known, then the report.
@@ -602,7 +620,7 @@ int finish_checked(ShardedScan &scan, const uint64_t *pows, uint64_t num_labels,
     metrics().prove_damaged_labels_total += check->damaged;
     if (rc) return rc;
     if (!have) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    return write_proof(scan, nonce, idx, pows, num_labels, out);
+    return write_proof(scan.scanned(), nonce, idx, pows, num_labels, out);
 }
 
 }  // namespace
@@ -697,28 +715,9 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
         return B200POST_ERR_IO;
     }
     // k2pow per nonce group (RandomX upstream) through the caller's hook
-    std::vector<uint64_t> pows(o.nonces / 16, 0);
-    if (o.pow_mode > B200POST_POW_SKIP || (o.pow_mode == B200POST_POW_CALLBACK && !o.pow_prove)) {
-        set_error("pow_mode CALLBACK needs a pow_prove function; to prove without k2pow ask for B200POST_POW_SKIP explicitly");
-        return B200POST_ERR_UNSUPPORTED;
-    }
-    if (o.pow_mode != B200POST_POW_SKIP) {
-        uint8_t scaled[32];
-        div256_u32(cfg->pow_difficulty, md.num_units, scaled);
-        if (o.pow_mode == B200POST_POW_CALLBACK) {
-            for (uint32_t g = 0; g < o.nonces / 16; g++)
-                if (o.pow_prove(o.pow_ctx, (uint8_t)g, challenge, scaled, md.node_id, &pows[g]) != 0) { set_error("k2pow hook failed"); return B200POST_ERR_INVALID_ARGUMENT; }
-        } else {
-            // the k2pow step of NIPostBuilder.Proof (activation/nipost.go:171 -> post-service): RandomX nonce search on the device
-            b200post_k2pow_params kp{};
-            kp.cache_key = o.pow_cache_key; kp.cache_key_len = o.pow_cache_key_len;
-            memcpy(kp.challenge8, challenge, 8);
-            memcpy(kp.node_id, md.node_id, 32);
-            memcpy(kp.difficulty, scaled, 32);
-            if ((rc = b200post_k2pow_search_groups_multi(providers, n_providers, &kp, o.nonces / 16, 0, pows.data(), nullptr, cancel))) return rc;
-            for (uint64_t v : pows) if (v == B200POST_K2POW_NOT_FOUND) { set_error("k2pow: nonce space exhausted"); return B200POST_ERR_INVALID_PROOF; }
-        }
-    }
+    std::vector<uint64_t> pows;
+    if ((rc = check_pow_mode(o))) return rc;
+    if ((rc = find_pows(o, challenge, md.node_id, md.num_units, cfg->pow_difficulty, providers, n_providers, &pows, cancel))) return rc;
     // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
     const uint64_t chunk = std::min<uint64_t>(o.chunk_labels, num_labels);
     ShardedScan scan((size_t)n_providers, o.nonces, cfg->k2);
@@ -748,21 +747,7 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
     meta.num_units = md.num_units; meta.labels_per_unit = md.labels_per_unit;
     if (check) {
         // the gate: a proof this library's own verifier rejects is never handed out
-        b200post_verify_params vp{};
-        vp.k1 = cfg->k1; vp.k2 = cfg->k2; vp.scrypt_n = md.scrypt_n;
-        memcpy(vp.pow_difficulty, cfg->pow_difficulty, 32);
-        b200post_verifier_opts vo{};
-        vo.pow_mode = o.pow_mode == B200POST_POW_BUILTIN ? B200POST_POW_BUILTIN : B200POST_POW_SKIP;
-        vo.pow_cache_key = o.pow_cache_key; vo.pow_cache_key_len = o.pow_cache_key_len;
-        const b200post_proof proof{out->nonce, out->indices, out->indices_len, out->pow};
-        int status = B200POST_OK;
-        uint64_t bad = 0;
-        if ((rc = b200post_verify_batch(providers[0], 1, &proof, &meta, &vp, nullptr, &vo, &status, &bad))) return rc;
-        if (status != B200POST_OK) {
-            memset(out, 0, sizeof *out);
-            set_error(bad == ~0ull ? "the proof failed the verifier's k2pow check" : "the proof failed the verifier at position " + std::to_string(bad));
-            return B200POST_ERR_INVALID_PROOF;
-        }
+        if ((rc = gate_proof(providers[0], *cfg, md.scrypt_n, o, meta, out))) return rc;
         check->proof_verified = 1;
     }
     if (meta_out) *meta_out = meta;

@@ -157,6 +157,16 @@ void RandomxEngine::last_timing(double *total_ms, double *vm_ms, uint64_t *hashe
     if (vm_launches) *vm_launches = vm_launches_;
 }
 
+void RandomxEngine::release() {
+    std::lock_guard<std::mutex> lk(mu_);
+    cudaSetDevice(dev_);
+    if (stream_.get()) cudaStreamSynchronize(stream_.get());
+    release_batch();
+    d_dataset_.reset();
+    d_inputs_.reset();
+    key_.clear();
+}
+
 int RandomxEngine::hash_inputs(const std::string &key, const uint8_t *inputs, size_t input_len, size_t n, uint8_t *out32) {
     std::lock_guard<std::mutex> lk(mu_);
     int rc = ensure_dataset(key);
@@ -251,6 +261,16 @@ RandomxEngine *randomx_engine_for(uint32_t provider) {
 void randomx_shutdown_all() {
     std::lock_guard<std::mutex> lk(g_rx_mu);
     g_rx.clear();
+}
+
+void randomx_release(int device) {
+    RandomxEngine *e = nullptr;
+    {
+        std::lock_guard<std::mutex> lk(g_rx_mu);
+        auto it = g_rx.find(device);
+        if (it != g_rx.end()) e = it->second.get();
+    }
+    if (e) e->release();
 }
 
 }  // namespace b200post

@@ -28,6 +28,8 @@ public:
     // dataset items [first_item, first_item + count) of `key` to host memory (64 bytes each; the range is checked by the caller)
     int dataset_read(const std::string &key, uint64_t first_item, uint64_t count, uint64_t *out);
     void last_timing(double *total_ms, double *vm_ms, uint64_t *hashes, uint64_t *vm_launches);
+    // frees the dataset and the batch buffers (~14 GiB); the next call rebuilds them
+    void release();
 
 private:
     int ensure_dataset(const std::string &key);
@@ -57,5 +59,7 @@ private:
 
 RandomxEngine *randomx_engine_for(uint32_t provider);
 void randomx_shutdown_all();
+// release() of the engine on `device`, if one was created: its HBM goes back to the device, the engine stays usable
+void randomx_release(int device);
 
 }  // namespace b200post

@@ -13,13 +13,15 @@
 #include <atomic>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
 
-#include "../../include/b200post_setup.h"
+#include "../../include/b200post_prove.h"
 #include "engine.h"
 #include "host_hash.h"
+#include "initial_proof.h"
 #include "metrics.h"
 #include "setup_internal.h"
 
@@ -170,6 +172,74 @@ int load_metadata(const std::string &dir, b200post_post_metadata *m, bool *missi
     return B200POST_OK;
 }
 
+const uint8_t kZeroChallenge[32] = {0};
+
+// initial_post.json: the proof, with the fields that decide whether it still answers the ZeroChallenge
+int save_initial_proof(const std::string &dir, const b200post_proof_metadata &pm, const b200post_post_config &cfg, uint32_t nonces,
+                       const b200post_proof_out &p) {
+    std::string j = "{\n";
+    j += " \"NodeId\": \"" + b64(pm.node_id, 32) + "\",\n";
+    j += " \"CommitmentAtxId\": \"" + b64(pm.commitment_atx_id, 32) + "\",\n";
+    j += " \"NumUnits\": " + std::to_string(pm.num_units) + ",\n";
+    j += " \"LabelsPerUnit\": " + std::to_string(pm.labels_per_unit) + ",\n";
+    j += " \"K1\": " + std::to_string(cfg.k1) + ",\n";
+    j += " \"K2\": " + std::to_string(cfg.k2) + ",\n";
+    j += " \"Nonces\": " + std::to_string(nonces) + ",\n";
+    j += " \"PowDifficulty\": \"" + hex(cfg.pow_difficulty, 32) + "\",\n";
+    j += " \"Challenge\": \"" + b64(pm.challenge, 32) + "\",\n";
+    j += " \"Nonce\": " + std::to_string(p.nonce) + ",\n";
+    j += " \"Indices\": \"" + b64(p.indices, p.indices_len) + "\",\n";
+    j += " \"Pow\": " + std::to_string(p.pow) + "\n}\n";
+    const std::string tmp = path_join(dir, std::string(kInitialProofFile) + ".tmp"), fin = path_join(dir, kInitialProofFile);
+    FILE *f = fopen(tmp.c_str(), "w");
+    if (!f) return io_error("open " + tmp);
+    const bool ok = fwrite(j.data(), 1, j.size(), f) == j.size();
+    if (fclose(f) != 0 || !ok) return io_error("write " + tmp);
+    if (rename(tmp.c_str(), fin.c_str()) != 0) return io_error("rename " + tmp);
+    return B200POST_OK;
+}
+
+int no_initial_proof(const std::string &why) {
+    set_error("no initial proof: " + why);
+    return B200POST_ERR_IO;
+}
+
+// the proof in initial_post.json if it answers the ZeroChallenge for this POST (md), cfg and nonce count
+int load_initial_proof(const std::string &dir, const b200post_post_metadata &md, const b200post_post_config &cfg, uint32_t nonces,
+                       b200post_proof_out *out, b200post_proof_metadata *pm) {
+    FILE *f = fopen(path_join(dir, kInitialProofFile).c_str(), "r");
+    if (!f) return no_initial_proof(std::string(kInitialProofFile) + " is absent");
+    std::string doc;
+    char buf[4096];
+    size_t n;
+    while ((n = fread(buf, 1, sizeof buf, f)) > 0) doc.append(buf, n);
+    fclose(f);
+    const uint64_t num_labels = (uint64_t)md.num_units * md.labels_per_unit;
+    const size_t packed = num_labels ? ((size_t)cfg.k2 * b200post_bits_per_index(num_labels) + 7) / 8 : 0;
+    b200post_proof_metadata m{};
+    b200post_proof_out p{};
+    uint8_t diff[32];
+    std::string s;
+    uint64_t units, lpu, k1, k2, nn, nonce, pow;
+    if (!json_raw(doc, "NodeId", &s) || !unb64(s, m.node_id, 32) || !json_raw(doc, "CommitmentAtxId", &s) ||
+        !unb64(s, m.commitment_atx_id, 32) || !json_raw(doc, "Challenge", &s) || !unb64(s, m.challenge, 32) ||
+        !json_raw(doc, "PowDifficulty", &s) || !unhex(s, diff, 32) || !json_u64(doc, "NumUnits", &units) ||
+        !json_u64(doc, "LabelsPerUnit", &lpu) || !json_u64(doc, "K1", &k1) || !json_u64(doc, "K2", &k2) ||
+        !json_u64(doc, "Nonces", &nn) || !json_u64(doc, "Nonce", &nonce) || !json_u64(doc, "Pow", &pow) ||
+        packed == 0 || packed > sizeof p.indices || !json_raw(doc, "Indices", &s) || !unb64(s, p.indices, packed))
+        return no_initial_proof(std::string(kInitialProofFile) + " is unreadable");
+    if (memcmp(m.node_id, md.node_id, 32) || memcmp(m.commitment_atx_id, md.commitment_atx_id, 32)) return no_initial_proof("it belongs to another identity");
+    if (units != md.num_units || lpu != md.labels_per_unit || lpu != cfg.labels_per_unit) return no_initial_proof("it was made for another POST size");
+    if (k1 != cfg.k1 || k2 != cfg.k2 || memcmp(diff, cfg.pow_difficulty, 32)) return no_initial_proof("it was made under another K1, K2 or pow difficulty");
+    if (nn != nonces) return no_initial_proof("it was made for another nonce count");
+    if (memcmp(m.challenge, kZeroChallenge, 32) || nonce >= nonces) return no_initial_proof("it does not answer the zero challenge");
+    m.num_units = md.num_units; m.labels_per_unit = md.labels_per_unit;
+    p.nonce = (uint32_t)nonce; p.pow = pow; p.indices_len = packed; p.labels_scanned = num_labels;
+    *out = p;
+    if (pm) *pm = m;
+    return B200POST_OK;
+}
+
 }  // namespace
 
 namespace b200post {
@@ -221,6 +291,14 @@ struct b200post_setup_manager {
     uint64_t num_labels = 0;
     uint64_t range_lo = 0, range_hi = 0;        // the session writes labels [range_lo, range_hi)
     bool range() const { return range_lo != 0 || range_hi != num_labels; }
+    // the initial proof: asked for between prepare and start (b200post_setup_request_initial_proof), produced by start
+    bool want_proof = false;
+    InitialProofRequest proof_req;
+    bool proof_done = false;                    // the last session that asked for it completed
+    int proof_rc = B200POST_OK;                 // its outcome: OK, or INVALID_PROOF with proof_err
+    std::string proof_err;
+    b200post_proof_out proof{};
+    b200post_proof_metadata proof_meta{};
 };
 
 namespace {
@@ -274,6 +352,10 @@ int b200post_setup_prepare_files(b200post_setup_manager *m, const b200post_setup
         set_error("post setup session in progress");   // activation/post.go:345
         return B200POST_ERR_STATE;
     }
+    // a request belongs to one prepared session, and so does its outcome
+    m->want_proof = m->proof_done = false;
+    m->proof_rc = B200POST_OK; m->proof_err.clear();
+    m->proof = b200post_proof_out{}; m->proof_meta = b200post_proof_metadata{};
     // ---- option validation (initialization.NewInitializer / config.Validate upstream; errors -> state Error, post.go:362-365)
     const b200post_post_config &c = m->cfg;
     if (!o->data_dir || !*o->data_dir) return fail_state(m, B200POST_ERR_INVALID_ARGUMENT, "invalid `opts.DataDir`: empty");
@@ -373,6 +455,22 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     uint8_t diff[32];
     if (m->meta.has_nonce) memcpy(diff, m->meta.nonce_value, 32); else vrf_difficulty(num_labels, diff);
 
+    // the initial proof: pows, state and the rescan of what is already on disk come before the first batch
+    std::unique_ptr<InitialProofScan> ip;
+    if (m->want_proof) {
+        m->proof_done = false;
+        if (m->opts.provider_id == B200POST_PROVIDER_UNSET) {
+            set_error("no provider specified");
+            return finish(B200POST_SETUP_ERROR, B200POST_ERR_NO_PROVIDER);
+        }
+        ip.reset(new InitialProofScan);
+        const int rc = ip->begin(m->proof_req, m->data_dir, m->meta, m->cfg, m->opts.provider_id, written, batch, cancel);
+        if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
+        if (rc) return finish(B200POST_SETUP_ERROR, rc);
+    }
+    // from here on a stop or failure first saves the initial proof's scan state
+    auto end = [&](int32_t state, int rc) { if (ip) ip->stop(); return finish(state, rc); };
+
     std::vector<uint8_t> buf;
     uint64_t n_batches = 0;
     auto note_nonce = [&](const b200post_vrf_nonce &nn) -> int {
@@ -383,19 +481,23 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     };
 
     while (written < hi) {
-        if (cancel && *cancel) { set_error("cancelled"); return finish(B200POST_SETUP_STOPPED, B200POST_ERR_CANCELLED); }
+        if (cancel && *cancel) { set_error("cancelled"); return end(B200POST_SETUP_STOPPED, B200POST_ERR_CANCELLED); }
         const uint64_t file_idx = written / per_file, in_file = written % per_file;
         const uint64_t count = std::min<uint64_t>({batch, per_file - in_file, hi - written});
-        buf.resize((size_t)count * 16);
+        int rc;
+        // with an initial proof the batch is computed into the scan's pinned staging, which the file is written from
+        uint8_t *labels = nullptr;
+        if (ip && (rc = ip->buffer(count, &labels))) return end(B200POST_SETUP_ERROR, rc);
+        if (!labels) { buf.resize((size_t)count * 16); labels = buf.data(); }
         b200post_vrf_nonce nn;
-        int rc = compute_labels(m->opts.provider_id, m->opts.scrypt_n, commitment, written, count, buf.data(), range ? nullptr : diff,
-                                &nn, cancel);
-        if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
-        if (rc) return finish(B200POST_SETUP_ERROR, rc);
+        rc = compute_labels(m->opts.provider_id, m->opts.scrypt_n, commitment, written, count, labels, range ? nullptr : diff,
+                            &nn, cancel);
+        if (rc == B200POST_ERR_CANCELLED) return end(B200POST_SETUP_STOPPED, rc);
+        if (rc) return end(B200POST_SETUP_ERROR, rc);
         // ErrReferenceLabelMismatch contract (activation/post.go:299-312): every self_check_every batches one label of the
         // batch is recomputed ON THE HOST CPU (reference_label.cpp: the kernels' own arithmetic header compiled for the
         // host) and compared with what the device wrote — independent of the device, its kernels' scheduling and memory.
-        if (options().debug_corrupt_next_batch.exchange(0) != 0 && count) buf[((n_batches * 7) % count) * 16 + 3] ^= 0x40;   // fault injection (tests)
+        if (options().debug_corrupt_next_batch.exchange(0) != 0 && count) labels[((n_batches * 7) % count) * 16 + 3] ^= 0x40;   // fault injection (tests)
         if (n_batches % m->opts.self_check_every == 0) {
             uint8_t ref[32];
             uint64_t pick = written + (n_batches * 2654435761ull) % count;
@@ -404,26 +506,30 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
                 pick = written + (n_batches * 7) % count;
             }
             reference_label32(commitment, pick, (uint32_t)m->opts.scrypt_n, ref);
-            if (memcmp(ref, buf.data() + (pick - written) * 16, 16)) {
+            if (memcmp(ref, labels + (pick - written) * 16, 16)) {
                 metrics().setup_label_mismatch_total++;
                 set_error("reference label mismatch at index " + std::to_string(pick));
-                return finish(B200POST_SETUP_ERROR, B200POST_ERR_LABEL_MISMATCH);
+                return end(B200POST_SETUP_ERROR, B200POST_ERR_LABEL_MISMATCH);
             }
         }
         n_batches++;
         const std::string path = data_file(m->data_dir, file_idx);
         const int fd = open(path.c_str(), O_WRONLY | O_CREAT, 0644);
-        if (fd < 0) return finish(B200POST_SETUP_ERROR, io_error("open " + path));
+        if (fd < 0) return end(B200POST_SETUP_ERROR, io_error("open " + path));
+        const size_t bytes = (size_t)count * 16;
         size_t done = 0;
         bool ok = lseek(fd, (off_t)(in_file * 16), SEEK_SET) >= 0;
-        while (ok && done < buf.size()) {
-            const ssize_t w = write(fd, buf.data() + done, buf.size() - done);
+        while (ok && done < bytes) {
+            const ssize_t w = write(fd, labels + done, bytes - done);
             if (w <= 0) ok = false; else done += (size_t)w;
         }
-        if (!ok || close(fd) != 0) { const int rcio = io_error("write " + path); if (ok) {} else close(fd); return finish(B200POST_SETUP_ERROR, rcio); }
+        if (!ok || close(fd) != 0) { const int rcio = io_error("write " + path); if (ok) {} else close(fd); return end(B200POST_SETUP_ERROR, rcio); }
+        // the scan of this batch overlaps the computation of the next one
+        if (ip && (rc = ip->scan(written, count, labels))) return end(B200POST_SETUP_ERROR, rc);
         written += count;
         m->labels_written.store(written - lo);
-        if ((rc = note_nonce(nn))) return finish(B200POST_SETUP_ERROR, rc);
+        if ((rc = note_nonce(nn))) return end(B200POST_SETUP_ERROR, rc);
+        if (ip && (written % per_file == 0 || written == hi) && (rc = ip->checkpoint())) return end(B200POST_SETUP_ERROR, rc);
     }
     if (!range) {
         int rc;
@@ -439,11 +545,23 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
             // "keep searching past numLabels until a VRF nonce is found" (SURVEY.md §8f.1): outputs are discarded
             rc = search_past_end(m->data_dir, &m->meta, num_labels, m->opts.provider_id, batch, commitment, diff, cancel);
         }
-        if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
-        if (rc) return finish(B200POST_SETUP_ERROR, rc);
+        if (rc == B200POST_ERR_CANCELLED) return end(B200POST_SETUP_STOPPED, rc);
+        if (rc) return end(B200POST_SETUP_ERROR, rc);
     }
-    const int rc = save_metadata(m->data_dir, m->meta);
-    if (rc) return finish(B200POST_SETUP_ERROR, rc);
+    int rc = save_metadata(m->data_dir, m->meta);
+    if (rc) return end(B200POST_SETUP_ERROR, rc);
+    if (ip) {
+        // every label is on disk and the VRF nonce is settled: decide, gate, publish.  No proof is not a failed session.
+        b200post_proof_out proof{};
+        b200post_proof_metadata pm{};
+        rc = ip->finish(&proof, &pm);
+        if (rc == B200POST_OK) rc = save_initial_proof(m->data_dir, pm, m->cfg, m->proof_req.opts.nonces, proof);
+        else if (rc == B200POST_ERR_INVALID_PROOF) unlink(path_join(m->data_dir, kInitialProofFile).c_str());   // a stale one must not answer
+        if (rc != B200POST_OK && rc != B200POST_ERR_INVALID_PROOF) return end(B200POST_SETUP_ERROR, rc);
+        std::lock_guard<std::mutex> lk(m->mu);
+        m->proof_done = true; m->proof_rc = rc; m->proof_err = rc ? last_error() : "";
+        m->proof = proof; m->proof_meta = pm;
+    }
     return finish(B200POST_SETUP_COMPLETE, B200POST_OK);
 }
 
@@ -466,7 +584,8 @@ int b200post_setup_reset(b200post_setup_manager *m) {
         while (struct dirent *e = readdir(d)) {
             const std::string name = e->d_name;
             const bool data = name.rfind("postdata_", 0) == 0 && name.size() > 13 && name.substr(name.size() - 4) == ".bin";
-            if (data || name == kMetaFile) {
+            const bool initial = name.rfind(kInitialProofFile, 0) == 0 || name.rfind(kInitialScanFile, 0) == 0;   // and their .tmp
+            if (data || name == kMetaFile || initial) {
                 if (unlink(path_join(m->data_dir, name).c_str()) != 0) { closedir(d); return io_error("unlink " + name); }
             }
         }
@@ -474,6 +593,7 @@ int b200post_setup_reset(b200post_setup_manager *m) {
     }
     m->labels_written.store(0);
     memset(&m->meta, 0, sizeof m->meta);
+    m->want_proof = m->proof_done = false;
     m->state = B200POST_SETUP_NOT_STARTED;
     return B200POST_OK;
 }
@@ -489,6 +609,45 @@ int b200post_setup_commitment_atx(b200post_setup_manager *m, uint8_t out[32]) {
 int b200post_load_metadata(const char *data_dir, b200post_post_metadata *out) {
     if (!data_dir || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     return load_metadata(data_dir, out, nullptr);
+}
+
+int b200post_setup_request_initial_proof(b200post_setup_manager *m, const b200post_prove_opts *opts) {
+    if (!m || !opts) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->state != B200POST_SETUP_PREPARED) { set_error("post session not prepared"); return B200POST_ERR_STATE; }
+    if (m->range()) { set_error("initial proof: a file-range session does not see the whole POST"); return B200POST_ERR_STATE; }
+    b200post_prove_opts o = *opts;
+    if (o.nonces == 0) o.nonces = 16;
+    if (o.nonces % 16 || o.nonces > 4096) { set_error("invalid nonce count (a positive multiple of 16, <= 4096)"); return B200POST_ERR_INVALID_ARGUMENT; }
+    const int rc = check_pow_mode(o);
+    if (rc) return rc;
+    m->proof_req.cache_key.assign(o.pow_cache_key, o.pow_cache_key ? o.pow_cache_key + o.pow_cache_key_len : o.pow_cache_key);
+    o.pow_cache_key = nullptr; o.pow_cache_key_len = 0;   // the copy above is the key
+    m->proof_req.opts = o;
+    m->want_proof = true;
+    return B200POST_OK;
+}
+
+int b200post_setup_initial_proof(b200post_setup_manager *m, b200post_proof_out *out, b200post_proof_metadata *meta) {
+    if (!m || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->state != B200POST_SETUP_COMPLETE || !m->proof_done) {
+        set_error("no initial proof: the session did not ask for one or has not completed");
+        return B200POST_ERR_STATE;
+    }
+    if (m->proof_rc) { set_error(m->proof_err); return m->proof_rc; }
+    *out = m->proof;
+    if (meta) *meta = m->proof_meta;
+    return B200POST_OK;
+}
+
+int b200post_load_initial_proof(const char *data_dir, const b200post_post_config *cfg, uint32_t nonces, b200post_proof_out *out,
+                                b200post_proof_metadata *meta) {
+    if (!data_dir || !cfg || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    b200post_post_metadata md;
+    const int rc = load_metadata(data_dir, &md, nullptr);
+    if (rc) return rc;
+    return load_initial_proof(data_dir, md, *cfg, nonces ? nonces : 16, out, meta);
 }
 
 }  // extern "C"

@@ -481,6 +481,46 @@ func GenerateProofChecked(ctx context.Context, providers []uint32, dataDir strin
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// The initial proof (BuildInitialPost's PostClient.Proof(ctx, nodeID, shared.ZeroChallenge, nil), activation/activation.go:350-403)
+// ---------------------------------------------------------------------------------------------------------
+
+// RequestInitialProof asks the prepared session (the whole POST, not a file range) for the initial proof: the proof
+// for the zero challenge, computed from the labels as StartSession writes them and stored in initial_post.json in the
+// data dir.  The k2pow runs on the session's devices (builtin RandomX search) before the first label batch.  Call it
+// between PrepareInitializer and StartSession; K1, K2 and the pow difficulty are the manager's SetupConfig.
+func (m *SetupManager) RequestInitialProof(nonces uint32) error {
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), pow_mode: C.B200POST_POW_BUILTIN}
+	return setupErr(checked(func() C.int { return C.b200post_setup_request_initial_proof(m.h, &o) }))
+}
+
+// InitialProof returns the initial proof of the completed session.  ErrInvalidProof-class errors (the status text
+// gives the reason) mean no nonce reached K2 or the verifier refused the proof: the post-service then proves from the
+// stored data.
+func (m *SetupManager) InitialProof() (*Proof, error) {
+	var out C.b200post_proof_out
+	if err := setupErr(checked(func() C.int { return C.b200post_setup_initial_proof(m.h, &out, nil) })); err != nil {
+		return nil, err
+	}
+	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
+}
+
+// LoadInitialProof is the post-service's answer to the ZeroChallenge without a scan: the proof a setup session stored
+// in dataDir, if it was made for this POST's metadata, cfg and nonce count.  An absent or stale proof is an error
+// ("no initial proof"); fall back to GenerateProofChecked.
+func LoadInitialProof(dataDir string, cfg SetupConfig, nonces uint32) (*Proof, error) {
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	var out C.b200post_proof_out
+	if err := setupErr(checked(func() C.int { return C.b200post_load_initial_proof(dir, &c, C.uint32_t(nonces), &out, nil) })); err != nil {
+		return nil, err
+	}
+	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // Checking stored POST data (postcli -verify; verifying.VerifyPos, recalled, unpinned)
 // ---------------------------------------------------------------------------------------------------------
 

@@ -120,6 +120,9 @@ def _bind():
     L.b200post_setup_prepare_files.argtypes = [vp, ctypes.POINTER(_SetupOpts), ctypes.c_char_p, ctypes.c_char_p, ctypes.c_uint64,
                                                ctypes.c_int64]
     L.b200post_search_vrf_nonce.argtypes = [ctypes.c_char_p, ctypes.POINTER(_VrfSearchOpts), ctypes.POINTER(VrfNonce), vp]
+    L.b200post_setup_request_initial_proof.argtypes = [vp, vp]
+    L.b200post_setup_initial_proof.argtypes = [vp, vp, vp]
+    L.b200post_load_initial_proof.argtypes = [ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.c_uint32, vp, vp]
     L._setup_bound = True
     return L
 
@@ -167,6 +170,19 @@ def verify_pos(data_dir: str, *, fraction: float = 0.2, provider_id: int = 0, fr
                            bool(r.argmin_ok), [int(r.bad_index[i]) for i in range(r.n_reported)])
 
 
+def load_initial_proof(data_dir: str, cfg: PostConfig, nonces: int = 16):
+    """The post-service side of the initial proof: the proof a setup session stored in data_dir/initial_post.json, if
+    it answers the zero challenge for this POST, cfg (K1, K2, pow difficulty) and nonce count.  Returns
+    (Proof, ProofMetadata, labels scanned) as prove.generate_proof does; raises B200PostError ERR_IO ("no initial proof")
+    when it is absent or stale, and the caller then proves from the stored data."""
+    from . import prove
+    from .verify import _Meta
+    out, meta = prove._ProofOut(), _Meta()
+    _err(_bind().b200post_load_initial_proof(data_dir.encode(), ctypes.byref(prove._c_cfg(cfg)), nonces, ctypes.byref(out),
+                                             ctypes.byref(meta)))
+    return prove._results(out, meta)
+
+
 def verify_pos_sample(seed: int, file: int, labels_in_file: int, fraction: float):
     """The positions (within the file, ascending, numpy uint64) that verify_pos checks for this seed and file."""
     import numpy as np
@@ -192,7 +208,10 @@ class PostSetupManager:
         L.b200post_default_post_config(ctypes.byref(c))
         c.min_num_units, c.max_num_units, c.labels_per_unit = cfg.min_num_units, cfg.max_num_units, cfg.labels_per_unit
         c.k1, c.k2, c.k3 = cfg.k1, cfg.k2, cfg.k3
+        if cfg.pow_difficulty is not None:   # the initial proof's k2pow difficulty
+            ctypes.memmove(c.pow_difficulty, cfg.pow_difficulty, 32)
         self.cfg = cfg
+        self._initial_opts = None
         self._h = ctypes.c_void_p()
         _err(L.b200post_setup_manager_new(ctypes.byref(c), ctypes.byref(self._h)))
 
@@ -207,6 +226,26 @@ class PostSetupManager:
     def start_session(self, cancel: ctypes.c_int | None = None) -> None:
         """Blocking.  `cancel` = a ctypes.c_int another thread sets to 1 (ctx cancel); raises code ERR_CANCELLED."""
         _err(_bind().b200post_setup_start_session(self._h, ctypes.addressof(cancel) if cancel is not None else None))
+
+    def request_initial_proof(self, *, nonces: int = 16, pow="builtin", pow_cache_key: bytes | None = None) -> None:
+        """Ask the prepared (whole-POST) session for the initial proof: the proof for the zero challenge, computed from
+        the labels as start_session writes them and stored in initial_post.json.  pow as in prove.generate_proof:
+        "builtin", "skip" or a callable.  Call between prepare_initializer and start_session."""
+        from . import prove
+        opts, _ = prove._opts(None, None, nonces, 0, pow)
+        if pow_cache_key is not None:
+            opts.pow_cache_key, opts.pow_cache_key_len = pow_cache_key, len(pow_cache_key)
+        self._initial_opts = opts   # keeps a pow callback alive for the session
+        _err(_bind().b200post_setup_request_initial_proof(self._h, ctypes.byref(opts)))
+
+    def initial_proof(self):
+        """After a completed session that asked for it: (Proof, ProofMetadata, labels scanned).  Raises ERR_INVALID_PROOF
+        with the reason when no nonce reached K2 or the verifier refused the proof, ERR_STATE before completion."""
+        from . import prove
+        from .verify import _Meta
+        out, meta = prove._ProofOut(), _Meta()
+        _err(_bind().b200post_setup_initial_proof(self._h, ctypes.byref(out), ctypes.byref(meta)))
+        return prove._results(out, meta)
 
     def status(self) -> PostSetupStatus:
         s = _Status()

@@ -118,6 +118,42 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
                                     b200post_proof_out *out, b200post_proof_metadata *meta_out, b200post_prove_check *check,
                                     const volatile int *cancel);
 
+/*
+ * The initial proof of a POST, produced by its setup session (DESIGN.md §3e).  go-spacemesh asks for it right after
+ * initialisation (BuildInitialPost: PostClient.Proof(ctx, nodeID, shared.ZeroChallenge, nil)); a proof over 32 zero bytes
+ * computed from the labels as the session writes them spares that second read of every stored label.
+ *
+ * b200post_setup_request_initial_proof: between prepare and start of a session over the whole POST (a file-range session:
+ * B200POST_ERR_STATE; not prepared: B200POST_ERR_STATE); prepare clears the request, a second call replaces it.  From
+ * opts: nonces (0 = 16; else a positive multiple of 16, <= 4096, or INVALID_ARGUMENT), pow_mode with pow_prove/pow_ctx
+ * (CALLBACK without a function: UNSUPPORTED) and the RandomX cache key (copied); provider and chunk_labels are ignored.
+ * K1, K2 and the pow difficulty are the manager's b200post_post_config.
+ * The session then (1) finds one pow per nonce group for the zero challenge before its first label batch (BUILTIN on the
+ * session's devices, then their RandomX memory is released so that the label layer keeps its size), (2) runs the
+ * proving scan (K6a/K6b on the first device of the session) over each batch of [0, numLabels) as it is written, with no
+ * stop rule, keeping each nonce's first K2 hits, and (3) once every label is on disk and the VRF nonce is settled, picks
+ * the winner with the prover's rule, passes the proof through b200post_verify_batch (k2pow checked under BUILTIN only) and
+ * writes it to initial_post.json in the data dir (tmp + rename).  (nonce, indices, pow) are byte-identical to
+ * b200post_generate_proof's over the written files with the same config, nonces and pows; labels_scanned = numLabels.
+ * Stop and resume: initial_post.scan (the pows, the end of the scanned prefix and the hit lists, checksummed) is saved at
+ * every completed postdata file and whenever the session stops or fails.  On start, a state that is missing, damaged,
+ * made for other inputs or ahead of the data on disk is ignored; whatever is on disk past the state is rescanned from
+ * the files before the session continues.  b200post_setup_reset deletes both files.
+ * No nonce with K2 hits, or a proof the gate refuses: the session still completes (its job is the labels), no proof
+ * file is written and b200post_setup_initial_proof returns B200POST_ERR_INVALID_PROOF with the reason.  Without a GPU,
+ * start_session returns B200POST_ERR_NO_DEVICE (no CPU path) and writes no state.
+ */
+int b200post_setup_request_initial_proof(b200post_setup_manager *mgr, const b200post_prove_opts *opts);
+/* After the session is COMPLETE: its initial proof and ProofMetadata (meta may be NULL), or INVALID_PROOF with the reason.
+ * Before that, or when the session did not ask for one: B200POST_ERR_STATE. */
+int b200post_setup_initial_proof(b200post_setup_manager *mgr, b200post_proof_out *out, b200post_proof_metadata *meta);
+/* The post-service side: the proof in data_dir/initial_post.json, without a scan, if it was made for this POST's
+ * metadata (identity, NumUnits, LabelsPerUnit), cfg (LabelsPerUnit, K1, K2, pow difficulty) and `nonces` (0 = 16), for
+ * the zero challenge.  Absent, unreadable or stale: B200POST_ERR_IO, "no initial proof: ..."; the caller then proves from
+ * the stored data (b200post_generate_proof_checked).  meta may be NULL. */
+int b200post_load_initial_proof(const char *data_dir, const b200post_post_config *cfg, uint32_t nonces, b200post_proof_out *out,
+                                b200post_proof_metadata *meta);
+
 /* The scan alone over labels already in host memory: labels16 = count x 16 bytes holding label indices
  * [first_index, first_index + count).  pows = one u64 per nonce group (nonces/16 of them). */
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count,
