@@ -54,6 +54,7 @@ std::string InitialProofScan::header() const {
     put<uint32_t>(&h, opts_.pow_mode);
     put<uint32_t>(&h, (uint32_t)key_.size());
     h.append(key_.begin(), key_.end());
+    if (windows_ > 1) put<uint32_t>(&h, windows_);   // absent for one window: such states stay valid
     return h;
 }
 
@@ -93,7 +94,7 @@ bool InitialProofScan::load_state(uint64_t written) {
     const std::string body = s.substr(0, s.size() - 8);
     if (fnv1a64(body) != sum) return false;
     size_t p = h.size();
-    std::vector<uint64_t> pows(opts_.nonces / 16);
+    std::vector<uint64_t> pows(nonces() / 16);
     for (uint64_t &v : pows) if (!get(body, &p, &v)) return false;
     uint64_t upto;
     uint32_t n_lists;
@@ -101,7 +102,7 @@ bool InitialProofScan::load_state(uint64_t written) {
     HitLists lists;
     for (uint32_t i = 0; i < n_lists; i++) {
         uint32_t nonce, len;
-        if (!get(body, &p, &nonce) || !get(body, &p, &len) || nonce >= opts_.nonces || len > cfg_.k2) return false;
+        if (!get(body, &p, &nonce) || !get(body, &p, &len) || nonce >= nonces() || len > cfg_.k2) return false;
         std::vector<uint64_t> &l = lists[nonce];
         l.resize(len);
         for (uint64_t &v : l) if (!get(body, &p, &v) || v >= upto) return false;
@@ -115,6 +116,7 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
                             const b200post_post_config &cfg, int64_t provider_id, uint64_t written, uint64_t batch,
                             const volatile int *cancel) {
     dir_ = dir; opts_ = req.opts; key_ = req.cache_key; md_ = md; cfg_ = cfg;
+    windows_ = std::max(opts_.windows_per_pass, 1u);
     opts_.pow_cache_key = key_.empty() ? nullptr : key_.data();
     opts_.pow_cache_key_len = key_.size();
     num_labels_ = (uint64_t)md.num_units * md.labels_per_unit;
@@ -129,14 +131,15 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
     int rc;
     if (!load_state(written)) {
         start_ = 0; restored_.clear();
-        if ((rc = find_pows(opts_, kZeroChallenge, md.node_id, md.num_units, cfg.pow_difficulty, devs.data(), (int)devs.size(), &pows_, cancel)))
+        if ((rc = find_pows(opts_, kZeroChallenge, md.node_id, md.num_units, cfg.pow_difficulty, devs.data(), (int)devs.size(), 0,
+                            nonces() / 16, &pows_, cancel)))
             return rc;
         // the RandomX dataset and batch (~14 GiB per device) would otherwise stay resident and shrink every label layer
         if (opts_.pow_mode == B200POST_POW_BUILTIN) for (uint32_t d : devs) randomx_release((int)d);
         if ((rc = save_state())) return rc;   // a resumed session never searches again
     }
     const uint64_t chunk = std::min<uint64_t>({std::max<uint64_t>(batch, 1), kMaxScanChunk, num_labels_});
-    if ((rc = sc_.init(scan_dev_, kZeroChallenge, opts_.nonces, pows_.data(), cfg.k1, cfg.k2, num_labels_, chunk))) return rc;
+    if ((rc = sc_.init(scan_dev_, kZeroChallenge, nonces(), pows_.data(), cfg.k1, cfg.k2, num_labels_, chunk))) return rc;
     sc_.restore(restored_);
     // the gap between the state's prefix and what is on disk, in index order, from the files
     PostDataReader reader(dir, md.max_file_size / 16);
@@ -216,8 +219,16 @@ int InitialProofScan::finish(b200post_proof_out *out, b200post_proof_metadata *m
     if (start_ + sc_.scanned() != num_labels_) { set_error("initial proof: the scan does not cover every label"); return B200POST_ERR_STATE; }
     uint32_t nonce = 0;
     std::vector<uint64_t> idx;
-    if (!pick_winner(sc_.lists(), cfg_.k2, &nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    if ((rc = write_proof(num_labels_, nonce, idx, pows_.data(), num_labels_, out))) return rc;
+    bool have = false;
+    for (uint32_t w = 0; w < windows_ && !have; w++)   // the lowest window with a winner, as the prover's passes
+        have = pick_winner_in(sc_.lists(), w * opts_.nonces, (w + 1) * opts_.nonces, cfg_.k2, &nonce, &idx);
+    if (!have) {
+        set_error(windows_ == 1 ? std::string(kNoProof)
+                                : std::string(kNoProof) + " in nonce windows 0.." + std::to_string(windows_ - 1) + " (nonces [0, " +
+                                      std::to_string(nonces()) + "))");
+        return B200POST_ERR_INVALID_PROOF;
+    }
+    if ((rc = write_proof(num_labels_, nonce, idx, pows_.data(), 0, num_labels_, out))) return rc;
     memset(meta, 0, sizeof *meta);
     memcpy(meta->node_id, md_.node_id, 32);
     memcpy(meta->commitment_atx_id, md_.commitment_atx_id, 32);

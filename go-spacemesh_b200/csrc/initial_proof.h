@@ -49,9 +49,11 @@ private:
     // the scanner's collect / submit, recording the first failure (after it nothing more is folded)
     int collect(int b);
     int submit(int b, uint64_t first, uint64_t count);
+    uint32_t nonces() const { return opts_.nonces * windows_; }   // every nonce of the session's windows
 
     std::string dir_;
     b200post_prove_opts opts_{};
+    uint32_t windows_ = 1;        // nonce windows scanned (the request's windows_per_pass)
     std::vector<uint8_t> key_;
     b200post_post_metadata md_{};
     b200post_post_config cfg_{};

@@ -151,7 +151,12 @@ int b200post_k2pow_search_multi(const uint32_t *providers, int n_providers, cons
 
 int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params *p, uint32_t n_groups, uint64_t max_nonces_per_group,
                                  uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel) {
-    if (!p || !pows || n_groups == 0 || n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    return b200post_k2pow_search_group_range(provider, p, 0, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
+}
+
+int b200post_k2pow_search_group_range(uint32_t provider, const b200post_k2pow_params *p, uint32_t first_group, uint32_t n_groups,
+                                      uint64_t max_nonces_per_group, uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel) {
+    if (!p || !pows || n_groups == 0 || (uint64_t)first_group + n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     RandomxEngine *e = randomx_engine_for(provider);
     if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
     const std::string key = key_of(p->cache_key, p->cache_key_len);
@@ -159,8 +164,8 @@ int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params 
     e->batch_size(&batch);
     for (uint32_t g = 0; g < n_groups; g++) pows[g] = B200POST_K2POW_NOT_FOUND;
     if (max_nonces_per_group == 0 || max_nonces_per_group > kNonceSpace) max_nonces_per_group = kNonceSpace;
-    std::vector<uint32_t> pending(n_groups);
-    for (uint32_t g = 0; g < n_groups; g++) pending[g] = g;
+    std::vector<uint32_t> pending(n_groups);   // absolute group numbers: they are the k2pow input's group byte
+    for (uint32_t g = 0; g < n_groups; g++) pending[g] = first_group + g;
     std::vector<uint8_t> in, out;
     std::vector<uint64_t> hit;
     uint64_t next = 0, total = 0;      // every pending group has tried nonces [0, next)
@@ -173,7 +178,7 @@ int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params 
         total += pending.size() * per;
         std::vector<uint32_t> still;
         for (size_t gi = 0; gi < pending.size(); gi++)
-            if (hit[gi] == B200POST_K2POW_NOT_FOUND) still.push_back(pending[gi]); else pows[pending[gi]] = hit[gi];
+            if (hit[gi] == B200POST_K2POW_NOT_FOUND) still.push_back(pending[gi]); else pows[pending[gi] - first_group] = hit[gi];
         pending.swap(still);
         next += per;
     }
@@ -184,8 +189,17 @@ int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params 
 int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
                                        uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
                                        uint64_t *hashes_done, const volatile int *cancel) {
-    if (!providers || n_providers <= 0 || !p || !pows || n_groups == 0 || n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    if (n_providers == 1) return b200post_k2pow_search_groups(providers[0], p, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
+    return b200post_k2pow_search_group_range_multi(providers, n_providers, p, 0, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
+}
+
+int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
+                                            uint32_t first_group, uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
+                                            uint64_t *hashes_done, const volatile int *cancel) {
+    if (!providers || n_providers <= 0 || !p || !pows || n_groups == 0 || (uint64_t)first_group + n_groups > 256) {
+        set_error("invalid argument");
+        return B200POST_ERR_INVALID_ARGUMENT;
+    }
+    if (n_providers == 1) return b200post_k2pow_search_group_range(providers[0], p, first_group, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
     std::vector<RandomxEngine *> eng(n_providers);
     for (int i = 0; i < n_providers; i++) {
         eng[i] = randomx_engine_for(providers[i]);
@@ -217,7 +231,7 @@ int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_provider
                 {
                     std::lock_guard<std::mutex> lk(mu);
                     groups.clear();
-                    for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(g);
+                    for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(first_group + g);
                     if (groups.empty() || next >= cap) break;
                     // one device batch: `per` consecutive nonces for each group still searching, as on one device
                     per = std::min<uint64_t>(std::max<uint64_t>(1, batch / groups.size()), cap - next);
@@ -227,7 +241,7 @@ int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_provider
                 if ((rcs[i] = search_window(eng[i], key, p, groups, lo, per, in, out, hit)) != B200POST_OK) break;
                 std::lock_guard<std::mutex> lk(mu);
                 total += groups.size() * per;
-                for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi]] = std::min(best[groups[gi]], hit[gi]);
+                for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi] - first_group] = std::min(best[groups[gi] - first_group], hit[gi]);
             }
             if (rcs[i] != B200POST_OK) { errs[i] = last_error(); stop = true; }
         });

@@ -50,6 +50,7 @@ extern "C" size_t b200post_metrics_text(char *buf, size_t cap) {
     o += "b200post_post_verification_seconds_count " + std::to_string(m.verify_seconds_bucket[10].load()) + "\n";
     line("b200post_prove_labels_scanned_total", "stored labels streamed through the proving scan", "counter", m.prove_labels_scanned_total);
     line("b200post_proofs_generated_total", "proofs generated", "counter", m.proofs_generated_total);
+    line("b200post_prove_passes_total", "reads of the stored POST data by the prover (one per pass of nonce windows)", "counter", m.prove_passes_total);
     line("b200post_prove_labels_rechecked_total", "proving-scan hits recomputed and compared with their stored bytes (checked proofs)", "counter", m.prove_labels_rechecked_total);
     line("b200post_prove_damaged_labels_total", "proving-scan hits whose stored bytes differed from their recomputation (checked proofs)", "counter", m.prove_damaged_labels_total);
     line("b200post_setup_sessions_total", "setup sessions started", "counter", m.setup_sessions_total);

@@ -19,6 +19,7 @@ struct Metrics {
     std::atomic<uint64_t> verify_seconds_bucket[11];
     std::atomic<uint64_t> verify_seconds_sum_us{0};
     std::atomic<uint64_t> prove_labels_scanned_total{0}, proofs_generated_total{0};
+    std::atomic<uint64_t> prove_passes_total{0};   // b200post_generate_proof[_multi|_checked]: one per read of the data
     std::atomic<uint64_t> prove_labels_rechecked_total{0}, prove_damaged_labels_total{0};   // b200post_generate_proof_checked
     std::atomic<uint64_t> setup_sessions_total{0}, setup_label_mismatch_total{0};
     std::atomic<uint64_t> post_data_labels_verified_total{0}, post_data_label_mismatch_total{0};   // b200post_verify_pos

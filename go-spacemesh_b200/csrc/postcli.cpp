@@ -20,8 +20,10 @@
 //
 // The initial proof (the proof for the zero challenge a node asks for right after initialisation) from the labels as
 // the session computes them, so that the node's post-service need not read the whole POST back:
-//   b200postcli <init flags> -initialProof [-nonces 288] [-k1 26] [-k2 37] [-powDifficulty <64 hex digits>]
+//   b200postcli <init flags> -initialProof [-nonces 288] [-nonceWindows 1] [-k1 26] [-k2 37] [-powDifficulty <64 hex digits>]
 // writes initial_post.json into the data dir (k2pow on the session's devices).  Not with -fromFile / -toFile.
+// -nonceWindows W scans the nonces [0, W x nonces) in the same pass: the proof comes from the lowest window of -nonces
+// nonces that has one, as a prover trying W windows would find it.
 // Exit codes: 0 ok, 1 error or damaged data, 2 usage, 130 stopped.
 #include <signal.h>
 
@@ -139,7 +141,7 @@ int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
     bool print_providers = false, verify = false, print_num_files = false, search = false, range = false, initial = false;
-    uint32_t nonces = 288, k1 = 0, k2 = 0;
+    uint32_t nonces = 288, windows = 1, k1 = 0, k2 = 0;
     std::string pow_difficulty;
     double fraction = 0.2;
     uint64_t from_file = 0, seed = 0;
@@ -170,6 +172,7 @@ int main(int argc, char **argv) {
         else if (a == "seed") seed = strtoull(val().c_str(), nullptr, 10);
         else if (a == "initialProof") initial = true;
         else if (a == "nonces") nonces = (uint32_t)strtoul(val().c_str(), nullptr, 10);
+        else if (a == "nonceWindows") windows = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "k1") k1 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "k2") k2 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "powDifficulty") pow_difficulty = val();
@@ -196,6 +199,7 @@ int main(int argc, char **argv) {
     b200post_default_post_config(&cfg);
     if (labels_per_unit) cfg.labels_per_unit = labels_per_unit;
     cfg.min_num_units = 1; cfg.max_num_units = 1u << 20;
+    if (windows == 0) { fprintf(stderr, "-nonceWindows must be at least 1\n"); return 2; }
     if (initial && range) { fprintf(stderr, "-initialProof needs the whole POST: it cannot be combined with -fromFile / -toFile\n"); return 2; }
     if (k1) cfg.k1 = k1;
     if (k2) cfg.k2 = cfg.k3 = k2;
@@ -216,7 +220,7 @@ int main(int argc, char **argv) {
     }
     if (initial) {
         b200post_prove_opts po{};
-        po.nonces = nonces; po.pow_mode = B200POST_POW_BUILTIN;
+        po.nonces = nonces; po.pow_mode = B200POST_POW_BUILTIN; po.windows_per_pass = windows;
         if (int rc = b200post_setup_request_initial_proof(mgr, &po)) {
             fprintf(stderr, "initial proof: %s (%d)\n", b200post_last_error(), rc);
             return rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;

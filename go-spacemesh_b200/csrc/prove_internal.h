@@ -27,14 +27,19 @@ bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vecto
 struct KeptHit { uint64_t index; uint8_t label[16]; bool good; };
 using KeptLists = std::map<uint32_t, std::vector<KeptHit>>;   // nonce -> every kept hit, ascending index
 
+// The same rule over the nonces [lo, hi) of `lists` only: the winner of one nonce window.
+bool pick_winner_in(const HitLists &lists, uint32_t lo, uint32_t hi, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices);
+
 // Streaming scan state: device buffers, keys, per-nonce hit lists.  With keep_stored (the checked proof) the kernels
 // write StoredHit records and every hit is kept with its bytes (kept()); otherwise the first K2 per nonce (lists()).
 // Chunks must be submitted in ascending label order and collected in submission order.
 class Scanner {
 public:
     ~Scanner() { if (dev_ >= 0) { cudaSetDevice(dev_); drain(); } }   // the members free themselves on the scan's device
+    // Scans the nonces [first_nonce, first_nonce + nonces) (first_nonce a multiple of 16, the end <= 4096); pows[g] is
+    // the pow of group first_nonce / 16 + g.  The kernels see pass-relative nonces; the hit lists hold absolute ones.
     int init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
-             uint64_t num_labels, uint64_t chunk, bool keep_stored = false);
+             uint64_t num_labels, uint64_t chunk, bool keep_stored = false, uint32_t first_nonce = 0);
     uint8_t *staging(int b) { return h_labels_[b].get(); }
     // enqueue chunk in staging(b): labels [first, first+count)
     int submit(int b, uint64_t first, uint32_t count);
@@ -66,7 +71,7 @@ private:
 
     DeviceEngine *engine_ = nullptr;
     int dev_ = -1;
-    uint32_t nonces_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0, full_ = 0;
+    uint32_t nonces_ = 0, first_ = 0, k2_ = 0, msb_ = 0, hit_cap_ = 0, grid_ = 0, full_ = 0;
     uint64_t lsb_ = 0, chunk_ = 0, scanned_ = 0;
     bool stored_ = false;
     size_t rec_ = 0;   // bytes per hit record (Hit or StoredHit), set by init
@@ -91,18 +96,18 @@ private:
 
 extern const char *const kNoProof;   // "no proof found: ..."
 
-// The proof record of winner (nonce, idx): packs the indices, takes the nonce group's pow, counts the proof in the
-// metrics with `scanned` labels.
-int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint64_t num_labels,
-                b200post_proof_out *out);
+// The proof record of winner (nonce, idx): packs the indices, takes the nonce group's pow (pows[g] is the pow of group
+// first_nonce / 16 + g), counts the proof in the metrics with `scanned` labels.
+int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint32_t first_nonce,
+                uint64_t num_labels, b200post_proof_out *out);
 
 // pow_mode and its hook: B200POST_ERR_UNSUPPORTED for an unknown mode or CALLBACK without pow_prove
 int check_pow_mode(const b200post_prove_opts &o);
-// The k2pow step of a proof: one pow per nonce group for `challenge` under cfg_difficulty / num_units (BUILTIN on
-// `providers`, CALLBACK through o.pow_prove, SKIP = 0).  pows gets o.nonces / 16 entries.
+// The k2pow step of a proof: one pow per nonce group first_group .. first_group + n_groups - 1 for `challenge` under
+// cfg_difficulty / num_units (BUILTIN on `providers`, CALLBACK through o.pow_prove, SKIP = 0).  pows gets n_groups entries.
 int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const uint8_t node_id[32], uint32_t num_units,
-              const uint8_t cfg_difficulty[32], const uint32_t *providers, int n_providers, std::vector<uint64_t> *pows,
-              const volatile int *cancel);
+              const uint8_t cfg_difficulty[32], const uint32_t *providers, int n_providers, uint32_t first_group, uint32_t n_groups,
+              std::vector<uint64_t> *pows, const volatile int *cancel);
 // The verifier gate: the proof through b200post_verify_batch on `provider` (k2pow checked under BUILTIN only).  A
 // rejection clears *out and returns B200POST_ERR_INVALID_PROOF with the verifier's reason.
 int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o,

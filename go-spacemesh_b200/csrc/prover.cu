@@ -13,6 +13,9 @@
 // the stop rule's tentative winner has its first K2 hits recomputed and compared on the device before the scan may stop
 // on it; damaged hits are dropped (DESIGN.md §5).
 //
+// Nonce windows (b200post_prove_opts.max_windows): generate() runs passes over the data, each scanning windows_per_pass
+// windows of nonces with their own pows, until a window has a proof; the kernels only ever see pass-relative nonces.
+//
 // The scanner, the selection rule, the proof record, the pow step and the verifier gate are declared in prove_internal.h:
 // the setup session's initial proof (initial_proof.cu) runs the same scan over the labels as it writes them.
 #include <algorithm>
@@ -133,24 +136,29 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
 
 }  // namespace
 
-bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
+bool pick_winner_in(const HitLists &lists, uint32_t lo, uint32_t hi, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
     bool have = false;
-    for (const auto &kv : lists) {
-        if (kv.second.size() < k2) continue;
-        if (!have || kv.second[k2 - 1] < (*indices)[k2 - 1]) { *nonce = kv.first; *indices = kv.second; have = true; }
+    for (auto it = lists.lower_bound(lo); it != lists.end() && it->first < hi; ++it) {
+        if (it->second.size() < k2) continue;
+        if (!have || it->second[k2 - 1] < (*indices)[k2 - 1]) { *nonce = it->first; *indices = it->second; have = true; }
     }
     return have;
 }
 
+bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
+    return pick_winner_in(lists, 0, UINT32_MAX, k2, nonce, indices);
+}
+
 int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
-                  uint64_t num_labels, uint64_t chunk, bool keep_stored) {
+                  uint64_t num_labels, uint64_t chunk, bool keep_stored, uint32_t first_nonce) {
     DeviceEngine *e = engine_for(provider);
     if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
-    if (nonces == 0 || nonces % 16 || nonces > 4096 || k1 == 0 || k2 == 0 || num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
+    if (nonces == 0 || nonces % 16 || first_nonce % 16 || (uint64_t)first_nonce + nonces > 4096 || k1 == 0 || k2 == 0 ||
+        num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
         set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
         return B200POST_ERR_INVALID_ARGUMENT;
     }
-    engine_ = e; dev_ = e->device(); nonces_ = nonces; k2_ = k2; chunk_ = chunk;
+    engine_ = e; dev_ = e->device(); nonces_ = nonces; first_ = first_nonce; k2_ = k2; chunk_ = chunk;
     stored_ = keep_stored; rec_ = stored_ ? sizeof(StoredHit) : sizeof(Hit);
     const uint64_t diff = b200post_proving_difficulty(k1, num_labels);
     msb_ = (uint32_t)(diff >> 56); lsb_ = diff & 0x00ffffffffffffffull;
@@ -159,15 +167,17 @@ int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonce
     hit_cap_ = (uint32_t)std::min<double>(std::max<double>(4.0 * expect + 65536.0, 65536.0), 4.0 * 1024 * 1024);
     CUDA_TRY(cudaSetDevice(dev_));
     std::vector<uint8_t> rk((size_t)(nonces / 16) * 176), lazy((size_t)nonces * 176);
+    // keys of the absolute groups and nonces; the kernels index them from 0, so their hit nonces are pass-relative
     for (uint32_t g = 0; g < nonces / 16; g++) {
         uint8_t key[16];
-        cipher_key(challenge, g, pows[g], nullptr, key);
+        cipher_key(challenge, first_nonce / 16 + g, pows[g], nullptr, key);
         const Aes128 a(key);
         memcpy(rk.data() + (size_t)g * 176, a.rk, 176);
     }
     for (uint32_t n = 0; n < nonces; n++) {
         uint8_t key[16];
-        cipher_key(challenge, n / 16, pows[n / 16], &n, key);
+        const uint32_t abs = first_nonce + n;
+        cipher_key(challenge, abs / 16, pows[n / 16], &abs, key);
         const Aes128 a(key);
         memcpy(lazy.data() + (size_t)n * 176, a.rk, 176);
     }
@@ -245,7 +255,7 @@ int Scanner::collect(int b, std::mutex *fold_mu) {
     std::unique_lock<std::mutex> lk;
     if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
     for (const Hit &h : v) {
-        std::vector<uint64_t> &l = lists_[h.nonce];
+        std::vector<uint64_t> &l = lists_[first_ + h.nonce];
         if (l.size() < k2_ && (l.push_back(h.index), l.size() == k2_)) full_++;
     }
     scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
@@ -261,7 +271,7 @@ int Scanner::fold_stored(int b, uint32_t n, std::mutex *fold_mu) {
     for (const StoredHit &h : v) {
         KeptHit k{h.index, {}, false};
         memcpy(k.label, &h.label, 16);
-        kept_[h.nonce].push_back(k);
+        kept_[first_ + h.nonce].push_back(k);
     }
     scanned_ += count_[b];
     return B200POST_OK;
@@ -313,15 +323,27 @@ std::vector<std::pair<uint64_t, uint64_t>> split_shards(uint64_t total, uint64_t
 // of [0, total), where a saturated shard counts as whole.  Once the hits below x give some nonce K2 of them the proof is
 // decided (every hit below x is known, so no nonce whose K2-th hit lies past x can win) and every shard stops.  A shard
 // also stops on its own once it is saturated.  With one shard this is "stop once a nonce has K2 hits".
+// One pass of a windowed proof scans `windows` nonce windows of `window` nonces from nonce `first`; the stop rule then
+// looks at the pass's lowest window only, saturation at every nonce of the pass, and the decision walks the windows in
+// order (DESIGN.md §5).
 class ShardedScan {
 public:
     // fill(shard, first label, count, dst): those labels into the shard's pinned staging
     using Fill = std::function<int(size_t, uint64_t, uint64_t, uint8_t *)>;
 
-    ShardedScan(size_t n, uint32_t nonces, uint32_t k2) : nonces_(nonces), k2_(k2) {
+    ShardedScan(size_t n, uint32_t first, uint32_t window, uint32_t windows, uint32_t k2)
+        : first_(first), window_(window), windows_(windows), k2_(k2) {
         for (size_t s = 0; s < n; s++) shards_.emplace_back(new Shard);
     }
     Shard &shard(size_t s) { return *shards_[s]; }
+
+    // After run() (unchecked): the winner of the lowest window of the pass that has one, over merged()
+    bool winner(uint32_t *nonce, std::vector<uint64_t> *indices) const {
+        const HitLists m = merged();
+        for (uint32_t w = 0; w < windows_; w++)
+            if (pick_winner_in(m, lo(w), lo(w) + window_, k2_, nonce, indices)) return true;
+        return false;
+    }
 
     // runs every shard (the calling thread alone when there is one) and returns the first failing shard's status, in
     // list order, once every thread has joined
@@ -362,16 +384,20 @@ public:
         memcpy(commitment_, commitment, 32);
         N_ = N; cancel_ = cancel;
     }
-    // After run(): recheck rounds over everything kept until the winner's first K2 hits are all good (the winner and its
-    // indices) or no nonce has K2 usable hits (false, *rc OK).  Needs no round when the scan stopped on a decision.
+    // After run(): per window of the pass in order, recheck rounds over everything kept until the window's winner has
+    // its first K2 hits all good (the winner and its indices) or no nonce of it has K2 usable hits (the next window);
+    // false with *rc OK when no window has one.  Needs no round when the scan stopped on a decision.
     bool decide(uint32_t *nonce, std::vector<uint64_t> *indices, int *rc) {
         *rc = B200POST_OK;
-        for (;;) {
-            std::vector<Item> items;
-            const Plan p = plan_winner(&items, nonce, indices);
-            if (p != RECHECK) return p == DECIDED;
-            if ((*rc = round(shards_[0]->sc.engine(), items))) return false;
-        }
+        for (uint32_t w = 0; w < windows_; w++)
+            for (;;) {
+                std::vector<Item> items;
+                const Plan p = plan_winner(w, &items, nonce, indices);
+                if (p == DECIDED) return true;
+                if (p == NONE) break;
+                if ((*rc = round(shards_[0]->sc.engine(), items))) return false;
+            }
+        return false;
     }
     uint64_t rechecked() const { return rechecked_; }
     uint32_t rounds() const { return rounds_; }
@@ -381,16 +407,19 @@ private:
     struct Item { size_t shard; uint32_t nonce; uint64_t index; uint8_t label[16]; };
     enum Plan { NONE, DECIDED, RECHECK };
 
-    // Under mu_ (or with the threads joined).  The stop rule over kept (good and pending) hits below x: NONE if no nonce
-    // has K2 of them; DECIDED with the winner when the winner's first K2 are all good; RECHECK with the pending ones.
-    Plan plan_winner(std::vector<Item> *items, uint32_t *nonce, std::vector<uint64_t> *indices) const {
+    uint32_t lo(uint32_t w) const { return first_ + w * window_; }   // the first nonce of window w of the pass
+
+    // Under mu_ (or with the threads joined).  The stop rule over kept (good and pending) hits below x of the nonces of
+    // window w of the pass: NONE if no such nonce has K2 of them; DECIDED with the winner when the winner's first K2 are
+    // all good; RECHECK with the pending ones.
+    Plan plan_winner(uint32_t w, std::vector<Item> *items, uint32_t *nonce, std::vector<uint64_t> *indices) const {
         struct Ref { size_t shard; const KeptHit *k; };
         std::map<uint32_t, std::vector<Ref>> m;   // per nonce, its first K2 kept hits below x in shard order
         for (size_t s = 0; s < shards_.size(); s++) {
             const Scanner &sc = shards_[s]->sc;
-            for (const auto &kv : sc.kept()) {
-                std::vector<Ref> &l = m[kv.first];
-                for (size_t i = 0; i < kv.second.size() && l.size() < k2_; i++) l.push_back({s, &kv.second[i]});
+            for (auto kv = sc.kept().lower_bound(lo(w)); kv != sc.kept().end() && kv->first < lo(w) + window_; ++kv) {
+                std::vector<Ref> &l = m[kv->first];
+                for (size_t i = 0; i < kv->second.size() && l.size() < k2_; i++) l.push_back({s, &kv->second[i]});
             }
             if (sc.scanned() < shards_[s]->hi - shards_[s]->lo && !sc.saturated()) break;   // x lies in this shard
         }
@@ -466,7 +495,7 @@ private:
                 if (!round_busy_) {
                     uint32_t nonce;
                     std::vector<uint64_t> idx;
-                    const Plan p = plan_winner(&items, &nonce, &idx);
+                    const Plan p = plan_winner(0, &items, &nonce, &idx);   // the pass's lowest window decides the stop
                     if (p == DECIDED) { decided_ = true; return true; }
                     winner_round = round_busy_ = p == RECHECK;
                 }
@@ -509,20 +538,29 @@ private:
         return B200POST_OK;
     }
 
+    // The unchecked stop rule, over the nonces of the pass's lowest window (a saturated shard has every nonce of the
+    // pass at K2, that window's included)
     bool should_stop(size_t s) {
-        if (shards_.size() == 1) return shards_[0]->sc.any_full();
+        if (shards_.size() == 1) {
+            if (windows_ == 1) return shards_[0]->sc.any_full();
+            const HitLists &l = shards_[0]->sc.lists();
+            for (auto kv = l.lower_bound(first_); kv != l.end() && kv->first < first_ + window_; ++kv)
+                if (kv->second.size() >= k2_) return true;
+            return false;
+        }
         std::lock_guard<std::mutex> lk(mu_);
         if (shards_[s]->sc.saturated()) return true;
-        below_x_.assign(nonces_, 0);   // hits below x per nonce
+        below_x_.assign(window_, 0);   // hits below x per nonce of the window
         for (const auto &sh : shards_) {
-            for (const auto &kv : sh->sc.lists())
-                if ((below_x_[kv.first] += kv.second.size()) >= k2_) return true;
+            const HitLists &l = sh->sc.lists();
+            for (auto kv = l.lower_bound(first_); kv != l.end() && kv->first < first_ + window_; ++kv)
+                if ((below_x_[kv->first - first_] += kv->second.size()) >= k2_) return true;
             if (sh->sc.scanned() < sh->hi - sh->lo && !sh->sc.saturated()) break;   // x lies in this shard
         }
         return false;
     }
 
-    uint32_t nonces_, k2_;
+    uint32_t first_, window_, windows_, k2_;
     std::vector<std::unique_ptr<Shard>> shards_;
     std::mutex mu_;                  // guards every shard's hit lists and progress once the threads run
     std::vector<uint64_t> below_x_;
@@ -531,11 +569,11 @@ private:
 
 }  // namespace
 
-int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint64_t num_labels,
-                b200post_proof_out *out) {
+int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &idx, const uint64_t *pows, uint32_t first_nonce,
+                uint64_t num_labels, b200post_proof_out *out) {
     metrics().prove_labels_scanned_total += scanned; metrics().proofs_generated_total++;
     memset(out, 0, sizeof *out);
-    out->nonce = nonce; out->pow = pows[nonce / 16]; out->labels_scanned = scanned;
+    out->nonce = nonce; out->pow = pows[(nonce - first_nonce) / 16]; out->labels_scanned = scanned;
     out->indices_len = b200post_pack_indices(idx.data(), idx.size(), b200post_bits_per_index(num_labels), out->indices, sizeof out->indices);
     if (out->indices_len == 0) { set_error("packed indices exceed the 800-byte wire cap"); return B200POST_ERR_INVALID_ARGUMENT; }
     return B200POST_OK;
@@ -552,15 +590,18 @@ int check_pow_mode(const b200post_prove_opts &o) {
 }
 
 int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const uint8_t node_id[32], uint32_t num_units,
-              const uint8_t cfg_difficulty[32], const uint32_t *providers, int n_providers, std::vector<uint64_t> *pows,
-              const volatile int *cancel) {
-    pows->assign(o.nonces / 16, 0);
+              const uint8_t cfg_difficulty[32], const uint32_t *providers, int n_providers, uint32_t first_group, uint32_t n_groups,
+              std::vector<uint64_t> *pows, const volatile int *cancel) {
+    pows->assign(n_groups, 0);
     if (o.pow_mode == B200POST_POW_SKIP) return B200POST_OK;
     uint8_t scaled[32];
     div256_u32(cfg_difficulty, num_units, scaled);
     if (o.pow_mode == B200POST_POW_CALLBACK) {
-        for (uint32_t g = 0; g < o.nonces / 16; g++)
-            if (o.pow_prove(o.pow_ctx, (uint8_t)g, challenge, scaled, node_id, &(*pows)[g]) != 0) { set_error("k2pow hook failed"); return B200POST_ERR_INVALID_ARGUMENT; }
+        for (uint32_t g = 0; g < n_groups; g++)
+            if (o.pow_prove(o.pow_ctx, (uint8_t)(first_group + g), challenge, scaled, node_id, &(*pows)[g]) != 0) {
+                set_error("k2pow hook failed");
+                return B200POST_ERR_INVALID_ARGUMENT;
+            }
         return B200POST_OK;
     }
     // the k2pow step of NIPostBuilder.Proof (activation/nipost.go:171 -> post-service): RandomX nonce search on the device
@@ -569,7 +610,7 @@ int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const u
     memcpy(kp.challenge8, challenge, 8);
     memcpy(kp.node_id, node_id, 32);
     memcpy(kp.difficulty, scaled, 32);
-    const int rc = b200post_k2pow_search_groups_multi(providers, n_providers, &kp, o.nonces / 16, 0, pows->data(), nullptr, cancel);
+    const int rc = b200post_k2pow_search_group_range_multi(providers, n_providers, &kp, first_group, n_groups, 0, pows->data(), nullptr, cancel);
     if (rc) return rc;
     for (uint64_t v : *pows) if (v == B200POST_K2POW_NOT_FOUND) { set_error("k2pow: nonce space exhausted"); return B200POST_ERR_INVALID_PROOF; }
     return B200POST_OK;
@@ -598,29 +639,22 @@ int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scry
 
 namespace {
 
-int finish(const ShardedScan &scan, uint32_t k2, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out) {
-    uint32_t nonce = 0;
-    std::vector<uint64_t> idx;
-    if (!pick_winner(scan.merged(), k2, &nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    return write_proof(scan.scanned(), nonce, idx, pows, num_labels, out);
-}
-
-// The checked proof's decision step: recheck rounds until the winner over usable hits is known, then the report.
-int finish_checked(ShardedScan &scan, const uint64_t *pows, uint64_t num_labels, b200post_proof_out *out, b200post_prove_check *check) {
-    uint32_t nonce = 0;
-    std::vector<uint64_t> idx;
-    int rc = B200POST_OK;
-    const bool have = scan.decide(&nonce, &idx, &rc);
-    check->labels_rechecked = scan.rechecked(); check->damaged = scan.damaged().size(); check->rounds = scan.rounds();
-    for (uint64_t i : scan.damaged()) {   // ascending
+// The checked proof's decision step for one pass: recheck rounds until the winner over usable hits is known (false: the
+// pass has none), then the report, which adds up over the passes (`damaged`: every distinct damaged index so far).
+bool decide_checked(ShardedScan &scan, uint32_t *nonce, std::vector<uint64_t> *idx, std::set<uint64_t> *damaged,
+                    b200post_prove_check *check, int *rc) {
+    const bool have = scan.decide(nonce, idx, rc);
+    const size_t before = damaged->size();
+    damaged->insert(scan.damaged().begin(), scan.damaged().end());
+    check->labels_rechecked += scan.rechecked(); check->rounds += scan.rounds(); check->damaged = damaged->size();
+    check->n_reported = 0;
+    for (uint64_t i : *damaged) {   // ascending
         if (check->n_reported == 64) break;
         check->damaged_index[check->n_reported++] = i;
     }
-    metrics().prove_labels_rechecked_total += check->labels_rechecked;
-    metrics().prove_damaged_labels_total += check->damaged;
-    if (rc) return rc;
-    if (!have) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    return write_proof(scan.scanned(), nonce, idx, pows, num_labels, out);
+    metrics().prove_labels_rechecked_total += scan.rechecked();
+    metrics().prove_damaged_labels_total += damaged->size() - before;
+    return have;
 }
 
 }  // namespace
@@ -656,7 +690,7 @@ extern "C" {
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count, const uint8_t challenge[32],
                         uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2, uint64_t num_labels, b200post_proof_out *out) {
     if (!labels16 || !challenge || !pows || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    ShardedScan scan(1, nonces, k2);
+    ShardedScan scan(1, 0, nonces, 1, k2);
     Shard &sh = scan.shard(0);
     const uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(count, 1), 1u << 22);
     int rc = sh.sc.init(provider, challenge, nonces, pows, k1, k2, num_labels, chunk);
@@ -667,7 +701,10 @@ int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t fir
         return B200POST_OK;
     }, chunk, first_index, nullptr);
     if (rc) return rc;
-    return finish(scan, k2, pows, num_labels, out);
+    uint32_t nonce = 0;
+    std::vector<uint64_t> idx;
+    if (!scan.winner(&nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
+    return write_proof(scan.scanned(), nonce, idx, pows, 0, num_labels, out);
 }
 
 int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
@@ -714,32 +751,54 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
         set_error("corrupt metadata: Scrypt.N out of range");
         return B200POST_ERR_IO;
     }
-    // k2pow per nonce group (RandomX upstream) through the caller's hook
-    std::vector<uint64_t> pows;
     if ((rc = check_pow_mode(o))) return rc;
-    if ((rc = find_pows(o, challenge, md.node_id, md.num_units, cfg->pow_difficulty, providers, n_providers, &pows, cancel))) return rc;
-    // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
+    // the nonce windows [w*n, (w+1)*n) to try, `per_pass` of them per read of the data (b200post_prove_opts)
+    const uint32_t n = o.nonces, windows = std::min(std::max(o.max_windows, 1u), 4096 / n);
+    const uint32_t per_pass = std::max(o.windows_per_pass, 1u);
     const uint64_t chunk = std::min<uint64_t>(o.chunk_labels, num_labels);
-    ShardedScan scan((size_t)n_providers, o.nonces, cfg->k2);
-    if (check) {
-        uint8_t commitment[32];
-        commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
-        scan.enable_check(commitment, md.scrypt_n, cancel);
-    }
     const auto ranges = split_shards(num_labels, chunk, (size_t)n_providers);
-    for (int s = 0; s < n_providers; s++) {
-        Shard &sh = scan.shard((size_t)s);
-        if ((rc = sh.sc.init(providers[s], challenge, o.nonces, pows.data(), cfg->k1, cfg->k2, num_labels, chunk, check != nullptr))) return rc;
-        sh.lo = ranges[(size_t)s].first; sh.hi = ranges[(size_t)s].second;
-    }
-
+    uint8_t commitment[32];
+    if (check) commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
     const uint64_t per_file = md.max_file_size / 16;
-    if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
-    std::vector<std::unique_ptr<PostDataReader>> readers;
-    for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
-    rc = scan.run([&](size_t s, uint64_t pos, uint64_t n, uint8_t *dst) { return readers[s]->read(pos, n, dst); }, chunk, 0, cancel);
-    if (rc) return rc;
-    if ((rc = check ? finish_checked(scan, pows.data(), num_labels, out, check) : finish(scan, cfg->k2, pows.data(), num_labels, out))) return rc;
+    uint64_t scanned = 0;              // over every pass
+    std::set<uint64_t> damaged;        // the checked report's, over every pass
+    bool have = false;
+    for (uint32_t a = 0; a < windows && !have;) {
+        const uint32_t m = std::min(per_pass, windows - a), first = a * n;
+        // k2pow per nonce group of the pass (RandomX upstream; or the caller's hook)
+        std::vector<uint64_t> pows;
+        if ((rc = find_pows(o, challenge, md.node_id, md.num_units, cfg->pow_difficulty, providers, n_providers, first / 16, m * n / 16,
+                            &pows, cancel)))
+            return rc;
+        // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
+        ShardedScan scan((size_t)n_providers, first, n, m, cfg->k2);
+        if (check) scan.enable_check(commitment, md.scrypt_n, cancel);
+        for (int s = 0; s < n_providers; s++) {
+            Shard &sh = scan.shard((size_t)s);
+            if ((rc = sh.sc.init(providers[s], challenge, m * n, pows.data(), cfg->k1, cfg->k2, num_labels, chunk, check != nullptr, first)))
+                return rc;
+            sh.lo = ranges[(size_t)s].first; sh.hi = ranges[(size_t)s].second;
+        }
+        if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
+        std::vector<std::unique_ptr<PostDataReader>> readers;
+        for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
+        rc = scan.run([&](size_t s, uint64_t pos, uint64_t cnt, uint8_t *dst) { return readers[s]->read(pos, cnt, dst); }, chunk, 0, cancel);
+        if (rc) return rc;
+        metrics().prove_passes_total++;
+        scanned += scan.scanned();
+        uint32_t nonce = 0;
+        std::vector<uint64_t> idx;
+        have = check ? decide_checked(scan, &nonce, &idx, &damaged, check, &rc) : scan.winner(&nonce, &idx);
+        if (rc) return rc;
+        if (have && (rc = write_proof(scanned, nonce, idx, pows.data(), first, num_labels, out))) return rc;
+        a += m;
+    }
+    if (!have) {
+        set_error(windows == 1 ? std::string(kNoProof)
+                               : std::string(kNoProof) + " in nonce windows 0.." + std::to_string(windows - 1) + " (nonces [0, " +
+                                     std::to_string((uint64_t)windows * n) + "))");
+        return B200POST_ERR_INVALID_PROOF;
+    }
     b200post_proof_metadata meta;
     memcpy(meta.node_id, md.node_id, 32);
     memcpy(meta.commitment_atx_id, md.commitment_atx_id, 32);

@@ -174,9 +174,10 @@ int load_metadata(const std::string &dir, b200post_post_metadata *m, bool *missi
 
 const uint8_t kZeroChallenge[32] = {0};
 
-// initial_post.json: the proof, with the fields that decide whether it still answers the ZeroChallenge
+// initial_post.json: the proof, with the fields that decide whether it still answers the ZeroChallenge.  "Windows" (the
+// nonce windows the session scanned) is written only above 1, so a one-window file is what it was before windows.
 int save_initial_proof(const std::string &dir, const b200post_proof_metadata &pm, const b200post_post_config &cfg, uint32_t nonces,
-                       const b200post_proof_out &p) {
+                       uint32_t windows, const b200post_proof_out &p) {
     std::string j = "{\n";
     j += " \"NodeId\": \"" + b64(pm.node_id, 32) + "\",\n";
     j += " \"CommitmentAtxId\": \"" + b64(pm.commitment_atx_id, 32) + "\",\n";
@@ -185,6 +186,7 @@ int save_initial_proof(const std::string &dir, const b200post_proof_metadata &pm
     j += " \"K1\": " + std::to_string(cfg.k1) + ",\n";
     j += " \"K2\": " + std::to_string(cfg.k2) + ",\n";
     j += " \"Nonces\": " + std::to_string(nonces) + ",\n";
+    if (windows > 1) j += " \"Windows\": " + std::to_string(windows) + ",\n";
     j += " \"PowDifficulty\": \"" + hex(cfg.pow_difficulty, 32) + "\",\n";
     j += " \"Challenge\": \"" + b64(pm.challenge, 32) + "\",\n";
     j += " \"Nonce\": " + std::to_string(p.nonce) + ",\n";
@@ -232,7 +234,11 @@ int load_initial_proof(const std::string &dir, const b200post_post_metadata &md,
     if (units != md.num_units || lpu != md.labels_per_unit || lpu != cfg.labels_per_unit) return no_initial_proof("it was made for another POST size");
     if (k1 != cfg.k1 || k2 != cfg.k2 || memcmp(diff, cfg.pow_difficulty, 32)) return no_initial_proof("it was made under another K1, K2 or pow difficulty");
     if (nn != nonces) return no_initial_proof("it was made for another nonce count");
-    if (memcmp(m.challenge, kZeroChallenge, 32) || nonce >= nonces) return no_initial_proof("it does not answer the zero challenge");
+    // a session that scanned several nonce windows may have proved with a nonce of any of them
+    uint64_t windows = 1;
+    if (doc.find("\"Windows\"") != std::string::npos && (!json_u64(doc, "Windows", &windows) || windows < 2 || windows > 4096 / nonces))
+        return no_initial_proof(std::string(kInitialProofFile) + " is unreadable");
+    if (memcmp(m.challenge, kZeroChallenge, 32) || nonce >= nonces * windows) return no_initial_proof("it does not answer the zero challenge");
     m.num_units = md.num_units; m.labels_per_unit = md.labels_per_unit;
     p.nonce = (uint32_t)nonce; p.pow = pow; p.indices_len = packed; p.labels_scanned = num_labels;
     *out = p;
@@ -555,7 +561,7 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         b200post_proof_out proof{};
         b200post_proof_metadata pm{};
         rc = ip->finish(&proof, &pm);
-        if (rc == B200POST_OK) rc = save_initial_proof(m->data_dir, pm, m->cfg, m->proof_req.opts.nonces, proof);
+        if (rc == B200POST_OK) rc = save_initial_proof(m->data_dir, pm, m->cfg, m->proof_req.opts.nonces, m->proof_req.opts.windows_per_pass, proof);
         else if (rc == B200POST_ERR_INVALID_PROOF) unlink(path_join(m->data_dir, kInitialProofFile).c_str());   // a stale one must not answer
         if (rc != B200POST_OK && rc != B200POST_ERR_INVALID_PROOF) return end(B200POST_SETUP_ERROR, rc);
         std::lock_guard<std::mutex> lk(m->mu);
@@ -619,6 +625,9 @@ int b200post_setup_request_initial_proof(b200post_setup_manager *m, const b200po
     b200post_prove_opts o = *opts;
     if (o.nonces == 0) o.nonces = 16;
     if (o.nonces % 16 || o.nonces > 4096) { set_error("invalid nonce count (a positive multiple of 16, <= 4096)"); return B200POST_ERR_INVALID_ARGUMENT; }
+    // the session's one pass scans windows_per_pass nonce windows (0 = 1, clamped to the group limit); max_windows is unused
+    o.windows_per_pass = std::min(std::max(o.windows_per_pass, 1u), 4096 / o.nonces);
+    o.max_windows = 0;
     const int rc = check_pow_mode(o);
     if (rc) return rc;
     m->proof_req.cache_key.assign(o.pow_cache_key, o.pow_cache_key ? o.pow_cache_key + o.pow_cache_key_len : o.pow_cache_key);

@@ -452,6 +452,24 @@ type ProveCheck struct {
 // before it is returned.  On clean data the proof equals GenerateProofOn's.  Damage is not an error: a non-empty
 // report means the data needs `b200postcli -verify -fraction 100` and the damaged file a repair.
 func GenerateProofChecked(ctx context.Context, providers []uint32, dataDir string, challenge []byte, cfg SetupConfig, nonces uint32) (*Proof, *ProveCheck, error) {
+	return GenerateProofCheckedWindows(ctx, providers, dataDir, challenge, cfg, nonces, NonceWindows{})
+}
+
+// AllWindows as NonceWindows.Max tries every nonce window below nonce 4096: libpost's loop.
+const AllWindows = ^uint32(0)
+
+// NonceWindows says which nonce windows a proof may come from (b200post_prove_opts.max_windows / windows_per_pass).
+// Window w is the nonces [w*nonces, (w+1)*nonces); the proof comes from the lowest window that has one.  Max: the
+// windows to try (0 or 1 = the first only, AllWindows = up to nonce 4096); PerPass: the windows scanned per read of the
+// data (0 or 1 = one).  The proof does not depend on PerPass.
+type NonceWindows struct {
+	Max, PerPass uint32
+}
+
+// GenerateProofCheckedWindows is GenerateProofChecked over the nonce windows w; NonceWindows{} is GenerateProofChecked.
+// A post-service replacement passes NonceWindows{Max: AllWindows}, which is libpost's behaviour.
+func GenerateProofCheckedWindows(ctx context.Context, providers []uint32, dataDir string, challenge []byte, cfg SetupConfig, nonces uint32,
+	w NonceWindows) (*Proof, *ProveCheck, error) {
 	if len(providers) == 0 {
 		return nil, nil, ErrNoProvider
 	}
@@ -460,7 +478,7 @@ func GenerateProofChecked(ctx context.Context, providers []uint32, dataDir strin
 	var c C.b200post_post_config
 	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
 	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
-	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces)}
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), max_windows: C.uint32_t(w.Max), windows_per_pass: C.uint32_t(w.PerPass)}
 	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
 	defer C.free(unsafe.Pointer(provs))
 	flag, stop := cancelFlag(ctx)
@@ -489,7 +507,14 @@ func GenerateProofChecked(ctx context.Context, providers []uint32, dataDir strin
 // data dir.  The k2pow runs on the session's devices (builtin RandomX search) before the first label batch.  Call it
 // between PrepareInitializer and StartSession; K1, K2 and the pow difficulty are the manager's SetupConfig.
 func (m *SetupManager) RequestInitialProof(nonces uint32) error {
-	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), pow_mode: C.B200POST_POW_BUILTIN}
+	return m.RequestInitialProofWindows(nonces, NonceWindows{})
+}
+
+// RequestInitialProofWindows is RequestInitialProof scanning w.PerPass nonce windows in the session's one pass (w.Max is
+// unused): the proof is GenerateProofCheckedWindows's with NonceWindows{Max: w.PerPass} over the written data, and
+// LoadInitialProof accepts it with the same nonce count.
+func (m *SetupManager) RequestInitialProofWindows(nonces uint32, w NonceWindows) error {
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), pow_mode: C.B200POST_POW_BUILTIN, windows_per_pass: C.uint32_t(w.PerPass)}
 	return setupErr(checked(func() C.int { return C.b200post_setup_request_initial_proof(m.h, &o) }))
 }
 

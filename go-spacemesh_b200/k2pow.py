@@ -37,6 +37,9 @@ def _bind():
         L.b200post_k2pow_search_groups.argtypes = [u32, ctypes.POINTER(_Params), u32, u64, vp, ctypes.POINTER(u64), vp]
         L.b200post_k2pow_search_groups_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u32, u64, vp,
                                                          ctypes.POINTER(u64), vp]
+        L.b200post_k2pow_search_group_range.argtypes = [u32, ctypes.POINTER(_Params), u32, u32, u64, vp, ctypes.POINTER(u64), vp]
+        L.b200post_k2pow_search_group_range_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u32, u32,
+                                                              u64, vp, ctypes.POINTER(u64), vp]
         L.b200post_k2pow_verify.argtypes = [u32, ctypes.POINTER(_Params), u64, ctypes.POINTER(ctypes.c_int)]
         L.b200post_randomx_dataset_read.argtypes = [u32, ctypes.c_char_p, sz, u64, u64, vp]
         L.b200post_randomx_last_timing.argtypes = [u32, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
@@ -120,6 +123,26 @@ def search_groups(challenge8: bytes, node_id: bytes, difficulty: bytes, n_groups
                                                     pows.ctypes.data, ctypes.byref(done), cptr))
     pows = pows[:n_groups]
     return [None if int(v) == NOT_FOUND else int(v) for v in pows], done.value
+
+
+def search_group_range(challenge8: bytes, node_id: bytes, difficulty: bytes, first_group: int, n_groups: int,
+                       max_nonces_per_group: int = 0, *, key: bytes | None = None, provider: int = 0,
+                       providers: list[int] | None = None, cancel=None):
+    """search_groups for the groups first_group .. first_group + n_groups - 1 (first_group + n_groups <= 256): the pows
+    of a pass of nonce windows.  -> (pows, hashes computed), pows[i] being group first_group + i's."""
+    p = _params(0, challenge8, node_id, difficulty, key)
+    pows = np.zeros(max(n_groups, 1), dtype=np.uint64)
+    done = ctypes.c_uint64(0)
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    if providers is not None:
+        arr = (ctypes.c_uint32 * len(providers))(*providers)
+        _check(_bind().b200post_k2pow_search_group_range_multi(arr if len(providers) else None, len(providers), ctypes.byref(p),
+                                                               first_group, n_groups, max_nonces_per_group, pows.ctypes.data,
+                                                               ctypes.byref(done), cptr))
+    else:
+        _check(_bind().b200post_k2pow_search_group_range(provider, ctypes.byref(p), first_group, n_groups, max_nonces_per_group,
+                                                         pows.ctypes.data, ctypes.byref(done), cptr))
+    return [None if int(v) == NOT_FOUND else int(v) for v in pows[:n_groups]], done.value
 
 
 def dataset(first: int, count: int, key: bytes | None = None, *, provider: int = 0) -> np.ndarray:

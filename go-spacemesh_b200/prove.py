@@ -19,10 +19,14 @@ POW_PROVE_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_uint8, c
                                 ctypes.POINTER(ctypes.c_uint8), ctypes.POINTER(ctypes.c_uint8), ctypes.POINTER(ctypes.c_uint64))
 
 
+ALL_WINDOWS = 2**32 - 1   # B200POST_PROVE_ALL_WINDOWS: every nonce window below nonce 4096
+
+
 class _ProveOpts(ctypes.Structure):
     _fields_ = [("provider", ctypes.c_uint32), ("nonces", ctypes.c_uint32), ("chunk_labels", ctypes.c_uint64),
                 ("pow_prove", POW_PROVE_FN), ("pow_ctx", ctypes.c_void_p), ("pow_mode", ctypes.c_uint32),
-                ("pow_cache_key", ctypes.c_char_p), ("pow_cache_key_len", ctypes.c_size_t)]
+                ("pow_cache_key", ctypes.c_char_p), ("pow_cache_key_len", ctypes.c_size_t),
+                ("max_windows", ctypes.c_uint32), ("windows_per_pass", ctypes.c_uint32)]
 
 
 class _ProofOut(ctypes.Structure):
@@ -80,7 +84,7 @@ def _err(rc):
         raise B200PostError(rc, lib().b200post_last_error().decode(errors="replace"))
 
 
-def _opts(provider, providers, nonces, chunk_labels, pow):
+def _opts(provider, providers, nonces, chunk_labels, pow, max_windows=1, windows_per_pass=1):
     if provider is not None and providers is not None:
         raise ValueError("give `provider` or `providers`, not both")
     if isinstance(providers, str):
@@ -93,7 +97,11 @@ def _opts(provider, providers, nonces, chunk_labels, pow):
         cb, mode = POW_PROVE_FN(pow), 1
     else:
         cb, mode = ctypes.cast(None, POW_PROVE_FN), {"builtin": 0, "skip": 2, "callback-missing": 1}[pow]
-    return _ProveOpts(provider or 0, nonces, chunk_labels, cb, None, mode, None, 0), providers
+    if isinstance(max_windows, str):
+        if max_windows != "all":
+            raise ValueError(f"max_windows must be a count or 'all', not {max_windows!r}")
+        max_windows = ALL_WINDOWS
+    return _ProveOpts(provider or 0, nonces, chunk_labels, cb, None, mode, None, 0, max_windows, windows_per_pass), providers
 
 
 def _results(out, meta):
@@ -104,14 +112,16 @@ def _results(out, meta):
 
 
 def generate_proof_checked(data_dir: str, challenge: bytes, cfg: PostConfig, *, providers=(0,), nonces: int = 16,
-                           chunk_labels: int = 0, pow="builtin", cancel=None):
+                           chunk_labels: int = 0, pow="builtin", cancel=None, max_windows=1, windows_per_pass: int = 1):
     """generate_proof over stored data that may be damaged (b200post_generate_proof_checked): a stored label is a hit
     only when it also equals its recomputed label, so a damaged label never enters the proof, and the proof passes the
     library's verifier before it is returned.  On undamaged data the proof equals generate_proof's.
     Returns (Proof, ProofMetadata, labels scanned, ProveCheck).  A non-empty report is damage in the stored POST data:
-    run `b200postcli -verify -fraction 100` to find all of it.  providers: a list of device ids or "all"."""
+    run `b200postcli -verify -fraction 100` to find all of it.  providers: a list of device ids or "all".
+    max_windows / windows_per_pass: as for generate_proof; the report covers every pass."""
     L = _bind()
-    opts, providers = _opts(None, list(providers) if not isinstance(providers, str) else providers, nonces, chunk_labels, pow)
+    opts, providers = _opts(None, list(providers) if not isinstance(providers, str) else providers, nonces, chunk_labels, pow,
+                            max_windows, windows_per_pass)
     out, meta, chk, c = _ProofOut(), _Meta(), _ProveCheck(), _c_cfg(cfg)
     cptr = ctypes.addressof(cancel) if cancel is not None else None
     arr = (ctypes.c_uint32 * len(providers))(*providers)
@@ -124,15 +134,18 @@ def generate_proof_checked(data_dir: str, challenge: bytes, cfg: PostConfig, *, 
 
 
 def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int | None = None, nonces: int = 16,
-                   chunk_labels: int = 0, pow="builtin", providers=None, cancel=None):
+                   chunk_labels: int = 0, pow="builtin", providers=None, cancel=None, max_windows=1, windows_per_pass: int = 1):
     """PostClient.Proof(ctx, challenge) -> (Post, PostInfo-like metadata); also returns labels scanned.
     pow: "builtin" (k2pow search on the device, the library default), "skip" (pow = 0, explicit) or a callable
     (ctx, nonce_group, challenge8, difficulty32, node_id32, pow_out) -> 0.
     providers: a list of device ids (repeats allowed) or "all" proves on several devices with the one-device result;
     it replaces `provider` (default 0), and giving both is an error.  cancel: an optional ctypes.c_int, polled per
-    chunk."""
+    chunk.
+    max_windows: how many nonce windows [w*nonces, (w+1)*nonces) to try when the first holds no proof (1, a count, or
+    "all" = every window below nonce 4096, libpost's loop); windows_per_pass: windows scanned per read of the data.
+    The proof is the lowest window's that has one, whatever windows_per_pass; labels scanned adds up over the reads."""
     L = _bind()
-    opts, providers = _opts(provider, providers, nonces, chunk_labels, pow)
+    opts, providers = _opts(provider, providers, nonces, chunk_labels, pow, max_windows, windows_per_pass)
     out, meta, c = _ProofOut(), _Meta(), _c_cfg(cfg)
     cptr = ctypes.addressof(cancel) if cancel is not None else None
     if providers is None:

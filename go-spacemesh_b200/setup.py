@@ -227,12 +227,14 @@ class PostSetupManager:
         """Blocking.  `cancel` = a ctypes.c_int another thread sets to 1 (ctx cancel); raises code ERR_CANCELLED."""
         _err(_bind().b200post_setup_start_session(self._h, ctypes.addressof(cancel) if cancel is not None else None))
 
-    def request_initial_proof(self, *, nonces: int = 16, pow="builtin", pow_cache_key: bytes | None = None) -> None:
+    def request_initial_proof(self, *, nonces: int = 16, pow="builtin", pow_cache_key: bytes | None = None,
+                              windows_per_pass: int = 1) -> None:
         """Ask the prepared (whole-POST) session for the initial proof: the proof for the zero challenge, computed from
         the labels as start_session writes them and stored in initial_post.json.  pow as in prove.generate_proof:
-        "builtin", "skip" or a callable.  Call between prepare_initializer and start_session."""
+        "builtin", "skip" or a callable.  windows_per_pass: the nonce windows the session scans (its proof is
+        prove.generate_proof's with max_windows = that count).  Call between prepare_initializer and start_session."""
         from . import prove
-        opts, _ = prove._opts(None, None, nonces, 0, pow)
+        opts, _ = prove._opts(None, None, nonces, 0, pow, 1, windows_per_pass)
         if pow_cache_key is not None:
             opts.pow_cache_key, opts.pow_cache_key_len = pow_cache_key, len(pow_cache_key)
         self._initial_opts = opts   # keeps a pow callback alive for the session

@@ -94,6 +94,16 @@ int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_provider
                                        uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
                                        uint64_t *hashes_done, const volatile int *cancel);
 
+/* The groups first_group .. first_group + n_groups - 1 (first_group + n_groups <= 256, n_groups >= 1): pows[i] is the
+ * pow of group first_group + i, found as b200post_k2pow_search_groups[_multi] finds it, so the results are those calls'
+ * entries for the same groups.  A windowed proof (b200post_prove_opts.max_windows) searches each pass's groups so.
+ * b200post_k2pow_search_groups[_multi] are the first_group = 0 case. */
+int b200post_k2pow_search_group_range(uint32_t provider, const b200post_k2pow_params *p, uint32_t first_group, uint32_t n_groups,
+                                      uint64_t max_nonces_per_group, uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel);
+int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
+                                            uint32_t first_group, uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
+                                            uint64_t *hashes_done, const volatile int *cancel);
+
 /* The verifier's check: *valid = 1 iff RandomX(input(pow)) < p->difficulty. */
 int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uint64_t pow, int *valid);
 

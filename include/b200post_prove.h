@@ -44,7 +44,26 @@ typedef struct b200post_prove_opts {
                                           (explicit opt-out: such a proof only verifies with the pow check skipped)  */
     const uint8_t *pow_cache_key;      /* BUILTIN: RandomX cache key, NULL = the spacemesh default                 */
     size_t pow_cache_key_len;
+    uint32_t max_windows;              /* nonce windows to try (see "Nonce windows" below): 0 or 1 = [0, nonces)
+                                          only; B200POST_PROVE_ALL_WINDOWS = up to the group limit (libpost's loop);
+                                          any value is clamped to floor(4096 / nonces)                          */
+    uint32_t windows_per_pass;         /* windows scanned per read of the POST: 0 or 1 = one; clamped to the
+                                          windows left                                                            */
 } b200post_prove_opts;
+
+#define B200POST_PROVE_ALL_WINDOWS UINT32_MAX
+
+/* Nonce windows.  With n = nonces, window w is the nonces [w*n, (w+1)*n), nonce groups w*n/16 .. (w+1)*n/16 - 1; only
+ * whole windows below nonce 4096 exist (the group is one byte of the k2pow input), so at most floor(4096 / n).  The
+ * proof comes from the lowest window in which some nonce reaches K2 (usable, for the checked call) hits; inside it the
+ * selection rule above applies and the pow is that nonce group's.
+ * A pass scans windows [a, a + m) in one read of the data (m = windows_per_pass): the pows of all m*n/16 groups first,
+ * then the scan, which stops early only once window a is decided (the usual stop rule restricted to window a's
+ * nonces), or when a shard is saturated for every nonce of the pass; otherwise it reads every label.  The lowest window
+ * of the pass with a winner gives the proof; with none, the next pass starts at window a + m.  So the proof does not
+ * depend on windows_per_pass, the device list or the chunk size: it is the one sequential windows give, and a pass
+ * never reads more labels than they would (it may only find pows for windows that turn out not to be needed).
+ * No window up to max_windows with a proof: B200POST_ERR_INVALID_PROOF, "no proof found: ..." naming the windows. */
 
 typedef struct b200post_proof_out {    /* types.Post / shared.Proof */
     uint32_t nonce;
@@ -52,8 +71,9 @@ typedef struct b200post_proof_out {    /* types.Post / shared.Proof */
     size_t indices_len;
     uint8_t indices[800];              /* wire cap, activation/wire/wire_v1.go:43                               */
     uint64_t labels_scanned;           /* labels streamed from the first index, in whole chunks (not an absolute
-                                          index): last proof index - first index < labels_scanned <= labels
-                                          offered (count, or num_labels for b200post_generate_proof)           */
+                                          index), summed over the passes of a windowed proof (so it may exceed
+                                          num_labels): in the last pass, last proof index - first index <
+                                          its labels <= labels offered (count, or num_labels for the generators) */
 } b200post_proof_out;
 
 /* Proof over the POST data in `data_dir` (postdata_N.bin + postdata_metadata.json written by a setup session).
@@ -126,7 +146,10 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
  * b200post_setup_request_initial_proof: between prepare and start of a session over the whole POST (a file-range session:
  * B200POST_ERR_STATE; not prepared: B200POST_ERR_STATE); prepare clears the request, a second call replaces it.  From
  * opts: nonces (0 = 16; else a positive multiple of 16, <= 4096, or INVALID_ARGUMENT), pow_mode with pow_prove/pow_ctx
- * (CALLBACK without a function: UNSUPPORTED) and the RandomX cache key (copied); provider and chunk_labels are ignored.
+ * (CALLBACK without a function: UNSUPPORTED), the RandomX cache key (copied) and windows_per_pass, the W nonce windows the
+ * session scans in its single pass (0 = 1, clamped to floor(4096 / nonces)); provider, chunk_labels and max_windows are
+ * ignored.  The proof is then b200post_generate_proof's with the same nonces and max_windows = W; initial_post.json gets
+ * a "Windows": W field and initial_post.scan's header ends with W, both only for W > 1 (one-window files are unchanged).
  * K1, K2 and the pow difficulty are the manager's b200post_post_config.
  * The session then (1) finds one pow per nonce group for the zero challenge before its first label batch (BUILTIN on the
  * session's devices, then their RandomX memory is released so that the label layer keeps its size), (2) runs the
@@ -149,8 +172,9 @@ int b200post_setup_request_initial_proof(b200post_setup_manager *mgr, const b200
 int b200post_setup_initial_proof(b200post_setup_manager *mgr, b200post_proof_out *out, b200post_proof_metadata *meta);
 /* The post-service side: the proof in data_dir/initial_post.json, without a scan, if it was made for this POST's
  * metadata (identity, NumUnits, LabelsPerUnit), cfg (LabelsPerUnit, K1, K2, pow difficulty) and `nonces` (0 = 16), for
- * the zero challenge.  Absent, unreadable or stale: B200POST_ERR_IO, "no initial proof: ..."; the caller then proves from
- * the stored data (b200post_generate_proof_checked).  meta may be NULL. */
+ * the zero challenge.  A file with "Windows": W may hold any nonce below nonces x W.  Absent, unreadable or stale:
+ * B200POST_ERR_IO, "no initial proof: ..."; the caller then proves from the stored data (b200post_generate_proof_checked).
+ * meta may be NULL. */
 int b200post_load_initial_proof(const char *data_dir, const b200post_post_config *cfg, uint32_t nonces, b200post_proof_out *out,
                                 b200post_proof_metadata *meta);
 
