@@ -62,12 +62,12 @@ std::string InitialProofScan::header() const {
 int InitialProofScan::save_state() {
     std::string s = header();
     for (uint64_t p : pows_) put<uint64_t>(&s, p);
-    put<uint64_t>(&s, start_ + sc_.scanned());
-    put<uint32_t>(&s, (uint32_t)sc_.lists().size());
-    for (const auto &kv : sc_.lists()) {
+    put<uint64_t>(&s, book().scanned());
+    put<uint32_t>(&s, (uint32_t)book().lists().size());
+    for (const auto &kv : book().lists()) {
         put<uint32_t>(&s, kv.first);
         put<uint32_t>(&s, (uint32_t)kv.second.size());
-        for (uint64_t i : kv.second) put<uint64_t>(&s, i);
+        for (const KeptHit &k : kv.second) put<uint64_t>(&s, k.index);
     }
     put<uint64_t>(&s, fnv1a64(s));
     const std::string fin = join(dir_, kInitialScanFile), tmp = fin + ".tmp";
@@ -99,16 +99,18 @@ bool InitialProofScan::load_state(uint64_t written) {
     uint64_t upto;
     uint32_t n_lists;
     if (!get(body, &p, &upto) || upto > written || upto > num_labels_ || !get(body, &p, &n_lists)) return false;
-    HitLists lists;
+    HitBook restored(nonces(), cfg_.k2, true);
     for (uint32_t i = 0; i < n_lists; i++) {
         uint32_t nonce, len;
         if (!get(body, &p, &nonce) || !get(body, &p, &len) || nonce >= nonces() || len > cfg_.k2) return false;
-        std::vector<uint64_t> &l = lists[nonce];
-        l.resize(len);
-        for (uint64_t &v : l) if (!get(body, &p, &v) || v >= upto) return false;
+        for (uint64_t j = 0, v; j < len; j++) {
+            if (!get(body, &p, &v) || v >= upto) return false;
+            restored.add(nonce, v, nullptr);
+        }
     }
     if (p != body.size()) return false;
-    pows_ = pows; start_ = upto; restored_ = lists;
+    restored.advance(upto);
+    pows_ = pows; book() = restored;
     return true;
 }
 
@@ -128,9 +130,9 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
     scan_dev_ = devs[0];
     if (!engine_for(scan_dev_)) return B200POST_ERR_NO_DEVICE;
 
+    rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{0, num_labels_}}, 0, opts_.nonces, windows_, cfg.k2);
     int rc;
     if (!load_state(written)) {
-        start_ = 0; restored_.clear();
         if ((rc = find_pows(opts_, kZeroChallenge, md.node_id, md.num_units, cfg.pow_difficulty, devs.data(), (int)devs.size(), 0,
                             nonces() / 16, &pows_, cancel)))
             return rc;
@@ -140,10 +142,9 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
     }
     const uint64_t chunk = std::min<uint64_t>({std::max<uint64_t>(batch, 1), kMaxScanChunk, num_labels_});
     if ((rc = sc_.init(scan_dev_, kZeroChallenge, nonces(), pows_.data(), cfg.k1, cfg.k2, num_labels_, chunk))) return rc;
-    sc_.restore(restored_);
     // the gap between the state's prefix and what is on disk, in index order, from the files
     PostDataReader reader(dir, md.max_file_size / 16);
-    for (uint64_t pos = start_; pos < written;) {
+    for (uint64_t pos = book().scanned(); pos < written;) {
         if (cancel && *cancel) { stop(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
         const uint64_t n = std::min<uint64_t>(chunk, written - pos);
         if ((rc = collect(b_)) || (rc = reader.read(pos, n, sc_.staging(b_))) || (rc = submit(b_, pos, n))) { stop(); return rc; }
@@ -194,7 +195,7 @@ int InitialProofScan::checkpoint() {
 // that failed to go in or come back, nothing more is folded: a later chunk would leave a hole below upto.
 int InitialProofScan::collect(int b) {
     if (failed_) { sc_.drain(); set_error("initial proof: an earlier scan chunk failed"); return B200POST_ERR_STATE; }
-    const int rc = sc_.collect(b);
+    const int rc = sc_.collect(b, &book());
     failed_ = rc != B200POST_OK;
     return rc;
 }
@@ -209,25 +210,17 @@ void InitialProofScan::stop() {
     const std::string err = last_error();
     for (int k = 0; k < 2 && !failed_; k++) collect(b_ ^ k);   // older chunk first; stops at a failure
     sc_.drain();
-    save_state();   // upto = the end of the folded prefix, whose hit lists are complete
+    save_state();   // upto = the end of the folded prefix, whose hits are all in the book
     set_error(err);   // the session reports its own failure, not the state's
 }
 
 int InitialProofScan::finish(b200post_proof_out *out, b200post_proof_metadata *meta) {
     int rc = checkpoint();
     if (rc) return rc;
-    if (start_ + sc_.scanned() != num_labels_) { set_error("initial proof: the scan does not cover every label"); return B200POST_ERR_STATE; }
+    if (book().scanned() != num_labels_) { set_error("initial proof: the scan does not cover every label"); return B200POST_ERR_STATE; }
     uint32_t nonce = 0;
     std::vector<uint64_t> idx;
-    bool have = false;
-    for (uint32_t w = 0; w < windows_ && !have; w++)   // the lowest window with a winner, as the prover's passes
-        have = pick_winner_in(sc_.lists(), w * opts_.nonces, (w + 1) * opts_.nonces, cfg_.k2, &nonce, &idx);
-    if (!have) {
-        set_error(windows_ == 1 ? std::string(kNoProof)
-                                : std::string(kNoProof) + " in nonce windows 0.." + std::to_string(windows_ - 1) + " (nonces [0, " +
-                                      std::to_string(nonces()) + "))");
-        return B200POST_ERR_INVALID_PROOF;
-    }
+    if (!rule_->decide(&nonce, &idx, &rc)) return no_proof(windows_, opts_.nonces);   // the lowest window with a winner
     if ((rc = write_proof(num_labels_, nonce, idx, pows_.data(), 0, num_labels_, out))) return rc;
     memset(meta, 0, sizeof *meta);
     memcpy(meta->node_id, md_.node_id, 32);

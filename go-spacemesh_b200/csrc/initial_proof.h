@@ -3,6 +3,7 @@
 // the data.  The session (setup.cu) drives it; the scan itself is the prover's (prove_internal.h).
 #pragma once
 #include <cstdint>
+#include <optional>
 #include <string>
 #include <vector>
 
@@ -37,7 +38,7 @@ public:
     int checkpoint();
     // cancel or failure: folds what finished, in order and up to the first failed chunk, then saves the state (best effort)
     void stop();
-    // After the last label: the winner (pick_winner over the first K2 hits per nonce), the proof record and the
+    // After the last label: the winner (the prover's window decision, ProveRule::decide), the proof record and the
     // verifier gate.  B200POST_ERR_INVALID_PROOF (reason in last_error) when no nonce reached K2 or the gate refused.
     int finish(b200post_proof_out *out, b200post_proof_metadata *meta);
 
@@ -50,6 +51,7 @@ private:
     int collect(int b);
     int submit(int b, uint64_t first, uint64_t count);
     uint32_t nonces() const { return opts_.nonces * windows_; }   // every nonce of the session's windows
+    HitBook &book() { return rule_->book(0); }
 
     std::string dir_;
     b200post_prove_opts opts_{};
@@ -60,8 +62,7 @@ private:
     uint64_t num_labels_ = 0;
     uint32_t scan_dev_ = 0;
     std::vector<uint64_t> pows_;
-    uint64_t start_ = 0;          // where this session's scanner began: the prefix below came from the state file
-    HitLists restored_;
+    std::optional<ProveRule> rule_;   // one shard, unchecked; its book holds the hits of the scanned prefix
     Scanner sc_;
     int b_ = 0;                   // staging buffer of the next chunk
     bool failed_ = false;         // a chunk failed to be submitted or collected

@@ -1,27 +1,26 @@
 // prover.cu — POST proof generation scan (include/b200post_prove.h, SURVEY.md §8f.3).
 //
 // K6 prove_scan_kernel streams 16-byte labels (H2D from the postdata files, double-buffered) through one
-// AES-128 cipher per nonce group and appends (nonce, index) hits to a small list; the host keeps the per-nonce
-// hit lists and stops when a nonce owns K2 of them.  Bandwidth view: 16 B in per label, ~nothing out; the
-// kernel is far faster than PCIe/NVMe can feed it, so the design goal is simply to keep copies and compute
-// overlapped.  Conventions: post-rs Prover8_56 from memory (ASSUMED, unpinned).
+// AES-128 cipher per nonce group and appends (nonce, index) hits to a small list; the host folds them into per-nonce
+// hit books and stops, under the rule of prove_rule.h, once a nonce owns K2 of them.  Bandwidth view: 16 B in per
+// label, ~nothing out; the kernel is far faster than PCIe/NVMe can feed it, so the design goal is simply to keep copies
+// and compute overlapped.  Conventions: post-rs Prover8_56 from memory (ASSUMED, unpinned).
 //
-// Several devices (b200post_generate_proof_multi): the label range is split into contiguous shards, one host thread and
-// Scanner each; their hit lists merge in shard order (ShardedScan), so the proof is the one-device proof.
+// Several devices (b200post_generate_proof_multi): the label range is split into contiguous shards, one host thread,
+// Scanner and hit book each (ShardedScan); the rule reads the books in shard order, so the proof is the one-device proof.
 //
-// Damaged stored data (b200post_generate_proof_checked): the kernels also return each hit's stored bytes (StoredHit), and
-// the stop rule's tentative winner has its first K2 hits recomputed and compared on the device before the scan may stop
-// on it; damaged hits are dropped (DESIGN.md §5).
+// Damaged stored data (b200post_generate_proof_checked): the same rule, with hits born pending instead of good.  The
+// kernels also return each hit's stored bytes (StoredHit), and the tentative winner has its first K2 hits recomputed and
+// compared on the device before the scan may stop on it; damaged hits are dropped (DESIGN.md §5).
 //
 // Nonce windows (b200post_prove_opts.max_windows): generate() runs passes over the data, each scanning windows_per_pass
 // windows of nonces with their own pows, until a window has a proof; the kernels only ever see pass-relative nonces.
 //
-// The scanner, the selection rule, the proof record, the pow step and the verifier gate are declared in prove_internal.h:
-// the setup session's initial proof (initial_proof.cu) runs the same scan over the labels as it writes them.
+// The scanner, the proof record, the pow step and the verifier gate are declared in prove_internal.h: the setup
+// session's initial proof (initial_proof.cu) runs the same scan over the labels as it writes them.
 #include <algorithm>
 #include <atomic>
 #include <functional>
-#include <map>
 #include <memory>
 #include <mutex>
 #include <set>
@@ -49,6 +48,9 @@ __device__ __forceinline__ Hit make_hit(const Hit *, uint32_t nonce, uint64_t in
 __device__ __forceinline__ StoredHit make_hit(const StoredHit *, uint32_t nonce, uint64_t index, uint4 label) {
     return StoredHit{nonce, 0, index, label};
 }
+// what the host folds into the hit book as the hit's stored bytes
+const uint8_t *stored_bytes(const Hit &) { return nullptr; }
+const uint8_t *stored_bytes(const StoredHit &h) { return reinterpret_cast<const uint8_t *>(&h.label); }
 
 // K6a: rk = per nonce group 11 round keys.  Every (label, group) costs one AES; ciphertext bytes below the
 // difficulty MSB are hits, bytes EQUAL to it (1 in 256) need the nonce's "lazy" cipher: those are queued as
@@ -136,19 +138,6 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
 
 }  // namespace
 
-bool pick_winner_in(const HitLists &lists, uint32_t lo, uint32_t hi, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
-    bool have = false;
-    for (auto it = lists.lower_bound(lo); it != lists.end() && it->first < hi; ++it) {
-        if (it->second.size() < k2) continue;
-        if (!have || it->second[k2 - 1] < (*indices)[k2 - 1]) { *nonce = it->first; *indices = it->second; have = true; }
-    }
-    return have;
-}
-
-bool pick_winner(const HitLists &lists, uint32_t k2, uint32_t *nonce, std::vector<uint64_t> *indices) {
-    return pick_winner_in(lists, 0, UINT32_MAX, k2, nonce, indices);
-}
-
 int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
                   uint64_t num_labels, uint64_t chunk, bool keep_stored, uint32_t first_nonce) {
     DeviceEngine *e = engine_for(provider);
@@ -158,7 +147,7 @@ int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonce
         set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
         return B200POST_ERR_INVALID_ARGUMENT;
     }
-    engine_ = e; dev_ = e->device(); nonces_ = nonces; first_ = first_nonce; k2_ = k2; chunk_ = chunk;
+    engine_ = e; dev_ = e->device(); nonces_ = nonces; first_ = first_nonce; chunk_ = chunk;
     stored_ = keep_stored; rec_ = stored_ ? sizeof(StoredHit) : sizeof(Hit);
     const uint64_t diff = b200post_proving_difficulty(k1, num_labels);
     msb_ = (uint32_t)(diff >> 56); lsb_ = diff & 0x00ffffffffffffffull;
@@ -242,59 +231,30 @@ int Scanner::submit(int b, uint64_t first, uint32_t count) {
     return B200POST_OK;
 }
 
-int Scanner::collect(int b, std::mutex *fold_mu) {
+int Scanner::collect(int b, HitBook *book, std::mutex *fold_mu) {
     if (!pending_[b]) return B200POST_OK;
     CUDA_TRY(cudaEventSynchronize(ev_[b].get()));
     pending_[b] = false;
     const uint32_t n = *h_nhits_[b].get();
     if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
-    if (stored_) return fold_stored(b, n, fold_mu);
-    const Hit *rec = reinterpret_cast<const Hit *>(h_hits_[b].get());
-    std::vector<Hit> v(rec, rec + n);
-    std::sort(v.begin(), v.end(), [](const Hit &x, const Hit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
-    std::unique_lock<std::mutex> lk;
-    if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
-    for (const Hit &h : v) {
-        std::vector<uint64_t> &l = lists_[first_ + h.nonce];
-        if (l.size() < k2_ && (l.push_back(h.index), l.size() == k2_)) full_++;
-    }
-    scanned_ += count_[b];   // chunks are contiguous from the first index: the sum is how far the scan went
+    if (stored_) fold<StoredHit>(b, n, book, fold_mu);
+    else fold<Hit>(b, n, book, fold_mu);
     return B200POST_OK;
 }
 
-int Scanner::fold_stored(int b, uint32_t n, std::mutex *fold_mu) {
-    const StoredHit *rec = reinterpret_cast<const StoredHit *>(h_hits_[b].get());
-    std::vector<StoredHit> v(rec, rec + n);
-    std::sort(v.begin(), v.end(), [](const StoredHit &x, const StoredHit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+template <class Rec>
+void Scanner::fold(int b, uint32_t n, HitBook *book, std::mutex *fold_mu) {
+    const Rec *rec = reinterpret_cast<const Rec *>(h_hits_[b].get());
+    std::vector<Rec> v(rec, rec + n);
+    std::sort(v.begin(), v.end(), [](const Rec &x, const Rec &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
     std::unique_lock<std::mutex> lk;
     if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
-    for (const StoredHit &h : v) {
-        KeptHit k{h.index, {}, false};
-        memcpy(k.label, &h.label, 16);
-        kept_[first_ + h.nonce].push_back(k);
-    }
-    scanned_ += count_[b];
-    return B200POST_OK;
+    for (const Rec &h : v) book->add(first_ + h.nonce, h.index, stored_bytes(h));
+    book->advance(count_[b]);   // chunks are contiguous from the first index: the sum is how far the scan went
 }
 
 void Scanner::drain() {
     for (int b = 0; b < 2; b++) if (pending_[b]) { cudaEventSynchronize(ev_[b].get()); pending_[b] = false; }
-}
-
-void Scanner::restore(const HitLists &lists) {
-    lists_ = lists;
-    full_ = 0;
-    for (const auto &kv : lists_) full_ += kv.second.size() >= k2_;
-}
-
-uint32_t Scanner::count_kept(bool good_only) const {
-    uint32_t full = 0;
-    for (const auto &kv : kept_) {
-        size_t c = 0;
-        for (const KeptHit &k : kv.second) if ((c += !good_only || k.good) >= k2_) break;
-        full += c >= k2_;
-    }
-    return full;
 }
 
 namespace {
@@ -319,31 +279,24 @@ std::vector<std::pair<uint64_t, uint64_t>> split_shards(uint64_t total, uint64_t
     return out;
 }
 
-// A scan split into shards, one host thread each.  Stop rule: let x be the end of the longest gap-free scanned prefix
-// of [0, total), where a saturated shard counts as whole.  Once the hits below x give some nonce K2 of them the proof is
-// decided (every hit below x is known, so no nonce whose K2-th hit lies past x can win) and every shard stops.  A shard
-// also stops on its own once it is saturated.  With one shard this is "stop once a nonce has K2 hits".
-// One pass of a windowed proof scans `windows` nonce windows of `window` nonces from nonce `first`; the stop rule then
-// looks at the pass's lowest window only, saturation at every nonce of the pass, and the decision walks the windows in
-// order (DESIGN.md §5).
+// One pass's scan split into shards, one host thread, Scanner and hit book each, driving the pass's ProveRule: its stop
+// rule after every chunk, its decision once every thread has joined.  With a commitment (the checked proof) hits are
+// born pending and the rule's recheck recomputes labels on the devices.
 class ShardedScan {
 public:
     // fill(shard, first label, count, dst): those labels into the shard's pinned staging
     using Fill = std::function<int(size_t, uint64_t, uint64_t, uint8_t *)>;
 
-    ShardedScan(size_t n, uint32_t first, uint32_t window, uint32_t windows, uint32_t k2)
-        : first_(first), window_(window), windows_(windows), k2_(k2) {
-        for (size_t s = 0; s < n; s++) shards_.emplace_back(new Shard);
+    // ranges[s]: shard s's labels [lo, hi); the pass scans `windows` nonce windows of `window` nonces from nonce `first`
+    ShardedScan(const std::vector<std::pair<uint64_t, uint64_t>> &ranges, uint32_t first, uint32_t window, uint32_t windows,
+                uint32_t k2, const uint8_t *commitment = nullptr, uint64_t N = 0, const volatile int *cancel = nullptr)
+        : rule_(ranges, first, window, windows, k2, commitment ? ProveRule::Recheck([this](auto &&...a) { return recheck(a...); }) : nullptr),
+          N_(N), cancel_(cancel) {
+        if (commitment) memcpy(commitment_, commitment, 32);
+        for (const auto &r : ranges) shards_.emplace_back(new Shard{{}, r.first, r.second});
     }
-    Shard &shard(size_t s) { return *shards_[s]; }
-
-    // After run() (unchecked): the winner of the lowest window of the pass that has one, over merged()
-    bool winner(uint32_t *nonce, std::vector<uint64_t> *indices) const {
-        const HitLists m = merged();
-        for (uint32_t w = 0; w < windows_; w++)
-            if (pick_winner_in(m, lo(w), lo(w) + window_, k2_, nonce, indices)) return true;
-        return false;
-    }
+    Scanner &scanner(size_t s) { return shards_[s]->sc; }
+    ProveRule &rule() { return rule_; }
 
     // runs every shard (the calling thread alone when there is one) and returns the first failing shard's status, in
     // list order, once every thread has joined
@@ -360,164 +313,31 @@ public:
         return B200POST_OK;
     }
 
-    // per nonce, the shards' hit lists appended in shard order, first K2 kept; with the stop rule above, the winner of
-    // these lists is the winner of a scan over every label
-    HitLists merged() const {
-        HitLists m;
-        for (const auto &sh : shards_)
-            for (const auto &kv : sh->sc.lists()) {
-                std::vector<uint64_t> &l = m[kv.first];
-                for (size_t i = 0; i < kv.second.size() && l.size() < k2_; i++) l.push_back(kv.second[i]);
-            }
-        return m;
-    }
-    uint64_t scanned() const {
-        uint64_t t = 0;
-        for (const auto &sh : shards_) t += sh->sc.scanned();
-        return t;
-    }
-
-    // ---- the checked proof (b200post_generate_proof_checked): every hit is kept with its stored bytes, and the stop
-    // rule's tentative winner has its first K2 hits recomputed under `commitment` before the scan may stop on it
-    void enable_check(const uint8_t commitment[32], uint64_t N, const volatile int *cancel) {
-        checked_ = true;
-        memcpy(commitment_, commitment, 32);
-        N_ = N; cancel_ = cancel;
-    }
-    // After run(): per window of the pass in order, recheck rounds over everything kept until the window's winner has
-    // its first K2 hits all good (the winner and its indices) or no nonce of it has K2 usable hits (the next window);
-    // false with *rc OK when no window has one.  Needs no round when the scan stopped on a decision.
-    bool decide(uint32_t *nonce, std::vector<uint64_t> *indices, int *rc) {
-        *rc = B200POST_OK;
-        for (uint32_t w = 0; w < windows_; w++)
-            for (;;) {
-                std::vector<Item> items;
-                const Plan p = plan_winner(w, &items, nonce, indices);
-                if (p == DECIDED) return true;
-                if (p == NONE) break;
-                if ((*rc = round(shards_[0]->sc.engine(), items))) return false;
-            }
-        return false;
-    }
-    uint64_t rechecked() const { return rechecked_; }
-    uint32_t rounds() const { return rounds_; }
-    const std::set<uint64_t> &damaged() const { return damaged_; }
-
 private:
-    struct Item { size_t shard; uint32_t nonce; uint64_t index; uint8_t label[16]; };
-    enum Plan { NONE, DECIDED, RECHECK };
-
-    uint32_t lo(uint32_t w) const { return first_ + w * window_; }   // the first nonce of window w of the pass
-
-    // Under mu_ (or with the threads joined).  The stop rule over kept (good and pending) hits below x of the nonces of
-    // window w of the pass: NONE if no such nonce has K2 of them; DECIDED with the winner when the winner's first K2 are
-    // all good; RECHECK with the pending ones.
-    Plan plan_winner(uint32_t w, std::vector<Item> *items, uint32_t *nonce, std::vector<uint64_t> *indices) const {
-        struct Ref { size_t shard; const KeptHit *k; };
-        std::map<uint32_t, std::vector<Ref>> m;   // per nonce, its first K2 kept hits below x in shard order
-        for (size_t s = 0; s < shards_.size(); s++) {
-            const Scanner &sc = shards_[s]->sc;
-            for (auto kv = sc.kept().lower_bound(lo(w)); kv != sc.kept().end() && kv->first < lo(w) + window_; ++kv) {
-                std::vector<Ref> &l = m[kv->first];
-                for (size_t i = 0; i < kv->second.size() && l.size() < k2_; i++) l.push_back({s, &kv->second[i]});
-            }
-            if (sc.scanned() < shards_[s]->hi - shards_[s]->lo && !sc.saturated()) break;   // x lies in this shard
-        }
-        const std::pair<const uint32_t, std::vector<Ref>> *win = nullptr;
-        for (const auto &kv : m)
-            if (kv.second.size() >= k2_ && (!win || kv.second[k2_ - 1].k->index < win->second[k2_ - 1].k->index)) win = &kv;
-        if (!win) return NONE;
-        for (const Ref &r : win->second) {
-            if (r.k->good) continue;
-            Item it{r.shard, win->first, r.k->index, {}};
-            memcpy(it.label, r.k->label, 16);
-            items->push_back(it);
-        }
-        if (!items->empty()) return RECHECK;
-        *nonce = win->first;
-        indices->clear();
-        for (const Ref &r : win->second) indices->push_back(r.k->index);
-        return DECIDED;
-    }
-    // Under mu_: when every nonce has K2 kept hits in shard s but not K2 good ones, the pending ones among each nonce's
-    // first K2 in the shard (the shard's own saturation stop counts good hits only).
-    bool plan_saturation(size_t s, std::vector<Item> *items) const {
-        const Scanner &sc = shards_[s]->sc;
-        if (sc.count_kept(false) != sc.nonces()) return false;
-        for (const auto &kv : sc.kept())
-            for (size_t i = 0; i < kv.second.size() && i < k2_; i++) {
-                const KeptHit &k = kv.second[i];
-                if (k.good) continue;
-                Item it{s, kv.first, k.index, {}};
-                memcpy(it.label, k.label, 16);
-                items->push_back(it);
-            }
-        return !items->empty();
-    }
-    // One recheck round on `e` (outside mu_): the items' labels recomputed and compared with their stored bytes, then,
-    // under mu_ when threads run, good ones marked and damaged ones dropped.  A compare reports at most
-    // CompareResult::kMaxReported positions, so it is repeated past the last reported one until every mismatch is known.
-    int round(DeviceEngine *e, const std::vector<Item> &items) {
+    // The rule's recheck on shard s's device: the items' labels recomputed under the commitment and compared with their
+    // stored bytes.  A compare reports at most CompareResult::kMaxReported positions, so it is repeated past the last
+    // reported one until every mismatch is known.
+    int recheck(size_t s, const std::vector<RecheckItem> &items, std::vector<uint8_t> *bad) {
         const size_t n = items.size();
         std::vector<uint64_t> idx(n);
-        std::vector<uint8_t> expect(n * 16), bad(n, 0);
+        std::vector<uint8_t> expect(n * 16);
         for (size_t i = 0; i < n; i++) { idx[i] = items[i].index; memcpy(&expect[i * 16], items[i].label, 16); }
         for (size_t from = 0; from < n;) {
             CompareResult cmp;
-            const int rc = e->labels_compare_indexed(commitment_, n - from, idx.data() + from, N_, expect.data() + from * 16, &cmp, cancel_);
+            const int rc = shards_[s]->sc.engine()->labels_compare_indexed(commitment_, n - from, idx.data() + from, N_,
+                                                                           expect.data() + from * 16, &cmp, cancel_);
             if (rc) return rc;
-            for (uint64_t p : cmp.first) bad[from + p] = 1;
+            for (uint64_t p : cmp.first) (*bad)[from + p] = 1;
             if (cmp.mismatches <= cmp.first.size()) break;
             from += cmp.first.back() + 1;
         }
-        std::unique_lock<std::mutex> lk(mu_);
-        for (size_t i = 0; i < n; i++) {
-            std::vector<KeptHit> &l = shards_[items[i].shard]->sc.kept()[items[i].nonce];
-            auto it = std::lower_bound(l.begin(), l.end(), items[i].index, [](const KeptHit &k, uint64_t v) { return k.index < v; });
-            if (it == l.end() || it->index != items[i].index) continue;
-            if (bad[i]) { l.erase(it); damaged_.insert(items[i].index); }
-            else it->good = true;
-        }
-        rechecked_ += n; rounds_++;
         return B200POST_OK;
     }
-    // The checked stop rule for shard s, run by its thread after each chunk: stop once a decision is taken or the shard is
-    // saturated by good hits.  When the multi-device stop rule fires (or the shard would saturate) this thread runs recheck
-    // rounds until that settles, while the other shards keep scanning.  One winner round runs at a time; a saturation
-    // round touches only its own shard's hits.
-    bool should_stop_checked(size_t s, int *rc) {
-        for (;;) {
-            std::vector<Item> items;
-            bool winner_round = false;
-            {
-                std::lock_guard<std::mutex> lk(mu_);
-                if (decided_ || shards_[s]->sc.saturated()) return true;
-                if (!round_busy_) {
-                    uint32_t nonce;
-                    std::vector<uint64_t> idx;
-                    const Plan p = plan_winner(0, &items, &nonce, &idx);   // the pass's lowest window decides the stop
-                    if (p == DECIDED) { decided_ = true; return true; }
-                    winner_round = round_busy_ = p == RECHECK;
-                }
-                if (!winner_round && !plan_saturation(s, &items)) return false;
-            }
-            *rc = round(shards_[s]->sc.engine(), items);
-            if (winner_round) { std::lock_guard<std::mutex> lk(mu_); round_busy_ = false; }
-            if (*rc) return true;
-        }
-    }
 
-    bool checked_ = false, decided_ = false, round_busy_ = false;   // the last two under mu_
-    uint8_t commitment_[32] = {0};
-    uint64_t N_ = 0;
-    const volatile int *cancel_ = nullptr;
-    uint64_t rechecked_ = 0;                 // under mu_
-    uint32_t rounds_ = 0;
-    std::set<uint64_t> damaged_;
     int run_shard(size_t s, const Fill &fill, uint64_t chunk, uint64_t base, const volatile int *cancel) {
         Shard &sh = *shards_[s];
         Scanner &sc = sh.sc;
-        std::mutex *mu = shards_.size() > 1 || checked_ ? &mu_ : nullptr;
+        HitBook &book = rule_.book(s);
         int rc = B200POST_OK;
         if (sh.lo == sh.hi) return rc;
         if (cudaSetDevice(sc.device()) != cudaSuccess) { cudaGetLastError(); set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
@@ -525,8 +345,8 @@ private:
         for (uint64_t pos = sh.lo; pos < sh.hi; b ^= 1) {
             if (cancel && *cancel) { sc.drain(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
             if (abort_) { sc.drain(); return B200POST_OK; }   // another shard failed: its status is the call's
-            if ((rc = sc.collect(b, mu))) { sc.drain(); return rc; }
-            const bool stop = checked_ ? should_stop_checked(s, &rc) : should_stop(s);
+            if ((rc = sc.collect(b, &book, &mu_))) { sc.drain(); return rc; }
+            const bool stop = rule_.should_stop(s, mu_, &rc);
             if (rc) { sc.drain(); return rc; }
             if (stop) break;
             // fill the staging buffer (a chunk may span files)
@@ -534,36 +354,16 @@ private:
             if ((rc = fill(s, pos, n, sc.staging(b))) || (rc = sc.submit(b, base + pos, (uint32_t)n))) { sc.drain(); return rc; }
             pos += n;
         }
-        for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, mu))) { sc.drain(); return rc; }   // older chunk first
+        for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, &book, &mu_))) { sc.drain(); return rc; }   // older chunk first
         return B200POST_OK;
     }
 
-    // The unchecked stop rule, over the nonces of the pass's lowest window (a saturated shard has every nonce of the
-    // pass at K2, that window's included)
-    bool should_stop(size_t s) {
-        if (shards_.size() == 1) {
-            if (windows_ == 1) return shards_[0]->sc.any_full();
-            const HitLists &l = shards_[0]->sc.lists();
-            for (auto kv = l.lower_bound(first_); kv != l.end() && kv->first < first_ + window_; ++kv)
-                if (kv->second.size() >= k2_) return true;
-            return false;
-        }
-        std::lock_guard<std::mutex> lk(mu_);
-        if (shards_[s]->sc.saturated()) return true;
-        below_x_.assign(window_, 0);   // hits below x per nonce of the window
-        for (const auto &sh : shards_) {
-            const HitLists &l = sh->sc.lists();
-            for (auto kv = l.lower_bound(first_); kv != l.end() && kv->first < first_ + window_; ++kv)
-                if ((below_x_[kv->first - first_] += kv->second.size()) >= k2_) return true;
-            if (sh->sc.scanned() < sh->hi - sh->lo && !sh->sc.saturated()) break;   // x lies in this shard
-        }
-        return false;
-    }
-
-    uint32_t first_, window_, windows_, k2_;
+    ProveRule rule_;
+    uint8_t commitment_[32] = {0};
+    uint64_t N_ = 0;
+    const volatile int *cancel_ = nullptr;
     std::vector<std::unique_ptr<Shard>> shards_;
-    std::mutex mu_;                  // guards every shard's hit lists and progress once the threads run
-    std::vector<uint64_t> below_x_;
+    std::mutex mu_;                  // guards every shard's hit book and the rule's state once the threads run
     std::atomic<bool> abort_{false};
 };
 
@@ -579,7 +379,12 @@ int write_proof(uint64_t scanned, uint32_t nonce, const std::vector<uint64_t> &i
     return B200POST_OK;
 }
 
-const char *const kNoProof = "no proof found: no nonce reached K2 qualifying labels";
+int no_proof(uint32_t windows, uint32_t n) {
+    std::string e = "no proof found: no nonce reached K2 qualifying labels";
+    if (windows > 1) e += " in nonce windows 0.." + std::to_string(windows - 1) + " (nonces [0, " + std::to_string((uint64_t)windows * n) + "))";
+    set_error(e);
+    return B200POST_ERR_INVALID_PROOF;
+}
 
 int check_pow_mode(const b200post_prove_opts &o) {
     if (o.pow_mode > B200POST_POW_SKIP || (o.pow_mode == B200POST_POW_CALLBACK && !o.pow_prove)) {
@@ -637,27 +442,6 @@ int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scry
     return B200POST_OK;
 }
 
-namespace {
-
-// The checked proof's decision step for one pass: recheck rounds until the winner over usable hits is known (false: the
-// pass has none), then the report, which adds up over the passes (`damaged`: every distinct damaged index so far).
-bool decide_checked(ShardedScan &scan, uint32_t *nonce, std::vector<uint64_t> *idx, std::set<uint64_t> *damaged,
-                    b200post_prove_check *check, int *rc) {
-    const bool have = scan.decide(nonce, idx, rc);
-    const size_t before = damaged->size();
-    damaged->insert(scan.damaged().begin(), scan.damaged().end());
-    check->labels_rechecked += scan.rechecked(); check->rounds += scan.rounds(); check->damaged = damaged->size();
-    check->n_reported = 0;
-    for (uint64_t i : *damaged) {   // ascending
-        if (check->n_reported == 64) break;
-        check->damaged_index[check->n_reported++] = i;
-    }
-    metrics().prove_labels_rechecked_total += scan.rechecked();
-    metrics().prove_damaged_labels_total += damaged->size() - before;
-    return have;
-}
-
-}  // namespace
 }  // namespace b200post
 
 using namespace b200post;
@@ -690,12 +474,10 @@ extern "C" {
 int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t first_index, uint64_t count, const uint8_t challenge[32],
                         uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2, uint64_t num_labels, b200post_proof_out *out) {
     if (!labels16 || !challenge || !pows || !out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    ShardedScan scan(1, 0, nonces, 1, k2);
-    Shard &sh = scan.shard(0);
+    ShardedScan scan({{0, count}}, 0, nonces, 1, k2);
     const uint64_t chunk = std::min<uint64_t>(std::max<uint64_t>(count, 1), 1u << 22);
-    int rc = sh.sc.init(provider, challenge, nonces, pows, k1, k2, num_labels, chunk);
+    int rc = scan.scanner(0).init(provider, challenge, nonces, pows, k1, k2, num_labels, chunk);
     if (rc) return rc;
-    sh.lo = 0; sh.hi = count;
     rc = scan.run([&](size_t, uint64_t off, uint64_t n, uint8_t *dst) {
         parallel_copy(dst, labels16 + off * 16, (size_t)n * 16);   // pageable -> pinned staging, the scan's host-side bound
         return B200POST_OK;
@@ -703,8 +485,8 @@ int b200post_prove_scan(uint32_t provider, const uint8_t *labels16, uint64_t fir
     if (rc) return rc;
     uint32_t nonce = 0;
     std::vector<uint64_t> idx;
-    if (!scan.winner(&nonce, &idx)) { set_error(kNoProof); return B200POST_ERR_INVALID_PROOF; }
-    return write_proof(scan.scanned(), nonce, idx, pows, 0, num_labels, out);
+    if (!scan.rule().decide(&nonce, &idx, &rc)) return no_proof(1, nonces);
+    return write_proof(scan.rule().scanned(), nonce, idx, pows, 0, num_labels, out);
 }
 
 int b200post_generate_proof(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
@@ -734,7 +516,7 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
 
 namespace {
 // b200post_generate_proof_multi (check == nullptr) and b200post_generate_proof_checked: they differ only in the scan's
-// hit records and the decision step (ShardedScan::enable_check, finish_checked) and the final verifier gate
+// hit records, whether hits are born pending (the ShardedScan's commitment), the report and the final verifier gate
 int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
              const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
              b200post_prove_check *check, const volatile int *cancel) {
@@ -752,6 +534,8 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
         return B200POST_ERR_IO;
     }
     if ((rc = check_pow_mode(o))) return rc;
+    const uint64_t per_file = md.max_file_size / 16;
+    if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
     // the nonce windows [w*n, (w+1)*n) to try, `per_pass` of them per read of the data (b200post_prove_opts)
     const uint32_t n = o.nonces, windows = std::min(std::max(o.max_windows, 1u), 4096 / n);
     const uint32_t per_pass = std::max(o.windows_per_pass, 1u);
@@ -759,7 +543,6 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
     const auto ranges = split_shards(num_labels, chunk, (size_t)n_providers);
     uint8_t commitment[32];
     if (check) commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
-    const uint64_t per_file = md.max_file_size / 16;
     uint64_t scanned = 0;              // over every pass
     std::set<uint64_t> damaged;        // the checked report's, over every pass
     bool have = false;
@@ -771,34 +554,38 @@ int generate(const char *data_dir, const uint8_t challenge[32], const b200post_p
                             &pows, cancel)))
             return rc;
         // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
-        ShardedScan scan((size_t)n_providers, first, n, m, cfg->k2);
-        if (check) scan.enable_check(commitment, md.scrypt_n, cancel);
-        for (int s = 0; s < n_providers; s++) {
-            Shard &sh = scan.shard((size_t)s);
-            if ((rc = sh.sc.init(providers[s], challenge, m * n, pows.data(), cfg->k1, cfg->k2, num_labels, chunk, check != nullptr, first)))
+        ShardedScan scan(ranges, first, n, m, cfg->k2, check ? commitment : nullptr, md.scrypt_n, cancel);
+        for (int s = 0; s < n_providers; s++)
+            if ((rc = scan.scanner((size_t)s).init(providers[s], challenge, m * n, pows.data(), cfg->k1, cfg->k2, num_labels, chunk,
+                                                   check != nullptr, first)))
                 return rc;
-            sh.lo = ranges[(size_t)s].first; sh.hi = ranges[(size_t)s].second;
-        }
-        if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
         std::vector<std::unique_ptr<PostDataReader>> readers;
         for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
         rc = scan.run([&](size_t s, uint64_t pos, uint64_t cnt, uint8_t *dst) { return readers[s]->read(pos, cnt, dst); }, chunk, 0, cancel);
         if (rc) return rc;
         metrics().prove_passes_total++;
-        scanned += scan.scanned();
+        ProveRule &rule = scan.rule();
+        scanned += rule.scanned();
         uint32_t nonce = 0;
         std::vector<uint64_t> idx;
-        have = check ? decide_checked(scan, &nonce, &idx, &damaged, check, &rc) : scan.winner(&nonce, &idx);
+        have = rule.decide(&nonce, &idx, &rc);
+        if (check) {   // the checked report adds up over the passes (`damaged`: every distinct damaged index so far)
+            const size_t before = damaged.size();
+            damaged.insert(rule.damaged().begin(), rule.damaged().end());
+            check->labels_rechecked += rule.rechecked(); check->rounds += rule.rounds(); check->damaged = damaged.size();
+            check->n_reported = 0;
+            for (uint64_t i : damaged) {   // ascending
+                if (check->n_reported == 64) break;
+                check->damaged_index[check->n_reported++] = i;
+            }
+            metrics().prove_labels_rechecked_total += rule.rechecked();
+            metrics().prove_damaged_labels_total += damaged.size() - before;
+        }
         if (rc) return rc;
         if (have && (rc = write_proof(scanned, nonce, idx, pows.data(), first, num_labels, out))) return rc;
         a += m;
     }
-    if (!have) {
-        set_error(windows == 1 ? std::string(kNoProof)
-                               : std::string(kNoProof) + " in nonce windows 0.." + std::to_string(windows - 1) + " (nonces [0, " +
-                                     std::to_string((uint64_t)windows * n) + "))");
-        return B200POST_ERR_INVALID_PROOF;
-    }
+    if (!have) return no_proof(windows, n);
     b200post_proof_metadata meta;
     memcpy(meta.node_id, md.node_id, 32);
     memcpy(meta.commitment_atx_id, md.commitment_atx_id, 32);
