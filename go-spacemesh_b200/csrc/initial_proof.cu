@@ -15,6 +15,7 @@ namespace b200post {
 
 const char kInitialProofFile[] = "initial_post.json";
 const char kInitialScanFile[] = "initial_post.scan";
+const char kRangeRecordPrefix[] = "range_";
 
 namespace {
 
@@ -37,15 +38,30 @@ std::string join(const std::string &d, const char *f) { return d.empty() || d.ba
 
 }  // namespace
 
-// Everything the scan's result depends on besides the labels: a state whose header differs is someone else's.
+// Everything the scan's result depends on besides the labels: a state whose header differs is someone else's.  A
+// record adds the POST's file size and its own range, and carries the proof part only when it was asked for.
 std::string InitialProofScan::header() const {
-    std::string h("B2IPSCAN", 8);
+    std::string h(record_ ? "B2RNGREC" : "B2IPSCAN", 8);
     put<uint32_t>(&h, 1);   // layout version
     h.append(reinterpret_cast<const char *>(md_.node_id), 32);
     h.append(reinterpret_cast<const char *>(md_.commitment_atx_id), 32);
     put<uint32_t>(&h, md_.num_units);
     put<uint64_t>(&h, md_.labels_per_unit);
     put<uint64_t>(&h, md_.scrypt_n);
+    if (record_) {
+        put<uint64_t>(&h, md_.max_file_size);
+        put<uint64_t>(&h, range_.from_file);
+        put<uint64_t>(&h, range_.to_file);
+        put<uint64_t>(&h, range_.lo);
+        put<uint64_t>(&h, range_.hi);
+        put<uint32_t>(&h, proof_);
+    }
+    if (proof_) h += proof_part();
+    return h;
+}
+
+std::string InitialProofScan::proof_part() const {
+    std::string h;
     put<uint32_t>(&h, cfg_.k1);
     put<uint32_t>(&h, cfg_.k2);
     put<uint32_t>(&h, opts_.nonces);
@@ -54,23 +70,35 @@ std::string InitialProofScan::header() const {
     put<uint32_t>(&h, opts_.pow_mode);
     put<uint32_t>(&h, (uint32_t)key_.size());
     h.append(key_.begin(), key_.end());
-    if (windows_ > 1) put<uint32_t>(&h, windows_);   // absent for one window: such states stay valid
+    if (record_ || windows_ > 1) put<uint32_t>(&h, windows_);   // absent from a one-window state: such states stay valid
     return h;
 }
 
-// header | pows | upto | lists (count, then nonce, length, indices) | FNV-1a 64 of everything before it
+std::string InitialProofScan::record_path() const {
+    return join(dir_, (std::string(kRangeRecordPrefix) + std::to_string(range_.from_file) + "_" + std::to_string(range_.to_file) + ".rec").c_str());
+}
+
+// header | pows | upto | lists (count, then nonce, length, indices) | a record's VRF best (found, index, label32) |
+// FNV-1a 64 of everything before it.  A record without the scan has no pows and no lists.
 int InitialProofScan::save_state() {
     std::string s = header();
     for (uint64_t p : pows_) put<uint64_t>(&s, p);
-    put<uint64_t>(&s, book().scanned());
-    put<uint32_t>(&s, (uint32_t)book().lists().size());
-    for (const auto &kv : book().lists()) {
-        put<uint32_t>(&s, kv.first);
-        put<uint32_t>(&s, (uint32_t)kv.second.size());
-        for (const KeptHit &k : kv.second) put<uint64_t>(&s, k.index);
+    put<uint64_t>(&s, upto());
+    if (proof_) {
+        put<uint32_t>(&s, (uint32_t)book().lists().size());
+        for (const auto &kv : book().lists()) {
+            put<uint32_t>(&s, kv.first);
+            put<uint32_t>(&s, (uint32_t)kv.second.size());
+            for (const KeptHit &k : kv.second) put<uint64_t>(&s, k.index);
+        }
+    }
+    if (record_) {
+        put<uint32_t>(&s, vrf_.found);
+        put<uint64_t>(&s, vrf_.index);
+        s.append(reinterpret_cast<const char *>(vrf_.label32), 32);
     }
     put<uint64_t>(&s, fnv1a64(s));
-    const std::string fin = join(dir_, kInitialScanFile), tmp = fin + ".tmp";
+    const std::string fin = record_ ? record_path() : join(dir_, kInitialScanFile), tmp = fin + ".tmp";
     FILE *f = fopen(tmp.c_str(), "wb");
     if (!f) { set_error("open " + tmp + ": " + strerror(errno)); return B200POST_ERR_IO; }
     const bool ok = fwrite(s.data(), 1, s.size(), f) == s.size();
@@ -79,14 +107,8 @@ int InitialProofScan::save_state() {
     return B200POST_OK;
 }
 
-bool InitialProofScan::load_state(uint64_t written) {
-    FILE *f = fopen(join(dir_, kInitialScanFile).c_str(), "rb");
-    if (!f) return false;
-    std::string s;
-    char buf[65536];
-    size_t n;
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, n);
-    fclose(f);
+// The state in s, if it is intact, has this object's header and covers a prefix ending at or below `written`.
+bool InitialProofScan::decode(const std::string &s, uint64_t written) {
     const std::string h = header();
     if (s.size() < h.size() + 8 || s.compare(0, h.size(), h) != 0) return false;
     uint64_t sum;
@@ -94,34 +116,97 @@ bool InitialProofScan::load_state(uint64_t written) {
     const std::string body = s.substr(0, s.size() - 8);
     if (fnv1a64(body) != sum) return false;
     size_t p = h.size();
-    std::vector<uint64_t> pows(nonces() / 16);
+    std::vector<uint64_t> pows(proof_ ? nonces() / 16 : 0);
     for (uint64_t &v : pows) if (!get(body, &p, &v)) return false;
     uint64_t upto;
-    uint32_t n_lists;
-    if (!get(body, &p, &upto) || upto > written || upto > num_labels_ || !get(body, &p, &n_lists)) return false;
-    HitBook restored(nonces(), cfg_.k2, true);
+    if (!get(body, &p, &upto) || upto > written || upto < range_.lo || upto > range_.hi) return false;
+    HitBook restored(proof_ ? nonces() : 0, cfg_.k2, true);
+    uint32_t n_lists = 0;
+    if (proof_ && !get(body, &p, &n_lists)) return false;
     for (uint32_t i = 0; i < n_lists; i++) {
         uint32_t nonce, len;
         if (!get(body, &p, &nonce) || !get(body, &p, &len) || nonce >= nonces() || len > cfg_.k2) return false;
         for (uint64_t j = 0, v; j < len; j++) {
-            if (!get(body, &p, &v) || v >= upto) return false;
+            if (!get(body, &p, &v) || v < range_.lo || v >= upto) return false;
             restored.add(nonce, v, nullptr);
         }
     }
+    b200post_vrf_nonce vrf{};
+    if (record_) {
+        // the best may lie past upto (the labels after it were computed, then the session stopped), never past hi
+        if (!get(body, &p, &vrf.found) || vrf.found > 1 || !get(body, &p, &vrf.index) || p + 32 > body.size()) return false;
+        memcpy(vrf.label32, body.data() + p, 32);
+        p += 32;
+        if (vrf.found && (vrf.index < range_.lo || vrf.index >= range_.hi)) return false;
+    }
     if (p != body.size()) return false;
-    restored.advance(upto);
-    pows_ = pows; book() = restored;
+    restored.advance(upto - range_.lo);
+    pows_ = pows; vrf_ = vrf; upto_ = upto;
+    if (proof_) book() = restored;
     return true;
 }
 
-int InitialProofScan::begin(const InitialProofRequest &req, const std::string &dir, const b200post_post_metadata &md,
-                            const b200post_post_config &cfg, int64_t provider_id, uint64_t written, uint64_t batch,
-                            const volatile int *cancel) {
-    dir_ = dir; opts_ = req.opts; key_ = req.cache_key; md_ = md; cfg_ = cfg;
-    windows_ = std::max(opts_.windows_per_pass, 1u);
-    opts_.pow_cache_key = key_.empty() ? nullptr : key_.data();
-    opts_.pow_cache_key_len = key_.size();
+bool InitialProofScan::load_state(uint64_t written) {
+    FILE *f = fopen((record_ ? record_path() : join(dir_, kInitialScanFile)).c_str(), "rb");
+    if (!f) return false;
+    std::string s;
+    char buf[65536];
+    size_t n;
+    while ((n = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, n);
+    fclose(f);
+    return decode(s, written);
+}
+
+bool InitialProofScan::read_record(const std::string &s) {
+    // the fields header() writes, in its order; decode() then compares the whole header as header() re-encodes it
+    size_t p = 8;
+    uint32_t version, proof = 0, key_len = 0;
+    record_ = true;
+    if (s.size() < 8 || s.compare(0, 8, "B2RNGREC") != 0 || !get(s, &p, &version) || version != 1 || p + 64 > s.size()) return false;
+    memcpy(md_.node_id, s.data() + p, 32);
+    memcpy(md_.commitment_atx_id, s.data() + p + 32, 32);
+    p += 64;
+    if (!get(s, &p, &md_.num_units) || !get(s, &p, &md_.labels_per_unit) || !get(s, &p, &md_.scrypt_n) ||
+        !get(s, &p, &md_.max_file_size) || !get(s, &p, &range_.from_file) || !get(s, &p, &range_.to_file) ||
+        !get(s, &p, &range_.lo) || !get(s, &p, &range_.hi) || !get(s, &p, &proof) || proof > 1)
+        return false;
+    proof_ = proof;
+    const unsigned __int128 nl = (unsigned __int128)md_.num_units * md_.labels_per_unit;
+    if (nl == 0 || nl > (~0ull >> 4) || range_.lo >= range_.hi || range_.hi > (uint64_t)nl) return false;
+    num_labels_ = (uint64_t)nl;
+    if (proof_) {
+        if (!get(s, &p, &cfg_.k1) || !get(s, &p, &cfg_.k2) || !get(s, &p, &opts_.nonces) || p + 64 > s.size()) return false;
+        memcpy(cfg_.pow_difficulty, s.data() + p, 32);
+        p += 64;   // and the zero challenge
+        if (!get(s, &p, &opts_.pow_mode) || !get(s, &p, &key_len) || p + key_len > s.size()) return false;
+        key_.assign(s.begin() + (long)p, s.begin() + (long)(p + key_len));
+        p += key_len;
+        if (!get(s, &p, &windows_)) return false;
+        if (cfg_.k2 == 0 || opts_.nonces == 0 || opts_.nonces % 16 || windows_ == 0 || windows_ > 4096 / std::min(opts_.nonces, 4096u) ||
+            opts_.nonces > 4096)
+            return false;
+        opts_.windows_per_pass = windows_;
+        opts_.pow_cache_key = key_.empty() ? nullptr : key_.data();
+        opts_.pow_cache_key_len = key_.size();
+        rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{range_.lo, range_.hi}}, 0, opts_.nonces, windows_, cfg_.k2);
+    }
+    return decode(s, range_.hi);
+}
+
+int InitialProofScan::begin(const InitialProofRequest *req, const RangeSpec *range, const std::string &dir,
+                            const b200post_post_metadata &md, const b200post_post_config &cfg, int64_t provider_id, uint64_t *written,
+                            uint64_t batch, const volatile int *cancel) {
+    dir_ = dir; md_ = md; cfg_ = cfg;
     num_labels_ = (uint64_t)md.num_units * md.labels_per_unit;
+    record_ = range != nullptr;
+    proof_ = req != nullptr;
+    range_ = record_ ? *range : RangeSpec{0, 0, 0, num_labels_};
+    if (proof_) {
+        opts_ = req->opts; key_ = req->cache_key;
+        windows_ = std::max(opts_.windows_per_pass, 1u);
+        opts_.pow_cache_key = key_.empty() ? nullptr : key_.data();
+        opts_.pow_cache_key_len = key_.size();
+    }
     // the session's devices: the proving scan runs on the first, a BUILTIN k2pow search on all of them
     std::vector<uint32_t> devs;
     if (provider_id == B200POST_PROVIDER_ALL) for (int i = 0; i < device_count(); i++) devs.push_back((uint32_t)i);
@@ -130,23 +215,29 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
     scan_dev_ = devs[0];
     if (!engine_for(scan_dev_)) return B200POST_ERR_NO_DEVICE;
 
-    rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{0, num_labels_}}, 0, opts_.nonces, windows_, cfg.k2);
+    if (proof_) rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{range_.lo, range_.hi}}, 0, opts_.nonces, windows_, cfg.k2);
     int rc;
-    if (!load_state(written)) {
-        if ((rc = find_pows(opts_, kZeroChallenge, md.node_id, md.num_units, cfg.pow_difficulty, devs.data(), (int)devs.size(), 0,
-                            nonces() / 16, &pows_, cancel)))
-            return rc;
-        // the RandomX dataset and batch (~14 GiB per device) would otherwise stay resident and shrink every label layer
-        if (opts_.pow_mode == B200POST_POW_BUILTIN) for (uint32_t d : devs) randomx_release((int)d);
+    if (!load_state(*written)) {
+        // a record restarts at lo with nothing in it; the whole POST's scan restarts at 0 and rescans what is on disk
+        vrf_ = b200post_vrf_nonce{}; upto_ = range_.lo;
+        if (proof_) {
+            if ((rc = find_pows(opts_, kZeroChallenge, md.node_id, md.num_units, cfg.pow_difficulty, devs.data(), (int)devs.size(), 0,
+                                nonces() / 16, &pows_, cancel)))
+                return rc;
+            // the RandomX dataset and batch (~14 GiB per device) would otherwise stay resident and shrink every label layer
+            if (opts_.pow_mode == B200POST_POW_BUILTIN) for (uint32_t d : devs) randomx_release((int)d);
+        }
         if ((rc = save_state())) return rc;   // a resumed session never searches again
     }
+    if (record_) *written = upto();   // a record speaks of computed labels only: nothing is read back
+    if (!proof_) return B200POST_OK;
     const uint64_t chunk = std::min<uint64_t>({std::max<uint64_t>(batch, 1), kMaxScanChunk, num_labels_});
     if ((rc = sc_.init(scan_dev_, kZeroChallenge, nonces(), pows_.data(), cfg.k1, cfg.k2, num_labels_, chunk))) return rc;
     // the gap between the state's prefix and what is on disk, in index order, from the files
     PostDataReader reader(dir, md.max_file_size / 16);
-    for (uint64_t pos = book().scanned(); pos < written;) {
+    for (uint64_t pos = upto(); pos < *written;) {
         if (cancel && *cancel) { stop(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
-        const uint64_t n = std::min<uint64_t>(chunk, written - pos);
+        const uint64_t n = std::min<uint64_t>(chunk, *written - pos);
         if ((rc = collect(b_)) || (rc = reader.read(pos, n, sc_.staging(b_))) || (rc = submit(b_, pos, n))) { stop(); return rc; }
         b_ ^= 1;
         pos += n;
@@ -156,13 +247,14 @@ int InitialProofScan::begin(const InitialProofRequest &req, const std::string &d
 
 int InitialProofScan::buffer(uint64_t count, uint8_t **dst) {
     *dst = nullptr;
-    if (count > sc_.chunk()) return B200POST_OK;
+    if (!proof_ || count > sc_.chunk()) return B200POST_OK;
     const int rc = collect(b_);   // the chunk that last used this staging buffer
     if (rc == B200POST_OK) *dst = sc_.staging(b_);
     return rc;
 }
 
 int InitialProofScan::scan(uint64_t first, uint64_t count, const uint8_t *src) {
+    if (!proof_) { upto_ = first + count; return B200POST_OK; }
     if (src == sc_.staging(b_)) {
         const int rc = submit(b_, first, count);
         b_ ^= 1;
@@ -187,7 +279,7 @@ int InitialProofScan::submit_from(const uint8_t *src, uint64_t first, uint64_t c
 
 int InitialProofScan::checkpoint() {
     int rc;
-    for (int k = 0; k < 2; k++) if ((rc = collect(b_ ^ k))) return rc;   // older chunk first
+    for (int k = 0; k < 2 && proof_; k++) if ((rc = collect(b_ ^ k))) return rc;   // older chunk first
     return save_state();
 }
 
@@ -208,8 +300,8 @@ int InitialProofScan::submit(int b, uint64_t first, uint64_t count) {
 
 void InitialProofScan::stop() {
     const std::string err = last_error();
-    for (int k = 0; k < 2 && !failed_; k++) collect(b_ ^ k);   // older chunk first; stops at a failure
-    sc_.drain();
+    for (int k = 0; k < 2 && proof_ && !failed_; k++) collect(b_ ^ k);   // older chunk first; stops at a failure
+    if (proof_) sc_.drain();
     save_state();   // upto = the end of the folded prefix, whose hits are all in the book
     set_error(err);   // the session reports its own failure, not the state's
 }

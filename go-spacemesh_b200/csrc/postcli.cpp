@@ -17,14 +17,21 @@
 //   b200postcli -printNumFiles -numUnits N -labelsPerUnit L [-maxFileSize S]   how many files the POST has
 //   b200postcli -searchForNonce -datadir D [-provider 0|all] [-computeBatchSize B]
 // The last one finds the VRF nonce of the merged files from their stored labels and writes it to the metadata.
+// Ranges with records spare that read, and the initial proof's too:
+//   b200postcli <init flags> -fromFile A -toFile B -rangeRecord [-initialProof [-nonces] [-nonceWindows] [-k1] [-k2] [-powDifficulty]]
+//   b200postcli -mergeRanges -datadir D [-provider 0|all] [-computeBatchSize B] [-k1 -k2 -powDifficulty]
+// Each range session keeps range_A_B.rec (its VRF candidate and, with -initialProof, its proving scan); -mergeRanges
+// on the directory holding every range's files, records and one metadata file writes the nonce and initial_post.json.
 //
 // The initial proof (the proof for the zero challenge a node asks for right after initialisation) from the labels as
 // the session computes them, so that the node's post-service need not read the whole POST back:
 //   b200postcli <init flags> -initialProof [-nonces 288] [-nonceWindows 1] [-k1 26] [-k2 37] [-powDifficulty <64 hex digits>]
-// writes initial_post.json into the data dir (k2pow on the session's devices).  Not with -fromFile / -toFile.
+// writes initial_post.json into the data dir (k2pow on the session's devices).  With -fromFile / -toFile only together
+// with -rangeRecord.
 // -nonceWindows W scans the nonces [0, W x nonces) in the same pass: the proof comes from the lowest window of -nonces
 // nonces that has one, as a prover trying W windows would find it.
-// Exit codes: 0 ok, 1 error or damaged data, 2 usage, 130 stopped.
+// Exit codes: 0 ok (-mergeRanges: the nonce is settled, with or without the initial proof), 1 error or damaged data,
+// 2 usage, 130 stopped.
 #include <signal.h>
 
 #include <chrono>
@@ -103,6 +110,27 @@ static int run_verify(const std::string &datadir, const std::string &provider, d
     return 1;
 }
 
+static int run_merge(const std::string &datadir, const std::string &provider, uint64_t batch, const b200post_post_config &cfg_in) {
+    b200post_merge_opts o{};
+    o.provider_id = provider == "all" ? B200POST_PROVIDER_ALL : (int64_t)strtoull(provider.c_str(), nullptr, 10);
+    if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) { fprintf(stderr, "provider 4294967295 (CPU) is not served: this build has no CPU path\n"); return 2; }
+    o.compute_batch_size = batch;
+    b200post_post_config cfg = cfg_in;
+    b200post_post_metadata md;
+    if (b200post_load_metadata(datadir.c_str(), &md) == 0) cfg.labels_per_unit = md.labels_per_unit;   // the POST's own
+    signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
+    b200post_merge_result r;
+    const int rc = b200post_merge_range_records(datadir.c_str(), &cfg, &o, &r, &g_cancel);
+    if (rc == B200POST_ERR_CANCELLED) { fprintf(stderr, "stopped; run again to finish the past-the-end search\n"); return 130; }
+    if (rc) { fprintf(stderr, "merge failed: %s (%d)\n", b200post_last_error(), rc); return 1; }
+    printf("merged %u range records; VRF nonce %llu%s\n", r.ranges, (unsigned long long)r.nonce.index,
+           r.past_end ? " (past the end of the POST)" : "");
+    const std::string where = datadir + (datadir.empty() || datadir.back() == '/' ? "" : "/") + "initial_post.json";
+    if (r.proof_rc == 0) printf("initial proof: nonce %u, written to %s\n", r.proof.nonce, where.c_str());
+    else printf("no initial proof: %s; the post-service proves from the stored data instead\n", r.proof_reason);
+    return 0;
+}
+
 static int run_search(const std::string &datadir, const std::string &provider, uint64_t batch) {
     b200post_vrf_search_opts o;
     b200post_default_vrf_search_opts(&o);
@@ -141,6 +169,7 @@ int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
     bool print_providers = false, verify = false, print_num_files = false, search = false, range = false, initial = false;
+    bool range_record = false, merge = false;
     uint32_t nonces = 288, windows = 1, k1 = 0, k2 = 0;
     std::string pow_difficulty;
     double fraction = 0.2;
@@ -171,6 +200,8 @@ int main(int argc, char **argv) {
         else if (a == "searchForNonce") search = true;
         else if (a == "seed") seed = strtoull(val().c_str(), nullptr, 10);
         else if (a == "initialProof") initial = true;
+        else if (a == "rangeRecord") range_record = true;
+        else if (a == "mergeRanges") merge = true;
         else if (a == "nonces") nonces = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "nonceWindows") windows = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "k1") k1 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
@@ -193,17 +224,22 @@ int main(int argc, char **argv) {
     }
     if (verify) return run_verify(datadir, provider, fraction, from_file, to_file, seed);
     if (search) return run_search(datadir, provider, batch);
-    uint8_t node_id[32], atx_id[32];
-    if (!unhex32(id, node_id) || !unhex32(atx, atx_id)) { fprintf(stderr, "-id and -commitmentAtxId must be 32-byte hex strings\n"); return 2; }
     b200post_post_config cfg;
     b200post_default_post_config(&cfg);
     if (labels_per_unit) cfg.labels_per_unit = labels_per_unit;
     cfg.min_num_units = 1; cfg.max_num_units = 1u << 20;
-    if (windows == 0) { fprintf(stderr, "-nonceWindows must be at least 1\n"); return 2; }
-    if (initial && range) { fprintf(stderr, "-initialProof needs the whole POST: it cannot be combined with -fromFile / -toFile\n"); return 2; }
     if (k1) cfg.k1 = k1;
     if (k2) cfg.k2 = cfg.k3 = k2;
     if (!pow_difficulty.empty() && !unhex32(pow_difficulty, cfg.pow_difficulty)) { fprintf(stderr, "-powDifficulty must be a 32-byte hex string\n"); return 2; }
+    if (merge) return run_merge(datadir, provider, batch, cfg);
+    uint8_t node_id[32], atx_id[32];
+    if (!unhex32(id, node_id) || !unhex32(atx, atx_id)) { fprintf(stderr, "-id and -commitmentAtxId must be 32-byte hex strings\n"); return 2; }
+    if (windows == 0) { fprintf(stderr, "-nonceWindows must be at least 1\n"); return 2; }
+    if (initial && range && !range_record) {
+        fprintf(stderr, "-initialProof needs the whole POST: with -fromFile / -toFile, add -rangeRecord and merge the ranges with -mergeRanges\n");
+        return 2;
+    }
+    if (range_record && !range) { fprintf(stderr, "-rangeRecord needs a file range (-fromFile / -toFile)\n"); return 2; }
     b200post_setup_opts o;
     b200post_default_setup_opts(&o);
     o.data_dir = datadir.c_str(); o.num_units = (uint32_t)num_units; o.scrypt_n = scrypt_n; o.max_file_size = max_file_size;
@@ -218,12 +254,13 @@ int main(int argc, char **argv) {
         fprintf(stderr, "prepare: %s (%d)\n", b200post_last_error(), rc);
         return range && rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;   // a file range outside the POST is a usage error
     }
-    if (initial) {
+    if (initial || range_record) {
         b200post_prove_opts po{};
         po.nonces = nonces; po.pow_mode = B200POST_POW_BUILTIN; po.windows_per_pass = windows;
-        if (int rc = b200post_setup_request_initial_proof(mgr, &po)) {
-            fprintf(stderr, "initial proof: %s (%d)\n", b200post_last_error(), rc);
-            return rc == B200POST_ERR_INVALID_ARGUMENT ? 2 : 1;
+        const int rc = range_record ? b200post_setup_request_range_record(mgr, initial ? &po : nullptr) : b200post_setup_request_initial_proof(mgr, &po);
+        if (rc) {
+            fprintf(stderr, "%s: %s (%d)\n", range_record ? "range record" : "initial proof", b200post_last_error(), rc);
+            return rc == B200POST_ERR_INVALID_ARGUMENT || rc == B200POST_ERR_STATE ? 2 : 1;
         }
     }
     signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
@@ -249,12 +286,16 @@ int main(int argc, char **argv) {
     if (rc) { fprintf(stderr, "init failed: %s (%d)\n", b200post_last_error(), rc); return 1; }
     b200post_post_metadata md;
     if (b200post_load_metadata(datadir.c_str(), &md) == 0) {
-        if (md.vrf_scan_pending)
+        if (md.vrf_scan_pending && range_record)
+            printf("files %llu..%llu complete with their range record; copy every range's files and record and one metadata file into one "
+                   "directory, then merge them with -mergeRanges\n", (unsigned long long)from_file,
+                   (unsigned long long)(from_file + (total + per_file - 1) / per_file - 1));
+        else if (md.vrf_scan_pending)
             printf("files %llu..%llu complete; copy every range's files and one metadata file into one directory, then search the VRF nonce "
                    "with -searchForNonce\n", (unsigned long long)from_file, (unsigned long long)(from_file + (total + per_file - 1) / per_file - 1));
         else if (md.has_nonce) printf("initialization complete; VRF nonce %llu\n", (unsigned long long)md.nonce);
     }
-    if (initial) {
+    if (initial && !range_record) {
         b200post_proof_out proof;
         const int prc = b200post_setup_initial_proof(mgr, &proof, nullptr);
         const std::string where = datadir + (datadir.empty() || datadir.back() == '/' ? "" : "/") + "initial_post.json";

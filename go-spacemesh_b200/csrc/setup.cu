@@ -251,6 +251,11 @@ int load_initial_proof(const std::string &dir, const b200post_post_metadata &md,
 namespace b200post {
 
 int save_post_metadata(const std::string &dir, const b200post_post_metadata &m) { return save_metadata(dir, m); }
+int load_post_metadata(const std::string &dir, b200post_post_metadata *m) { return load_metadata(dir, m, nullptr); }
+int save_initial_proof_file(const std::string &dir, const b200post_proof_metadata &pm, const b200post_post_config &cfg, uint32_t nonces,
+                            uint32_t windows, const b200post_proof_out &p) {
+    return save_initial_proof(dir, pm, cfg, nonces, windows, p);
+}
 
 int compute_labels(int64_t provider_id, uint64_t N, const uint8_t commitment[32], uint64_t start, uint64_t count, uint8_t *out,
                    const uint8_t *diff, b200post_vrf_nonce *nonce, const volatile int *cancel) {
@@ -296,7 +301,11 @@ struct b200post_setup_manager {
     std::atomic<uint64_t> labels_written{0};   // of the session's label range
     uint64_t num_labels = 0;
     uint64_t range_lo = 0, range_hi = 0;        // the session writes labels [range_lo, range_hi)
+    uint64_t range_from = 0, range_to = 0;      // of files [range_from, range_to]
     bool range() const { return range_lo != 0 || range_hi != num_labels; }
+    // a file range's record (b200post_setup_request_range_record): asked for between prepare and start, kept by start
+    bool want_record = false, record_proof = false;
+    InitialProofRequest record_req;
     // the initial proof: asked for between prepare and start (b200post_setup_request_initial_proof), produced by start
     bool want_proof = false;
     InitialProofRequest proof_req;
@@ -359,7 +368,7 @@ int b200post_setup_prepare_files(b200post_setup_manager *m, const b200post_setup
         return B200POST_ERR_STATE;
     }
     // a request belongs to one prepared session, and so does its outcome
-    m->want_proof = m->proof_done = false;
+    m->want_proof = m->proof_done = m->want_record = false;
     m->proof_rc = B200POST_OK; m->proof_err.clear();
     m->proof = b200post_proof_out{}; m->proof_meta = b200post_proof_metadata{};
     // ---- option validation (initialization.NewInitializer / config.Validate upstream; errors -> state Error, post.go:362-365)
@@ -431,6 +440,7 @@ int b200post_setup_prepare_files(b200post_setup_manager *m, const b200post_setup
     memcpy(m->node_id, node_id, 32);
     m->meta = meta; m->num_labels = num_labels; m->have_opts = true;
     m->range_lo = lo; m->range_hi = hi;
+    m->range_from = from_file; m->range_to = last_file;
     m->labels_written.store(written);
     if ((rc = save_metadata(dir, m->meta))) { m->state = B200POST_SETUP_ERROR; return rc; }
     m->state = B200POST_SETUP_PREPARED;
@@ -449,7 +459,9 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
 
     const uint64_t num_labels = m->num_labels, per_file = m->opts.max_file_size / 16, batch = m->opts.compute_batch_size;
     const uint64_t lo = m->range_lo, hi = m->range_hi;
-    const bool range = m->range();   // no VRF scan, no nonce, no past-the-end search: a range's arg-min is not the POST's
+    const bool range = m->range();   // no nonce, no past-the-end search: a range's arg-min is not the POST's
+    // a range with a record scans its labels for the VRF into the record, not into the metadata
+    const bool record = range && m->want_record;
     uint64_t written = lo + m->labels_written.load();   // the next label to write
     const bool need_work = written < hi || (!range && (!m->meta.has_nonce || m->meta.vrf_scan_pending));
     if (need_work && m->opts.provider_id == B200POST_PROVIDER_UNSET) {
@@ -459,20 +471,27 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     uint8_t commitment[32];
     commitment_bytes(m->meta.node_id, m->meta.commitment_atx_id, commitment);
     uint8_t diff[32];
-    if (m->meta.has_nonce) memcpy(diff, m->meta.nonce_value, 32); else vrf_difficulty(num_labels, diff);
+    if (m->meta.has_nonce) memcpy(diff, m->meta.nonce_value, 32); else vrf_difficulty(num_labels, diff);   // numLabels of the whole POST
 
-    // the initial proof: pows, state and the rescan of what is already on disk come before the first batch
+    // the initial proof: pows, state and the rescan of what is already on disk come before the first batch.  A record:
+    // pows and record, and the session resumes at the record's prefix (labels past it are computed again).
     std::unique_ptr<InitialProofScan> ip;
-    if (m->want_proof) {
+    if (m->want_proof || record) {
         m->proof_done = false;
         if (m->opts.provider_id == B200POST_PROVIDER_UNSET) {
             set_error("no provider specified");
             return finish(B200POST_SETUP_ERROR, B200POST_ERR_NO_PROVIDER);
         }
         ip.reset(new InitialProofScan);
-        const int rc = ip->begin(m->proof_req, m->data_dir, m->meta, m->cfg, m->opts.provider_id, written, batch, cancel);
+        const RangeSpec rs{m->range_from, m->range_to, lo, hi};
+        const InitialProofRequest *req = record ? (m->record_proof ? &m->record_req : nullptr) : &m->proof_req;
+        const int rc = ip->begin(req, record ? &rs : nullptr, m->data_dir, m->meta, m->cfg, m->opts.provider_id, &written, batch, cancel);
         if (rc == B200POST_ERR_CANCELLED) return finish(B200POST_SETUP_STOPPED, rc);
         if (rc) return finish(B200POST_SETUP_ERROR, rc);
+        if (record) {
+            m->labels_written.store(written - lo);   // the status counts from the resume point
+            if (ip->vrf().found) memcpy(diff, ip->vrf().label32, 32);
+        }
     }
     // from here on a stop or failure first saves the initial proof's scan state
     auto end = [&](int32_t state, int rc) { if (ip) ip->stop(); return finish(state, rc); };
@@ -496,7 +515,7 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         if (ip && (rc = ip->buffer(count, &labels))) return end(B200POST_SETUP_ERROR, rc);
         if (!labels) { buf.resize((size_t)count * 16); labels = buf.data(); }
         b200post_vrf_nonce nn;
-        rc = compute_labels(m->opts.provider_id, m->opts.scrypt_n, commitment, written, count, labels, range ? nullptr : diff,
+        rc = compute_labels(m->opts.provider_id, m->opts.scrypt_n, commitment, written, count, labels, range && !record ? nullptr : diff,
                             &nn, cancel);
         if (rc == B200POST_ERR_CANCELLED) return end(B200POST_SETUP_STOPPED, rc);
         if (rc) return end(B200POST_SETUP_ERROR, rc);
@@ -519,6 +538,8 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
             }
         }
         n_batches++;
+        // a record's VRF best covers every batch that its scan folds: it is noted before the batch goes to the scan
+        if (record && nn.found) { ip->note_vrf(nn); memcpy(diff, nn.label32, 32); }
         const std::string path = data_file(m->data_dir, file_idx);
         const int fd = open(path.c_str(), O_WRONLY | O_CREAT, 0644);
         if (fd < 0) return end(B200POST_SETUP_ERROR, io_error("open " + path));
@@ -534,7 +555,7 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         if (ip && (rc = ip->scan(written, count, labels))) return end(B200POST_SETUP_ERROR, rc);
         written += count;
         m->labels_written.store(written - lo);
-        if ((rc = note_nonce(nn))) return end(B200POST_SETUP_ERROR, rc);
+        if (!record && (rc = note_nonce(nn))) return end(B200POST_SETUP_ERROR, rc);
         if (ip && (written % per_file == 0 || written == hi) && (rc = ip->checkpoint())) return end(B200POST_SETUP_ERROR, rc);
     }
     if (!range) {
@@ -556,7 +577,7 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     }
     int rc = save_metadata(m->data_dir, m->meta);
     if (rc) return end(B200POST_SETUP_ERROR, rc);
-    if (ip) {
+    if (ip && !record) {
         // every label is on disk and the VRF nonce is settled: decide, gate, publish.  No proof is not a failed session.
         b200post_proof_out proof{};
         b200post_proof_metadata pm{};
@@ -591,7 +612,10 @@ int b200post_setup_reset(b200post_setup_manager *m) {
             const std::string name = e->d_name;
             const bool data = name.rfind("postdata_", 0) == 0 && name.size() > 13 && name.substr(name.size() - 4) == ".bin";
             const bool initial = name.rfind(kInitialProofFile, 0) == 0 || name.rfind(kInitialScanFile, 0) == 0;   // and their .tmp
-            if (data || name == kMetaFile || initial) {
+            const bool record = name.rfind(kRangeRecordPrefix, 0) == 0 &&
+                                ((name.size() > 4 && name.substr(name.size() - 4) == ".rec") ||
+                                 (name.size() > 8 && name.substr(name.size() - 8) == ".rec.tmp"));   // range_<from>_<to>.rec[.tmp]
+            if (data || name == kMetaFile || initial || record) {
                 if (unlink(path_join(m->data_dir, name).c_str()) != 0) { closedir(d); return io_error("unlink " + name); }
             }
         }
@@ -599,7 +623,7 @@ int b200post_setup_reset(b200post_setup_manager *m) {
     }
     m->labels_written.store(0);
     memset(&m->meta, 0, sizeof m->meta);
-    m->want_proof = m->proof_done = false;
+    m->want_proof = m->proof_done = m->want_record = false;
     m->state = B200POST_SETUP_NOT_STARTED;
     return B200POST_OK;
 }
@@ -617,11 +641,12 @@ int b200post_load_metadata(const char *data_dir, b200post_post_metadata *out) {
     return load_metadata(data_dir, out, nullptr);
 }
 
-int b200post_setup_request_initial_proof(b200post_setup_manager *m, const b200post_prove_opts *opts) {
-    if (!m || !opts) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    std::lock_guard<std::mutex> lk(m->mu);
-    if (m->state != B200POST_SETUP_PREPARED) { set_error("post session not prepared"); return B200POST_ERR_STATE; }
-    if (m->range()) { set_error("initial proof: a file-range session does not see the whole POST"); return B200POST_ERR_STATE; }
+}  // extern "C"
+
+namespace {
+
+// the fields of an initial-proof request that the session's scan uses, checked and copied into *req
+int take_proof_request(const b200post_prove_opts *opts, InitialProofRequest *req) {
     b200post_prove_opts o = *opts;
     if (o.nonces == 0) o.nonces = 16;
     if (o.nonces % 16 || o.nonces > 4096) { set_error("invalid nonce count (a positive multiple of 16, <= 4096)"); return B200POST_ERR_INVALID_ARGUMENT; }
@@ -630,10 +655,39 @@ int b200post_setup_request_initial_proof(b200post_setup_manager *m, const b200po
     o.max_windows = 0;
     const int rc = check_pow_mode(o);
     if (rc) return rc;
-    m->proof_req.cache_key.assign(o.pow_cache_key, o.pow_cache_key ? o.pow_cache_key + o.pow_cache_key_len : o.pow_cache_key);
+    req->cache_key.assign(o.pow_cache_key, o.pow_cache_key ? o.pow_cache_key + o.pow_cache_key_len : o.pow_cache_key);
     o.pow_cache_key = nullptr; o.pow_cache_key_len = 0;   // the copy above is the key
-    m->proof_req.opts = o;
+    req->opts = o;
+    return B200POST_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int b200post_setup_request_initial_proof(b200post_setup_manager *m, const b200post_prove_opts *opts) {
+    if (!m || !opts) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->state != B200POST_SETUP_PREPARED) { set_error("post session not prepared"); return B200POST_ERR_STATE; }
+    if (m->range()) { set_error("initial proof: a file-range session does not see the whole POST"); return B200POST_ERR_STATE; }
+    const int rc = take_proof_request(opts, &m->proof_req);
+    if (rc) return rc;
     m->want_proof = true;
+    return B200POST_OK;
+}
+
+int b200post_setup_request_range_record(b200post_setup_manager *m, const b200post_prove_opts *proof) {
+    if (!m) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->state != B200POST_SETUP_PREPARED) { set_error("post session not prepared"); return B200POST_ERR_STATE; }
+    if (!m->range()) { set_error("range record: the session covers the whole POST (it finds the nonce and proof itself)"); return B200POST_ERR_STATE; }
+    if (m->meta.has_nonce) { set_error("range record: the metadata already holds the VRF nonce"); return B200POST_ERR_STATE; }
+    if (proof) {
+        const int rc = take_proof_request(proof, &m->record_req);
+        if (rc) return rc;
+    }
+    m->want_record = true;
+    m->record_proof = proof != nullptr;
     return B200POST_OK;
 }
 

@@ -227,20 +227,9 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     if (chunk > kMaxChunk) return fail(B200POST_ERR_INVALID_ARGUMENT, "chunk_labels above 2^26");
 
     // ---- metadata and files, on the host before any device is touched
-    const unsigned __int128 nl = (unsigned __int128)md->num_units * md->labels_per_unit;
+    if (int rc = check_post_files(dir, *md)) return rc;
     const uint64_t N = md->scrypt_n;
-    if (nl == 0 || nl > (~0ull >> 4) || md->max_file_size < 16 || md->max_file_size % 16 || N < 2 || N > (1ull << 20) || (N & (N - 1)))
-        return fail(B200POST_ERR_IO, "corrupt metadata: label count, MaxFileSize or Scrypt.N out of range");
-    const uint64_t num_labels = (uint64_t)nl, per_file = md->max_file_size / 16, n_files = (num_labels + per_file - 1) / per_file;
-    for (uint64_t f = 0; f < n_files; f++) {
-        struct stat st;
-        const std::string p = postdata_path(dir, f);
-        const uint64_t want = std::min<uint64_t>(per_file, num_labels - f * per_file) * 16;
-        if (stat(p.c_str(), &st) != 0) return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " is missing");
-        if ((uint64_t)st.st_size != want)
-            return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " holds " + std::to_string(st.st_size) + " bytes, the metadata implies " +
-                                             std::to_string(want));
-    }
+    const uint64_t num_labels = (uint64_t)md->num_units * md->labels_per_unit, per_file = md->max_file_size / 16;
 
     // ---- device: the scan runs on one (it is bound by storage, not by the GPU)
     if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) return fail(B200POST_ERR_UNSUPPORTED, "provider 0xffffffff (CPU): this library has no CPU path");
@@ -306,17 +295,44 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     if (best.n_ties > pos.size())
         return fail(B200POST_ERR_LABEL_MISMATCH, std::to_string(best.n_ties) + " stored labels share the smallest 16-byte prefix: the POST data is damaged");
 
-    // ---- the rule of an init: below the threshold, or the past-the-end search
-    uint8_t diff[32];
+    return settle_nonce(dir, md, best_index, best32, o.provider_id, batch, out, nullptr, cancel);
+}
+
+int check_post_files(const std::string &dir, const b200post_post_metadata &md) {
+    const unsigned __int128 nl = (unsigned __int128)md.num_units * md.labels_per_unit;
+    const uint64_t N = md.scrypt_n;
+    if (nl == 0 || nl > (~0ull >> 4) || md.max_file_size < 16 || md.max_file_size % 16 || N < 2 || N > (1ull << 20) || (N & (N - 1)))
+        return fail(B200POST_ERR_IO, "corrupt metadata: label count, MaxFileSize or Scrypt.N out of range");
+    const uint64_t num_labels = (uint64_t)nl, per_file = md.max_file_size / 16, n_files = (num_labels + per_file - 1) / per_file;
+    for (uint64_t f = 0; f < n_files; f++) {
+        struct stat st;
+        const std::string p = postdata_path(dir, f);
+        const uint64_t want = std::min<uint64_t>(per_file, num_labels - f * per_file) * 16;
+        if (stat(p.c_str(), &st) != 0) return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " is missing");
+        if ((uint64_t)st.st_size != want)
+            return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " holds " + std::to_string(st.st_size) + " bytes, the metadata implies " +
+                                             std::to_string(want));
+    }
+    return B200POST_OK;
+}
+
+// The rule of an init: below the threshold, or the past-the-end search.
+int settle_nonce(const std::string &dir, b200post_post_metadata *md, uint64_t best_index, const uint8_t best32[32], int64_t provider_id,
+                 uint64_t batch, b200post_vrf_nonce *out, bool *past_end, const volatile int *cancel) {
+    const uint64_t num_labels = (uint64_t)md->num_units * md->labels_per_unit;
+    uint8_t diff[32], commitment[32];
     vrf_difficulty(num_labels, diff);
-    if (memcmp(best32, diff, 32) < 0) {
+    commitment_bytes(md->node_id, md->commitment_atx_id, commitment);
+    const bool below = memcmp(best32, diff, 32) < 0;
+    if (past_end) *past_end = !below;
+    if (below) {
         md->has_nonce = 1; md->nonce = best_index; memcpy(md->nonce_value, best32, 32); md->last_position = 0;
     } else {
         // a recorded nonce is replaced, so the search starts at numLabels; without one it resumes a stopped search.
         // The marker stays set until the search ends, so a stopped search is finished by the next search or session.
         if (md->has_nonce) md->last_position = 0;
         md->has_nonce = 0; md->vrf_scan_pending = 1;
-        if (int rc = search_past_end(dir, md, num_labels, o.provider_id, batch, commitment, diff, cancel)) return rc;
+        if (int rc = search_past_end(dir, md, num_labels, provider_id, batch, commitment, diff, cancel)) return rc;
     }
     md->vrf_scan_pending = 0;
     if (int rc = save_post_metadata(dir, *md)) return rc;

@@ -529,6 +529,74 @@ func (m *SetupManager) InitialProof() (*Proof, error) {
 	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, nil
 }
 
+// RequestRangeRecord asks the prepared file-range session (PrepareFiles, metadata without a nonce) to keep
+// range_<from>_<to>.rec in the data dir: the range's VRF candidate and, when nonces > 0, the initial-proof scan of its
+// labels (builtin k2pow on the session's devices, w.PerPass nonce windows).  Call it between PrepareFiles and
+// StartSession; MergeRangeRecords turns the records of every range into the POST's nonce and initial proof.
+func (m *SetupManager) RequestRangeRecord(nonces uint32, w NonceWindows) error {
+	if nonces == 0 {
+		return setupErr(checked(func() C.int { return C.b200post_setup_request_range_record(m.h, nil) }))
+	}
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), pow_mode: C.B200POST_POW_BUILTIN, windows_per_pass: C.uint32_t(w.PerPass)}
+	return setupErr(checked(func() C.int { return C.b200post_setup_request_range_record(m.h, &o) }))
+}
+
+// MergeResult is what MergeRangeRecords settled: the records merged, the VRF nonce now in the metadata, whether the
+// past-the-end search found it, and the initial proof written to initial_post.json (nil, with ProofErr saying why,
+// when the records hold no common proof scan, no nonce reached K2 or the verifier refused it).
+type MergeResult struct {
+	Ranges     uint32
+	Nonce      uint64
+	NonceValue [32]byte
+	PastEnd    bool
+	Proof      *Proof
+	ProofErr   error
+}
+
+// MergeRangeRecords writes the VRF nonce and initial proof of the POST in dataDir from its range records, without
+// reading a stored label, exactly as one full session with the initial proof would have written them.  cfg gives
+// LabelsPerUnit, K1, K2 and the pow difficulty; batch is the past-the-end batch (0 = 2^20).  Records that do not tile
+// the POST, damaged or foreign records and incomplete data are errors that leave the metadata untouched.
+func MergeRangeRecords(ctx context.Context, dataDir string, cfg SetupConfig, providerID uint32, batch uint64) (*MergeResult, error) {
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	var o C.b200post_merge_opts
+	if providerID == AllProviders {
+		o.provider_id = C.B200POST_PROVIDER_ALL
+	} else {
+		o.provider_id = C.int64_t(providerID)
+	}
+	o.compute_batch_size = C.uint64_t(batch)
+	var cancel int32
+	done := make(chan struct{})
+	defer close(done)
+	go func() {
+		select {
+		case <-ctx.Done():
+			atomic.StoreInt32(&cancel, 1)
+		case <-done:
+		}
+	}()
+	var out C.b200post_merge_result
+	if err := setupErr(checked(func() C.int {
+		return C.b200post_merge_range_records(dir, &c, &o, &out, (*C.int)(unsafe.Pointer(&cancel)))
+	})); err != nil {
+		return nil, err
+	}
+	r := &MergeResult{Ranges: uint32(out.ranges), Nonce: uint64(out.nonce.index), PastEnd: out.past_end != 0}
+	C.memcpy(unsafe.Pointer(&r.NonceValue[0]), unsafe.Pointer(&out.nonce.label32[0]), 32)
+	if out.proof_rc == C.B200POST_OK {
+		r.Proof = &Proof{Nonce: uint32(out.proof.nonce), Pow: uint64(out.proof.pow),
+			Indices: C.GoBytes(unsafe.Pointer(&out.proof.indices[0]), C.int(out.proof.indices_len))}
+	} else {
+		r.ProofErr = statusErr(C.int(out.proof_rc), C.GoString(&out.proof_reason[0]))
+	}
+	return r, nil
+}
+
 // LoadInitialProof is the post-service's answer to the ZeroChallenge without a scan: the proof a setup session stored
 // in dataDir, if it was made for this POST's metadata, cfg and nonce count.  An absent or stale proof is an error
 // ("no initial proof"); fall back to GenerateProofChecked.

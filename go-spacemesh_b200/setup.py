@@ -7,6 +7,7 @@ states NotStarted(1) .. Error(6).  The state machine itself lives in C++ (csrc/s
 from __future__ import annotations
 
 import ctypes
+import functools
 from dataclasses import dataclass
 
 from . import B200PostError, ERR_CANCELLED, OK, VrfNonce, lib
@@ -53,6 +54,29 @@ class _VerifyPosResult(ctypes.Structure):
 class _VrfSearchOpts(ctypes.Structure):
     _fields_ = [("provider_id", ctypes.c_int64), ("compute_batch_size", ctypes.c_uint64), ("chunk_labels", ctypes.c_uint64),
                 ("progress", ctypes.c_void_p)]
+
+
+class _MergeOpts(ctypes.Structure):
+    _fields_ = [("provider_id", ctypes.c_int64), ("compute_batch_size", ctypes.c_uint64)]
+
+
+@functools.lru_cache(maxsize=None)
+def _merge_result_type():
+    from . import prove   # imports this module: the proof struct is bound on first use
+    return type("_MergeResult", (ctypes.Structure,), {"_fields_": [
+        ("ranges", ctypes.c_uint32), ("nonce", VrfNonce), ("past_end", ctypes.c_uint32), ("proof_rc", ctypes.c_int32),
+        ("proof_reason", ctypes.c_char * 256), ("proof", prove._ProofOut)]})
+
+
+@dataclass
+class MergeResult:           # b200post_merge_result
+    ranges: int              # records merged
+    nonce: int               # the VRF nonce the metadata now holds
+    nonce_value: bytes       # its label32
+    past_end: bool           # no label was below the threshold: the past-the-end search found the nonce
+    proof_rc: int            # OK: initial_post.json written; ERR_INVALID_PROOF or ERR_STATE: no initial proof
+    proof_reason: str        # why there is none
+    proof: object = None     # the Proof written to initial_post.json, or None
 
 
 @dataclass
@@ -123,6 +147,8 @@ def _bind():
     L.b200post_setup_request_initial_proof.argtypes = [vp, vp]
     L.b200post_setup_initial_proof.argtypes = [vp, vp, vp]
     L.b200post_load_initial_proof.argtypes = [ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.c_uint32, vp, vp]
+    L.b200post_setup_request_range_record.argtypes = [vp, vp]
+    L.b200post_merge_range_records.argtypes = [ctypes.c_char_p, vp, ctypes.POINTER(_MergeOpts), vp, vp]
     L._setup_bound = True
     return L
 
@@ -183,6 +209,29 @@ def load_initial_proof(data_dir: str, cfg: PostConfig, nonces: int = 16):
     return prove._results(out, meta)
 
 
+def merge_range_records(data_dir: str, cfg: PostConfig, *, provider_id: int = 0, compute_batch_size: int = 0,
+                        cancel: ctypes.c_int | None = None) -> MergeResult:
+    """b200postcli -mergeRanges: the VRF nonce and initial proof of a POST whose files were written by range sessions
+    with records (request_range_record), from the range_*.rec files in data_dir and without reading a stored label.
+    The nonce is written to the metadata and the proof (when every record carries a common proof scan and it yields one)
+    to initial_post.json, as one full session with the initial proof would have written them.  cfg gives K1, K2 and the
+    pow difficulty; compute_batch_size the past-the-end batch (0 = 2^20).  Raises B200PostError when the records do not
+    tile the POST, are damaged or foreign, or the data is incomplete (the metadata is then untouched)."""
+    from . import prove
+    o = _MergeOpts(provider_id, compute_batch_size)
+    r = _merge_result_type()()
+    _err(_bind().b200post_merge_range_records(data_dir.encode(), ctypes.byref(prove._c_cfg(cfg)), ctypes.byref(o), ctypes.byref(r),
+                                              ctypes.addressof(cancel) if cancel is not None else None))
+    proof = prove._results(r.proof, _zero_meta())[0] if r.proof_rc == OK else None
+    return MergeResult(int(r.ranges), int(r.nonce.index), bytes(r.nonce.label32), bool(r.past_end), int(r.proof_rc),
+                       r.proof_reason.decode(errors="replace"), proof)
+
+
+def _zero_meta():
+    from .verify import _Meta
+    return _Meta()
+
+
 def verify_pos_sample(seed: int, file: int, labels_in_file: int, fraction: float):
     """The positions (within the file, ascending, numpy uint64) that verify_pos checks for this seed and file."""
     import numpy as np
@@ -239,6 +288,23 @@ class PostSetupManager:
             opts.pow_cache_key, opts.pow_cache_key_len = pow_cache_key, len(pow_cache_key)
         self._initial_opts = opts   # keeps a pow callback alive for the session
         _err(_bind().b200post_setup_request_initial_proof(self._h, ctypes.byref(opts)))
+
+    def request_range_record(self, *, initial_proof: bool = False, nonces: int = 16, pow="builtin",
+                             pow_cache_key: bytes | None = None, windows_per_pass: int = 1) -> None:
+        """Ask the prepared file-range session (prepare_files, metadata without a nonce) to keep a record of its range in
+        range_<from>_<to>.rec: the range's VRF candidate, and with initial_proof=True also the initial-proof scan of its
+        labels (nonces, pow, pow_cache_key and windows_per_pass as in request_initial_proof).  merge_range_records turns
+        the records of every range into the POST's nonce and initial proof.  Call between prepare_files and start_session."""
+        if not initial_proof:
+            self._initial_opts = None
+            _err(_bind().b200post_setup_request_range_record(self._h, None))
+            return
+        from . import prove
+        opts, _ = prove._opts(None, None, nonces, 0, pow, 1, windows_per_pass)
+        if pow_cache_key is not None:
+            opts.pow_cache_key, opts.pow_cache_key_len = pow_cache_key, len(pow_cache_key)
+        self._initial_opts = opts   # keeps a pow callback alive for the session
+        _err(_bind().b200post_setup_request_range_record(self._h, ctypes.byref(opts)))
 
     def initial_proof(self):
         """After a completed session that asked for it: (Proof, ProofMetadata, labels scanned).  Raises ERR_INVALID_PROOF

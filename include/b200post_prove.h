@@ -144,7 +144,7 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
  * computed from the labels as the session writes them spares that second read of every stored label.
  *
  * b200post_setup_request_initial_proof: between prepare and start of a session over the whole POST (a file-range session:
- * B200POST_ERR_STATE; not prepared: B200POST_ERR_STATE); prepare clears the request, a second call replaces it.  From
+ * B200POST_ERR_STATE, it asks for a range record instead, see below; not prepared: B200POST_ERR_STATE); prepare clears the request, a second call replaces it.  From
  * opts: nonces (0 = 16; else a positive multiple of 16, <= 4096, or INVALID_ARGUMENT), pow_mode with pow_prove/pow_ctx
  * (CALLBACK without a function: UNSUPPORTED), the RandomX cache key (copied) and windows_per_pass, the W nonce windows the
  * session scans in its single pass (0 = 1, clamped to floor(4096 / nonces)); provider, chunk_labels and max_windows are
@@ -167,6 +167,67 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
  * start_session returns B200POST_ERR_NO_DEVICE (no CPU path) and writes no state.
  */
 int b200post_setup_request_initial_proof(b200post_setup_manager *mgr, const b200post_prove_opts *opts);
+/*
+ * One POST initialised on several machines (DESIGN.md §3c, §3e): each file-range session keeps a record of what its
+ * labels contribute, and b200post_merge_range_records turns the records into the POST's VRF nonce and initial proof
+ * without reading a stored label.
+ *
+ * b200post_setup_request_range_record: between b200post_setup_prepare_files and start, for a range short of the whole
+ * POST whose metadata has no nonce (not prepared, a whole-POST session or metadata with a nonce: B200POST_ERR_STATE).
+ * proof == NULL: the record holds the VRF candidate only.  Otherwise also the initial-proof scan, with the fields of
+ * b200post_setup_request_initial_proof (nonces, pow_mode/pow_prove/pow_ctx, the cache key (copied), windows_per_pass)
+ * and its errors (bad nonces: INVALID_ARGUMENT; CALLBACK without a function: UNSUPPORTED).  Prepare clears the request,
+ * a second call replaces it.
+ * The session then computes every batch with the VRF scan on, from the threshold floor(2^256 / numLabels) of the whole
+ * POST, tightened to the best label found so far; the best (found, index, label32) goes into the record, not into the
+ * metadata, which keeps VrfScanPending and no nonce.  With proof, the pows of the zero challenge for all groups of the
+ * W windows are found first (then the RandomX memory is released), and each batch goes through the proving scan as it is
+ * written, over [lo, hi), with no stop rule: each nonce keeps its first K2 hits in the range.
+ * The record is range_<from>_<to>.rec in the data dir (tmp + rename, FNV-1a 64 checksum): a header with everything its
+ * result depends on (identity, NumUnits, LabelsPerUnit, MaxFileSize, scrypt N, the files and labels [lo, hi), and for
+ * the proof K1, K2, nonces, W, pow difficulty, pow mode and cache key), then upto (the end of the covered prefix), the
+ * VRF best, and for the proof the pows and hit lists.  It is saved at every completed postdata file, when the session
+ * stops or fails, and at the end (upto == hi).
+ * Resume: a record that is intact, matches and has upto at or below the labels on disk is used, and the session resumes
+ * at upto, computing [upto, written) again over the same bytes; any other record is ignored and the range is computed
+ * from lo.  A record so speaks only of computed labels, never of stored bytes.  The status counts from the resume point.
+ * b200post_setup_reset deletes range_*.rec and their .tmp files.  Without a request a range session writes no record.
+ */
+int b200post_setup_request_range_record(b200post_setup_manager *mgr, const b200post_prove_opts *proof);
+
+typedef struct b200post_merge_opts {
+    int64_t provider_id;               /* CUDA ordinal or B200POST_PROVIDER_ALL: the past-the-end search and the gate   */
+    uint64_t compute_batch_size;       /* past-the-end batch, 0 = 2^20 (the init's batch gives the init's LastPosition) */
+} b200post_merge_opts;
+
+typedef struct b200post_merge_result {
+    uint32_t ranges;                   /* records merged                                                              */
+    b200post_vrf_nonce nonce;          /* what the metadata now holds                                                 */
+    uint32_t past_end;                 /* 1: no label below the threshold; the past-the-end search found it          */
+    int32_t proof_rc;                  /* OK: initial_post.json written; INVALID_PROOF: no nonce reached K2 or the
+                                          gate refused; STATE: the records hold no common proof scan                  */
+    char proof_reason[256];
+    b200post_proof_out proof;
+} b200post_merge_result;
+
+/* Merges the range records in data_dir (every postdata file and one range's metadata copied in beside them).
+ * Host checks first, before any device is touched; each refusal leaves the metadata and initial_post.json untouched:
+ * metadata present (B200POST_ERR_IO); every range_*.rec intact (B200POST_ERR_IO naming the file) and made for this
+ * metadata (B200POST_ERR_CONFIG_MISMATCH); the records tile [0, numLabels) with no gap or overlap and each is complete
+ * (B200POST_ERR_STATE naming the uncovered labels or the record); every postdata file present with its implied size
+ * (B200POST_ERR_IO, "POST data is incomplete"); then B200POST_ERR_UNSUPPORTED for the CPU id and NO_DEVICE without a GPU.
+ * Nonce: the minimum of the records' VRF bests under (label32, index), then the rule of an init (below the threshold:
+ * LastPosition 0; else the past-the-end search on provider_id, resumable); VrfScanPending is cleared and the metadata
+ * saved.  No stored label is read.
+ * Initial proof, once the nonce is settled: every record must carry the proof part with the same K1, K2, nonces, W, pow
+ * difficulty (also cfg's), pow mode and cache key, and the same pows; the records' hit lists go into the prover's rule as
+ * one shard each in range order, the winner goes through the verifier gate on the first device of provider_id and into
+ * initial_post.json.  Without a proof, any initial_post.json in data_dir is deleted.  The nonce fields and
+ * initial_post.json are byte-identical to those of one uninterrupted full session with the initial proof.
+ * Returns OK once the nonce is settled (proof_rc says what became of the proof), CANCELLED when stopped. */
+int b200post_merge_range_records(const char *data_dir, const b200post_post_config *cfg, const b200post_merge_opts *o,
+                                 b200post_merge_result *out, const volatile int *cancel);
+
 /* After the session is COMPLETE: its initial proof and ProofMetadata (meta may be NULL), or INVALID_PROOF with the reason.
  * Before that, or when the session did not ask for one: B200POST_ERR_STATE. */
 int b200post_setup_initial_proof(b200post_setup_manager *mgr, b200post_proof_out *out, b200post_proof_metadata *meta);
