@@ -19,6 +19,7 @@
 #include <vector>
 
 #include "../../include/b200post.h"
+#include "../../include/b200post_setup.h"
 #include "metrics.h"
 
 namespace b200post {
@@ -29,6 +30,7 @@ std::atomic<uint64_t> g_launches{0};
 static thread_local std::string t_error;
 void set_error(const std::string &msg) { t_error = msg; }
 const char *last_error() { return t_error.c_str(); }
+int fail(int rc, const std::string &msg) { set_error(msg); return rc; }
 
 static inline uint32_t round_up(uint32_t x, uint32_t m) { return (x + m - 1) / m * m; }
 
@@ -549,6 +551,15 @@ int device_count() {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
     return n;
+}
+
+int provider_devices(int64_t provider_id, std::vector<uint32_t> *devs) {
+    if (provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) return fail(B200POST_ERR_UNSUPPORTED, "provider 0xffffffff (CPU): this library has no CPU path");
+    const int n = device_count();
+    if (n == 0) return fail(B200POST_ERR_NO_DEVICE, "no CUDA device available");
+    if (provider_id != B200POST_PROVIDER_ALL) devs->push_back((uint32_t)provider_id);
+    else for (int d = 0; d < n; d++) devs->push_back((uint32_t)d);
+    return B200POST_OK;
 }
 
 DeviceEngine *engine_for(uint32_t provider) {

@@ -47,6 +47,7 @@ struct CompareResult {
 
 void set_error(const std::string &msg);
 const char *last_error();
+int fail(int rc, const std::string &msg);   // set_error(msg), then rc
 
 class DeviceEngine {
 public:
@@ -179,6 +180,10 @@ private:
 // registry: lazily created engine per CUDA ordinal (nullptr + error text if the device is unusable)
 DeviceEngine *engine_for(uint32_t provider);
 int device_count();
+// The CUDA ordinals a provider id names at a host entry point: every device for B200POST_PROVIDER_ALL, else the id.
+// B200POST_ERR_UNSUPPORTED for the CPU id, B200POST_ERR_NO_DEVICE when the machine has no device; an ordinal past the
+// last device is left to engine_for.
+int provider_devices(int64_t provider_id, std::vector<uint32_t> *devs);
 void shutdown_all();
 
 }  // namespace b200post

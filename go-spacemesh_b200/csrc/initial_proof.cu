@@ -3,23 +3,14 @@
 #include "initial_proof.h"
 
 #include <algorithm>
-#include <cerrno>
-#include <cstdio>
 #include <cstring>
 
 #include "postdata_io.h"
 #include "randomx_engine.h"
-#include "setup_internal.h"
 
 namespace b200post {
-
-const char kInitialProofFile[] = "initial_post.json";
-const char kInitialScanFile[] = "initial_post.scan";
-const char kRangeRecordPrefix[] = "range_";
-
 namespace {
 
-const uint8_t kZeroChallenge[32] = {0};   // shared.ZeroChallenge: the challenge of the initial proof
 const uint64_t kMaxScanChunk = 1ull << 22;   // labels per scan chunk (64 MiB of pinned staging per buffer), as the prover
 
 uint64_t fnv1a64(const std::string &s) {
@@ -34,8 +25,6 @@ template <class T> bool get(const std::string &s, size_t *p, T *v) {
     *p += sizeof(T);
     return true;
 }
-std::string join(const std::string &d, const char *f) { return d.empty() || d.back() == '/' ? d + f : d + "/" + f; }
-
 }  // namespace
 
 // Everything the scan's result depends on besides the labels: a state whose header differs is someone else's.  A
@@ -74,8 +63,8 @@ std::string InitialProofScan::proof_part() const {
     return h;
 }
 
-std::string InitialProofScan::record_path() const {
-    return join(dir_, (std::string(kRangeRecordPrefix) + std::to_string(range_.from_file) + "_" + std::to_string(range_.to_file) + ".rec").c_str());
+std::string InitialProofScan::state_path() const {
+    return record_ ? range_record_path(dir_, range_.from_file, range_.to_file) : join(dir_, kInitialScanFile);
 }
 
 // header | pows | upto | lists (count, then nonce, length, indices) | a record's VRF best (found, index, label32) |
@@ -98,13 +87,7 @@ int InitialProofScan::save_state() {
         s.append(reinterpret_cast<const char *>(vrf_.label32), 32);
     }
     put<uint64_t>(&s, fnv1a64(s));
-    const std::string fin = record_ ? record_path() : join(dir_, kInitialScanFile), tmp = fin + ".tmp";
-    FILE *f = fopen(tmp.c_str(), "wb");
-    if (!f) { set_error("open " + tmp + ": " + strerror(errno)); return B200POST_ERR_IO; }
-    const bool ok = fwrite(s.data(), 1, s.size(), f) == s.size();
-    if (fclose(f) != 0 || !ok) { set_error("write " + tmp + ": " + strerror(errno)); return B200POST_ERR_IO; }
-    if (rename(tmp.c_str(), fin.c_str()) != 0) { set_error("rename " + tmp + ": " + strerror(errno)); return B200POST_ERR_IO; }
-    return B200POST_OK;
+    return write_file_atomic(state_path(), s);
 }
 
 // The state in s, if it is intact, has this object's header and covers a prefix ending at or below `written`.
@@ -147,14 +130,8 @@ bool InitialProofScan::decode(const std::string &s, uint64_t written) {
 }
 
 bool InitialProofScan::load_state(uint64_t written) {
-    FILE *f = fopen((record_ ? record_path() : join(dir_, kInitialScanFile)).c_str(), "rb");
-    if (!f) return false;
     std::string s;
-    char buf[65536];
-    size_t n;
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) s.append(buf, n);
-    fclose(f);
-    return decode(s, written);
+    return read_file(state_path(), &s) && decode(s, written);
 }
 
 bool InitialProofScan::read_record(const std::string &s) {
@@ -197,7 +174,8 @@ int InitialProofScan::begin(const InitialProofRequest *req, const RangeSpec *ran
                             const b200post_post_metadata &md, const b200post_post_config &cfg, int64_t provider_id, uint64_t *written,
                             uint64_t batch, const volatile int *cancel) {
     dir_ = dir; md_ = md; cfg_ = cfg;
-    num_labels_ = (uint64_t)md.num_units * md.labels_per_unit;
+    const Layout lay(md);
+    num_labels_ = lay.num_labels;
     record_ = range != nullptr;
     proof_ = req != nullptr;
     range_ = record_ ? *range : RangeSpec{0, 0, 0, num_labels_};
@@ -209,14 +187,12 @@ int InitialProofScan::begin(const InitialProofRequest *req, const RangeSpec *ran
     }
     // the session's devices: the proving scan runs on the first, a BUILTIN k2pow search on all of them
     std::vector<uint32_t> devs;
-    if (provider_id == B200POST_PROVIDER_ALL) for (int i = 0; i < device_count(); i++) devs.push_back((uint32_t)i);
-    else devs.push_back((uint32_t)provider_id);
-    if (devs.empty()) { set_error("no CUDA device available"); return B200POST_ERR_NO_DEVICE; }
+    int rc = provider_devices(provider_id, &devs);
+    if (rc) return rc;
     scan_dev_ = devs[0];
     if (!engine_for(scan_dev_)) return B200POST_ERR_NO_DEVICE;
 
     if (proof_) rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{range_.lo, range_.hi}}, 0, opts_.nonces, windows_, cfg.k2);
-    int rc;
     if (!load_state(*written)) {
         // a record restarts at lo with nothing in it; the whole POST's scan restarts at 0 and rescans what is on disk
         vrf_ = b200post_vrf_nonce{}; upto_ = range_.lo;
@@ -234,7 +210,7 @@ int InitialProofScan::begin(const InitialProofRequest *req, const RangeSpec *ran
     const uint64_t chunk = std::min<uint64_t>({std::max<uint64_t>(batch, 1), kMaxScanChunk, num_labels_});
     if ((rc = sc_.init(scan_dev_, kZeroChallenge, nonces(), pows_.data(), cfg.k1, cfg.k2, num_labels_, chunk))) return rc;
     // the gap between the state's prefix and what is on disk, in index order, from the files
-    PostDataReader reader(dir, md.max_file_size / 16);
+    PostDataReader reader(dir, lay.per_file);
     for (uint64_t pos = upto(); pos < *written;) {
         if (cancel && *cancel) { stop(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
         const uint64_t n = std::min<uint64_t>(chunk, *written - pos);

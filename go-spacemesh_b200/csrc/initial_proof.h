@@ -55,7 +55,7 @@ public:
 
     // A record file read back for the merge: false unless it is intact and laid out as header() writes it.
     bool read_record(const std::string &bytes);
-    std::string record_path() const;   // range_<from>_<to>.rec in the data dir
+    std::string state_path() const;   // the scan state's or the record's file (a record read back has no directory)
     const b200post_post_metadata &md() const { return md_; }
     const b200post_post_config &cfg() const { return cfg_; }
     const b200post_prove_opts &opts() const { return opts_; }   // pow_cache_key points into this object
@@ -98,9 +98,5 @@ private:
     int b_ = 0;                   // staging buffer of the next chunk
     bool failed_ = false;         // a chunk failed to be submitted or collected
 };
-
-extern const char kInitialProofFile[];   // "initial_post.json"
-extern const char kInitialScanFile[];    // "initial_post.scan"
-extern const char kRangeRecordPrefix[];  // "range_": range_<from>_<to>.rec
 
 }  // namespace b200post

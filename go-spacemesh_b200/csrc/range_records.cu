@@ -20,37 +20,23 @@
 #include "../../include/b200post_prove.h"
 #include "engine.h"
 #include "initial_proof.h"
+#include "postdata_io.h"
 #include "prove_internal.h"
 #include "setup_internal.h"
 
 namespace b200post {
 namespace {
 
-int fail(int rc, const std::string &msg) { set_error(msg); return rc; }
-std::string join(const std::string &d, const std::string &f) { return d.empty() || d.back() == '/' ? d + f : d + "/" + f; }
-
-bool read_file(const std::string &path, std::string *out) {
-    FILE *f = fopen(path.c_str(), "rb");
-    if (!f) return false;
-    char buf[65536];
-    size_t n;
-    out->clear();
-    while ((n = fread(buf, 1, sizeof buf, f)) > 0) out->append(buf, n);
-    const bool ok = !ferror(f);
-    fclose(f);
-    return ok;
-}
-
 std::string span(uint64_t lo, uint64_t hi) { return "[" + std::to_string(lo) + ", " + std::to_string(hi) + ")"; }
 
 // The initial proof from the records (in range order), or the reason there is none: STATE when they hold no common
 // proof scan, INVALID_PROOF when no nonce reached K2 or the gate refused.  Other codes are errors of the call.
-int merged_proof(const std::vector<std::unique_ptr<InitialProofScan>> &recs, const b200post_post_metadata &md,
+int merged_proof(const std::vector<std::unique_ptr<InitialProofScan>> &recs, const b200post_post_metadata &md, const Layout &lay,
                  const b200post_post_config &cfg, uint32_t gate_dev, b200post_proof_out *out, b200post_proof_metadata *pm) {
     InitialProofScan &first = *recs[0];
     for (const auto &rp : recs) {
         InitialProofScan &r = *rp;
-        const std::string name = r.record_path();   // read back, a record has no directory
+        const std::string name = r.state_path();   // read back, a record has no directory
         if (!r.has_proof()) return fail(B200POST_ERR_STATE, name + " holds no initial-proof scan (VRF only)");
         if (r.proof_part() != first.proof_part())
             return fail(B200POST_ERR_STATE, name + " was scanned under other K1, K2, nonces, nonce windows, pow difficulty, pow mode or cache key");
@@ -59,7 +45,6 @@ int merged_proof(const std::vector<std::unique_ptr<InitialProofScan>> &recs, con
     const b200post_post_config &rc_cfg = first.cfg();
     if (rc_cfg.k1 != cfg.k1 || rc_cfg.k2 != cfg.k2 || memcmp(rc_cfg.pow_difficulty, cfg.pow_difficulty, 32))
         return fail(B200POST_ERR_STATE, "the records were scanned under another K1, K2 or pow difficulty than asked for");
-    const uint64_t num_labels = (uint64_t)md.num_units * md.labels_per_unit;
     const uint32_t nonces = first.opts().nonces, windows = first.windows();
     std::vector<std::pair<uint64_t, uint64_t>> ranges;
     for (const auto &r : recs) ranges.emplace_back(r->range().lo, r->range().hi);
@@ -74,7 +59,7 @@ int merged_proof(const std::vector<std::unique_ptr<InitialProofScan>> &recs, con
     std::vector<uint64_t> idx;
     int rc;
     if (!rule.decide(&nonce, &idx, &rc)) return rc ? rc : no_proof(windows, nonces);
-    if ((rc = write_proof(num_labels, nonce, idx, first.pows().data(), 0, num_labels, out))) return rc;
+    if ((rc = write_proof(lay.num_labels, nonce, idx, first.pows().data(), 0, lay.num_labels, out))) return rc;
     memset(pm, 0, sizeof *pm);
     memcpy(pm->node_id, md.node_id, 32);
     memcpy(pm->commitment_atx_id, md.commitment_atx_id, 32);
@@ -98,12 +83,12 @@ extern "C" int b200post_merge_range_records(const char *data_dir, const b200post
     b200post_post_metadata md;
     if (int rc = load_post_metadata(dir, &md)) return rc;
     if (cfg->labels_per_unit != md.labels_per_unit) return fail(B200POST_ERR_CONFIG_MISMATCH, "`LabelsPerUnit` mismatch with the metadata in DataDir");
-    const uint64_t num_labels = (uint64_t)md.num_units * md.labels_per_unit;
+    const Layout lay(md);   // checked with the files, below
     std::vector<std::string> names;
     if (DIR *d = opendir(dir.c_str())) {
         while (struct dirent *e = readdir(d)) {
-            const std::string n = e->d_name;
-            if (n.rfind(kRangeRecordPrefix, 0) == 0 && n.size() > 4 && n.substr(n.size() - 4) == ".rec") names.push_back(n);
+            bool tmp;
+            if (post_file_kind(e->d_name, &tmp) == PostFile::kRangeRecord && !tmp) names.push_back(e->d_name);
         }
         closedir(d);
     }
@@ -134,16 +119,17 @@ extern "C" int b200post_merge_range_records(const char *data_dir, const b200post
         if (r.lo > covered) gaps += (gaps.empty() ? "" : ", ") + span(covered, r.lo);
         covered = r.hi;
     }
-    if (covered < num_labels) gaps += (gaps.empty() ? "" : ", ") + span(covered, num_labels);
+    if (covered < lay.num_labels) gaps += (gaps.empty() ? "" : ", ") + span(covered, lay.num_labels);
     if (!gaps.empty()) return fail(B200POST_ERR_STATE, "the range records do not cover labels " + gaps + ": those ranges have no record");
     for (const auto &r : recs)
         if (r->upto() != r->range().hi)
-            return fail(B200POST_ERR_STATE, "range record " + r->record_path() + " is incomplete: it covers labels " + span(r->range().lo, r->upto()) +
+            return fail(B200POST_ERR_STATE, "range record " + r->state_path() + " is incomplete: it covers labels " + span(r->range().lo, r->upto()) +
                                                 " of " + span(r->range().lo, r->range().hi) + "; finish its range session first");
-    if (int rc = check_post_files(dir, md)) return rc;
-    if (o->provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) return fail(B200POST_ERR_UNSUPPORTED, "provider 0xffffffff (CPU): this library has no CPU path");
-    if (device_count() == 0) return fail(B200POST_ERR_NO_DEVICE, "no CUDA device available");
-    const uint32_t dev = o->provider_id == B200POST_PROVIDER_ALL ? 0u : (uint32_t)o->provider_id;
+    if (int rc = check_layout(md)) return rc;
+    if (int rc = check_post_files(dir, lay, 0, lay.n_files - 1)) return rc;
+    std::vector<uint32_t> devs;
+    if (int rc = provider_devices(o->provider_id, &devs)) return rc;
+    const uint32_t dev = devs[0];
     if (!engine_for(dev)) return B200POST_ERR_NO_DEVICE;
     out->ranges = (uint32_t)recs.size();
 
@@ -166,7 +152,7 @@ extern "C" int b200post_merge_range_records(const char *data_dir, const b200post
 
     // ---- the initial proof, once the nonce is settled (as in a full session); a stale file must not answer
     b200post_proof_metadata pm{};
-    int rc = merged_proof(recs, md, *cfg, dev, &out->proof, &pm);
+    int rc = merged_proof(recs, md, lay, *cfg, dev, &out->proof, &pm);
     if (rc == B200POST_OK) {
         if ((rc = save_initial_proof_file(dir, pm, *cfg, recs[0]->opts().nonces, recs[0]->windows(), out->proof))) return rc;
     } else if (rc == B200POST_ERR_STATE || rc == B200POST_ERR_INVALID_PROOF) {

@@ -1,6 +1,6 @@
 // setup_internal.h — what the setup sessions (setup.cu), the stored-data VRF search (vrf_search.cu) and the merge of
-// range records (range_records.cu) share: the metadata and proof files, the label calls of a provider choice, the
-// check that the POST's files are complete, and the rule that settles the VRF nonce.
+// range records (range_records.cu) share: the label calls of a provider choice and the rule that settles the VRF
+// nonce.  Their files are postdata_io.h's.
 #pragma once
 #include <cstdint>
 #include <string>
@@ -8,14 +8,6 @@
 #include "../../include/b200post_prove.h"
 
 namespace b200post {
-
-int save_post_metadata(const std::string &dir, const b200post_post_metadata &m);
-// B200POST_ERR_IO "metadata file is missing" when absent
-int load_post_metadata(const std::string &dir, b200post_post_metadata *m);
-// initial_post.json (tmp + rename): the proof for the zero challenge, the POST it belongs to, K1, K2, the pow
-// difficulty, the nonce count and (above 1) the nonce windows scanned
-int save_initial_proof_file(const std::string &dir, const b200post_proof_metadata &pm, const b200post_post_config &cfg, uint32_t nonces,
-                            uint32_t windows, const b200post_proof_out &p);
 
 // labels [start, start + count) of scrypt-N on provider_id (a CUDA ordinal or B200POST_PROVIDER_ALL); nonce (may be
 // NULL) is zeroed, then filled by the VRF scan when diff is given
@@ -27,10 +19,6 @@ int compute_labels(int64_t provider_id, uint64_t N, const uint8_t commitment[32]
 // batch, so a stopped search resumes where it stopped
 int search_past_end(const std::string &dir, b200post_post_metadata *md, uint64_t num_labels, int64_t provider_id, uint64_t batch,
                     const uint8_t commitment[32], const uint8_t diff[32], const volatile int *cancel);
-
-// "POST data is incomplete": every postdata file of the metadata exists with its implied size (B200POST_ERR_IO otherwise,
-// also for metadata whose label count, MaxFileSize or Scrypt.N is out of range).  Reads no label.
-int check_post_files(const std::string &dir, const b200post_post_metadata &md);
 
 // The rule of an init, given the arg-min (best_index, best32) of label32 over [0, numLabels): strictly below
 // floor(2^256 / numLabels) it is the nonce (LastPosition 0), else the past-the-end search on provider_id finds it

@@ -5,7 +5,6 @@
 //   fraction 100: range compare jobs over the checked files, with the VRF scan (arg-min) fused in
 //   fraction < 100: per file max(1, floor(L * fraction / 100)) positions drawn from (seed, file), indexed compare jobs
 #include <sys/random.h>
-#include <sys/stat.h>
 
 #include <algorithm>
 #include <cmath>
@@ -90,11 +89,6 @@ private:
     Rng r_{0};
     std::vector<uint64_t> all_;
     size_t at_ = 0;
-};
-
-struct Layout {
-    uint64_t num_labels = 0, per_file = 0, n_files = 0;
-    uint64_t labels_in(uint64_t f) const { return std::min<uint64_t>(per_file, num_labels - f * per_file); }
 };
 
 // one compare job and the stored labels it checks
@@ -258,8 +252,6 @@ void check_sampled(DeviceEngine *e, const Layout &lay, const std::string &dir, u
     if (res->rc == B200POST_OK) res->files = f1 - f0;
 }
 
-int fail(int rc, const std::string &msg) { set_error(msg); return rc; }
-
 }  // namespace
 
 extern "C" {
@@ -291,27 +283,15 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
 
     // ---- metadata and files, on the host before any device is touched
     b200post_post_metadata md;
-    int rc = b200post_load_metadata(data_dir, &md);
-    if (rc) return rc;
-    const unsigned __int128 nl = (unsigned __int128)md.num_units * md.labels_per_unit;
+    int rc = load_post_metadata(data_dir, &md);
+    if (rc || (rc = check_layout(md))) return rc;
+    const Layout lay(md);
     const uint64_t N = md.scrypt_n;
-    if (nl == 0 || nl > (~0ull >> 4) || md.max_file_size < 16 || md.max_file_size % 16 || N < 2 || N > (1ull << 20) || (N & (N - 1)))
-        return fail(B200POST_ERR_IO, "corrupt metadata: label count, MaxFileSize or Scrypt.N out of range");
-    Layout lay;
-    lay.num_labels = (uint64_t)nl; lay.per_file = md.max_file_size / 16;
-    lay.n_files = (lay.num_labels + lay.per_file - 1) / lay.per_file;
     const uint64_t last = o->to_file < 0 ? lay.n_files - 1 : (uint64_t)o->to_file;
     if (last >= lay.n_files || o->from_file > last)
         return fail(B200POST_ERR_INVALID_ARGUMENT, "invalid file range: the POST has " + std::to_string(lay.n_files) + " files");
     const std::string dir = data_dir;
-    for (uint64_t f = o->from_file; f <= last; f++) {
-        struct stat st;
-        const std::string p = postdata_path(dir, f);
-        if (stat(p.c_str(), &st) != 0) return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " is missing");
-        if ((uint64_t)st.st_size != lay.labels_in(f) * 16)
-            return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " holds " + std::to_string(st.st_size) + " bytes, the metadata implies " +
-                                             std::to_string(lay.labels_in(f) * 16));
-    }
+    if ((rc = check_post_files(dir, lay, o->from_file, last))) return rc;
     uint64_t seed = o->seed;
     while (seed == 0) {
         if (getrandom(&seed, sizeof seed, 0) != (ssize_t)sizeof seed) return fail(B200POST_ERR_IO, "getrandom failed");
@@ -319,16 +299,10 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
     out->seed = seed;
 
     // ---- devices
-    if (o->provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) return fail(B200POST_ERR_UNSUPPORTED, "provider 0xffffffff (CPU): this library has no CPU path");
-    const int n_dev = device_count();
-    if (n_dev == 0) return fail(B200POST_ERR_NO_DEVICE, "no CUDA device available");
+    std::vector<uint32_t> devs;
+    if ((rc = provider_devices(o->provider_id, &devs))) return rc;
     std::vector<DeviceEngine *> engines;
-    if (o->provider_id == B200POST_PROVIDER_ALL) {
-        for (int d = 0; d < n_dev; d++) engines.push_back(engine_for((uint32_t)d));
-    } else {
-        engines.push_back(engine_for((uint32_t)o->provider_id));
-    }
-    for (DeviceEngine *e : engines) if (!e) return B200POST_ERR_NO_DEVICE;
+    for (uint32_t d : devs) if (!engines.emplace_back(engine_for(d))) return B200POST_ERR_NO_DEVICE;
 
     uint8_t commitment[32], diff[32];
     commitment_bytes(md.node_id, md.commitment_atx_id, commitment);

@@ -14,8 +14,6 @@
 #include <utility>
 #include <vector>
 
-#include <sys/stat.h>
-
 #include "../../include/b200post_setup.h"
 #include "engine.h"
 #include "host_hash.h"
@@ -214,8 +212,6 @@ struct Running {
     }
 };
 
-int fail(int rc, const std::string &msg) { set_error(msg); return rc; }
-
 }  // namespace
 
 int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const b200post_vrf_search_opts &o, b200post_vrf_nonce *out,
@@ -227,20 +223,21 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     if (chunk > kMaxChunk) return fail(B200POST_ERR_INVALID_ARGUMENT, "chunk_labels above 2^26");
 
     // ---- metadata and files, on the host before any device is touched
-    if (int rc = check_post_files(dir, *md)) return rc;
-    const uint64_t N = md->scrypt_n;
-    const uint64_t num_labels = (uint64_t)md->num_units * md->labels_per_unit, per_file = md->max_file_size / 16;
+    if (int rc = check_layout(*md)) return rc;
+    const Layout lay(*md);
+    if (int rc = check_post_files(dir, lay, 0, lay.n_files - 1)) return rc;
+    const uint64_t N = md->scrypt_n, num_labels = lay.num_labels;
 
     // ---- device: the scan runs on one (it is bound by storage, not by the GPU)
-    if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) return fail(B200POST_ERR_UNSUPPORTED, "provider 0xffffffff (CPU): this library has no CPU path");
-    if (device_count() == 0) return fail(B200POST_ERR_NO_DEVICE, "no CUDA device available");
-    DeviceEngine *e = engine_for(o.provider_id == B200POST_PROVIDER_ALL ? 0u : (uint32_t)o.provider_id);
+    std::vector<uint32_t> devs;
+    if (int rc = provider_devices(o.provider_id, &devs)) return rc;
+    DeviceEngine *e = engine_for(devs[0]);
     if (!e) return B200POST_ERR_NO_DEVICE;
     chunk = std::min(chunk, num_labels);
 
     Running best;
     {
-        PostDataReader reader(dir, per_file);
+        PostDataReader reader(dir, lay.per_file);
         StoredScan scan;
         int rc = scan.init(e, chunk);
         if (rc) return rc;
@@ -298,24 +295,6 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     return settle_nonce(dir, md, best_index, best32, o.provider_id, batch, out, nullptr, cancel);
 }
 
-int check_post_files(const std::string &dir, const b200post_post_metadata &md) {
-    const unsigned __int128 nl = (unsigned __int128)md.num_units * md.labels_per_unit;
-    const uint64_t N = md.scrypt_n;
-    if (nl == 0 || nl > (~0ull >> 4) || md.max_file_size < 16 || md.max_file_size % 16 || N < 2 || N > (1ull << 20) || (N & (N - 1)))
-        return fail(B200POST_ERR_IO, "corrupt metadata: label count, MaxFileSize or Scrypt.N out of range");
-    const uint64_t num_labels = (uint64_t)nl, per_file = md.max_file_size / 16, n_files = (num_labels + per_file - 1) / per_file;
-    for (uint64_t f = 0; f < n_files; f++) {
-        struct stat st;
-        const std::string p = postdata_path(dir, f);
-        const uint64_t want = std::min<uint64_t>(per_file, num_labels - f * per_file) * 16;
-        if (stat(p.c_str(), &st) != 0) return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " is missing");
-        if ((uint64_t)st.st_size != want)
-            return fail(B200POST_ERR_IO, "POST data is incomplete: " + p + " holds " + std::to_string(st.st_size) + " bytes, the metadata implies " +
-                                             std::to_string(want));
-    }
-    return B200POST_OK;
-}
-
 // The rule of an init: below the threshold, or the past-the-end search.
 int settle_nonce(const std::string &dir, b200post_post_metadata *md, uint64_t best_index, const uint8_t best32[32], int64_t provider_id,
                  uint64_t batch, b200post_vrf_nonce *out, bool *past_end, const volatile int *cancel) {
@@ -355,7 +334,7 @@ void b200post_default_vrf_search_opts(b200post_vrf_search_opts *o) {
 int b200post_search_vrf_nonce(const char *data_dir, const b200post_vrf_search_opts *o, b200post_vrf_nonce *out, const volatile int *cancel) {
     if (!data_dir || !o || !out) return fail(B200POST_ERR_INVALID_ARGUMENT, "invalid argument");
     b200post_post_metadata md;
-    if (int rc = b200post_load_metadata(data_dir, &md)) return rc;
+    if (int rc = load_post_metadata(data_dir, &md)) return rc;
     return stored_vrf_search(data_dir, &md, *o, out, cancel);
 }
 
