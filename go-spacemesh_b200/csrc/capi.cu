@@ -3,7 +3,6 @@
 #include <chrono>
 #include <cstring>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "../../include/b200post.h"
@@ -35,18 +34,12 @@ int range_common(uint32_t provider, const uint8_t *commitment, uint64_t n, uint6
         set_error("invalid argument (commitment NULL, N not a power of two in [2, 2^20], missing nonce out, or index overflow)");
         return B200POST_ERR_INVALID_ARGUMENT;
     }
-    if (provider == B200POST_CPU_PROVIDER_ID) { engine_for(provider); return B200POST_ERR_UNSUPPORTED; }
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     VrfResult vr;
     const int rc = e->labels_range(commitment, n, start, count, out_host, out_dev, vrf_difficulty, &vr, cancel);
     if (rc == B200POST_OK) fill_nonce(nonce, vr);
     return rc;
-}
-
-bool label_less(const uint8_t a[32], uint64_t ai, const uint8_t b[32], uint64_t bi) {
-    const int c = memcmp(a, b, 32);
-    return c ? c < 0 : ai < bi;
 }
 
 }  // namespace
@@ -131,30 +124,21 @@ int b200post_labels_range_multi(const uint32_t *providers, int n_providers, cons
     // contiguous shards: device g gets [start + g*per, start + (g+1)*per) — keeps each device's output a
     // contiguous slice of the POST data (SURVEY.md §8e)
     const uint64_t per = (count + (uint64_t)n_providers - 1) / (uint64_t)n_providers;
-    std::vector<int> rcs((size_t)n_providers, B200POST_OK);
     std::vector<b200post_vrf_nonce> nonces((size_t)n_providers);
-    std::vector<std::string> errs((size_t)n_providers);
-    std::vector<std::thread> threads;
-    for (int g = 0; g < n_providers; g++) {
+    const int rc = fan_out((size_t)n_providers, [&](size_t g) {
         const uint64_t off = std::min<uint64_t>(per * (uint64_t)g, count);
         const uint64_t cnt = std::min<uint64_t>(per, count - off);
-        threads.emplace_back([=, &rcs, &nonces, &errs] {
-            memset(&nonces[(size_t)g], 0, sizeof(b200post_vrf_nonce));
-            rcs[(size_t)g] = b200post_labels_range(providers[g], commitment, n, start + off, cnt,
-                                                   out16 ? out16 + off * 16 : nullptr, vrf_difficulty,
-                                                   vrf_difficulty ? &nonces[(size_t)g] : nullptr, cancel);
-            if (rcs[(size_t)g]) errs[(size_t)g] = last_error();
-        });
-    }
-    for (auto &t : threads) t.join();
-    for (int g = 0; g < n_providers; g++)
-        if (rcs[(size_t)g]) { set_error("provider " + std::to_string(providers[g]) + ": " + errs[(size_t)g]); return rcs[(size_t)g]; }
+        memset(&nonces[g], 0, sizeof(b200post_vrf_nonce));
+        const int r = b200post_labels_range(providers[g], commitment, n, start + off, cnt, out16 ? out16 + off * 16 : nullptr,
+                                            vrf_difficulty, vrf_difficulty ? &nonces[g] : nullptr, cancel);
+        if (r) set_error("provider " + std::to_string(providers[g]) + ": " + last_error());
+        return r;
+    });
+    if (rc) return rc;
     if (vrf_difficulty && nonce) {
         memset(nonce, 0, sizeof *nonce);
-        for (int g = 0; g < n_providers; g++) {
-            const b200post_vrf_nonce &c = nonces[(size_t)g];
-            if (c.found && (!nonce->found || label_less(c.label32, c.index, nonce->label32, nonce->index))) *nonce = c;
-        }
+        for (const b200post_vrf_nonce &c : nonces)
+            if (c.found && (!nonce->found || vrf_less(c.label32, c.index, nonce->label32, nonce->index))) *nonce = c;
     }
     return B200POST_OK;
 }
@@ -165,9 +149,8 @@ int b200post_labels_gather(uint32_t provider, size_t n_items, const uint8_t *com
         set_error("invalid argument");
         return B200POST_ERR_INVALID_ARGUMENT;
     }
-    if (provider == B200POST_CPU_PROVIDER_ID) { engine_for(provider); return B200POST_ERR_UNSUPPORTED; }
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     return e->labels_gather(n_items, commitments, indices, n, out16);
 }
 
@@ -180,9 +163,8 @@ int b200post_labels_gather_indexed(uint32_t provider, size_t n_items, size_t n_c
     }
     for (size_t i = 0; i < n_items; i++)
         if (commitment_index[i] >= n_commitments) { set_error("commitment_index out of range"); return B200POST_ERR_INVALID_ARGUMENT; }
-    if (provider == B200POST_CPU_PROVIDER_ID) { engine_for(provider); return B200POST_ERR_UNSUPPORTED; }
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     return e->labels_gather_indexed(n_items, n_commitments, commitments, commitment_index, indices, n, out16, nullptr);
 }
 
@@ -237,8 +219,8 @@ int b200post_benchmark(uint32_t provider, uint64_t n, double seconds, double *la
     if (!labels_per_sec || !valid_n(n)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     uint8_t commitment[32];
     memset(commitment, 0x5a, 32);
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     // batches of 4 whole layers (the software pipeline needs >= 4 to run filled, and back-to-back calls continue it:
     // DeviceEngine's speculative next-layer fill); the first call allocates the scratch and is not timed
     uint64_t slots = 0;
@@ -271,8 +253,8 @@ int b200post_romix_time(uint32_t provider, double *ms_total, uint64_t *launches,
 
 int b200post_wave_slots(uint32_t provider, uint64_t n, uint64_t *slots) {
     if (!slots || !valid_n(n)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     *slots = e->wave_slots(n);
     return *slots ? B200POST_OK : B200POST_ERR_CUDA;
 }

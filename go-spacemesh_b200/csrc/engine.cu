@@ -16,6 +16,7 @@
 #include <cstring>
 #include <map>
 #include <memory>
+#include <thread>
 #include <vector>
 
 #include "../../include/b200post.h"
@@ -578,9 +579,47 @@ DeviceEngine *engine_for(uint32_t provider) {
     return it->second.get();
 }
 
+int device_engine(uint32_t provider, DeviceEngine **e) {
+    DeviceEngine *got = engine_for(provider);
+    if (e) *e = got;
+    if (got) return B200POST_OK;
+    return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+}
+
+int device_engines(const uint32_t *providers, int n, std::vector<DeviceEngine *> *out) {
+    if (out) out->assign((size_t)n, nullptr);
+    for (int i = 0; i < n; i++)
+        if (int rc = device_engine(providers[i], out ? &(*out)[(size_t)i] : nullptr)) return rc;
+    return B200POST_OK;
+}
+
 void shutdown_all() {
     std::lock_guard<std::mutex> lk(g_reg_mu);
     g_engines.clear();
+}
+
+int fan_out(size_t parts, const std::function<int(size_t)> &part) {
+    std::vector<int> rcs(parts, B200POST_OK);
+    std::vector<std::string> errs(parts);
+    std::vector<std::thread> th;
+    for (size_t i = 0; i < parts; i++)
+        th.emplace_back([&, i] {
+            if ((rcs[i] = part(i)) != B200POST_OK) errs[i] = last_error();
+        });
+    for (auto &t : th) t.join();
+    for (size_t i = 0; i < parts; i++)
+        if (rcs[i] != B200POST_OK) return fail(rcs[i], errs[i]);
+    return B200POST_OK;
+}
+
+int label32_at(DeviceEngine *e, const uint8_t commitment[32], uint64_t N, uint64_t index, uint8_t out[32]) {
+    uint8_t all[32];
+    memset(all, 0xff, 32);
+    VrfResult vr;
+    if (int rc = e->labels_range(commitment, N, index, 1, nullptr, nullptr, all, &vr, nullptr)) return rc;
+    if (!vr.found) memset(vr.label32, 0xff, 32);   // found is 0 only for the all-ones label
+    memcpy(out, vr.label32, 32);
+    return B200POST_OK;
 }
 
 }  // namespace b200post

@@ -179,11 +179,23 @@ private:
 
 // registry: lazily created engine per CUDA ordinal (nullptr + error text if the device is unusable)
 DeviceEngine *engine_for(uint32_t provider);
+// engine_for as a B200POST_* code: B200POST_ERR_UNSUPPORTED for the CPU id (no CPU path), B200POST_ERR_NO_DEVICE for an
+// id that names no device.  e / out (optional) get the engines.  A list answers with its first failing entry's code.
+int device_engine(uint32_t provider, DeviceEngine **e = nullptr);
+int device_engines(const uint32_t *providers, int n, std::vector<DeviceEngine *> *out = nullptr);
 int device_count();
 // The CUDA ordinals a provider id names at a host entry point: every device for B200POST_PROVIDER_ALL, else the id.
 // B200POST_ERR_UNSUPPORTED for the CPU id, B200POST_ERR_NO_DEVICE when the machine has no device; an ordinal past the
 // last device is left to engine_for.
 int provider_devices(int64_t provider_id, std::vector<uint32_t> *devs);
 void shutdown_all();
+
+// Runs part(0) .. part(parts - 1) on one thread each and returns once all have ended: B200POST_OK, or the code of the
+// first failing part in list order, whose error text (thread-local, so copied out as its thread ends) is then this
+// thread's.
+int fan_out(size_t parts, const std::function<int(size_t)> &part);
+
+// The label32 at `index` (one label, recomputed on e); all-ones is a label32 like any other
+int label32_at(DeviceEngine *e, const uint8_t commitment[32], uint64_t N, uint64_t index, uint8_t out[32]);
 
 }  // namespace b200post

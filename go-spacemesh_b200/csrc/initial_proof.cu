@@ -190,7 +190,7 @@ int InitialProofScan::begin(const InitialProofRequest *req, const RangeSpec *ran
     int rc = provider_devices(provider_id, &devs);
     if (rc) return rc;
     scan_dev_ = devs[0];
-    if (!engine_for(scan_dev_)) return B200POST_ERR_NO_DEVICE;
+    if ((rc = device_engine(scan_dev_))) return rc;
 
     if (proof_) rule_.emplace(std::vector<std::pair<uint64_t, uint64_t>>{{range_.lo, range_.hi}}, 0, opts_.nonces, windows_, cfg.k2);
     if (!load_state(*written)) {

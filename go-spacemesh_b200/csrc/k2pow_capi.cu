@@ -3,7 +3,6 @@
 #include <atomic>
 #include <cstring>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "../../include/b200post_k2pow.h"
@@ -61,6 +60,14 @@ int search_window(RandomxEngine *e, const std::string &key, const b200post_k2pow
     return B200POST_OK;
 }
 
+// randomx_engine of every entry in list order; the first failing entry's code (and text) answers
+int randomx_engines(const uint32_t *providers, int n, std::vector<RandomxEngine *> *out) {
+    out->assign((size_t)n, nullptr);
+    for (int i = 0; i < n; i++)
+        if (int rc = randomx_engine(providers[i], &(*out)[(size_t)i])) return rc;
+    return B200POST_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -71,16 +78,16 @@ void b200post_k2pow_scale_difficulty(const uint8_t pow_difficulty[32], uint32_t 
 }
 
 int b200post_randomx_prepare(uint32_t provider, const uint8_t *key, size_t key_len) {
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     return e->prepare(key_of(key, key_len));
 }
 
 int b200post_randomx_hash(uint32_t provider, const uint8_t *key, size_t key_len, const uint8_t *inputs, size_t input_len, size_t n,
                           uint8_t *out32) {
     if ((n && !out32) || (n && input_len && !inputs) || input_len > (1u << 20)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     return e->hash_inputs(key_of(key, key_len), inputs, input_len, n, out32);
 }
 
@@ -90,23 +97,23 @@ int b200post_randomx_dataset_read(uint32_t provider, const uint8_t *key, size_t 
         set_error("invalid argument: items past the end of the dataset, or no output buffer");
         return B200POST_ERR_INVALID_ARGUMENT;
     }
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     return e->dataset_read(key_of(key, key_len), first_item, count, out);
 }
 
 int b200post_k2pow_hashes(uint32_t provider, const b200post_k2pow_params *p, uint64_t start, uint64_t count, uint8_t *out32) {
     if (!p || (count && !out32) || !clamp_range(start, count)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     return e->k2pow(key_of(p->cache_key, p->cache_key_len), template_of(p), nullptr, start, count, out32, nullptr, nullptr, nullptr);
 }
 
 int b200post_k2pow_search(uint32_t provider, const b200post_k2pow_params *p, uint64_t start, uint64_t count, uint64_t *found,
                           uint64_t *hashes_done, const volatile int *cancel) {
     if (!p || !found || !clamp_range(start, count)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     return e->k2pow(key_of(p->cache_key, p->cache_key_len), template_of(p), p->difficulty, start, count, nullptr, found, hashes_done, cancel);
 }
 
@@ -114,39 +121,31 @@ int b200post_k2pow_search_multi(const uint32_t *providers, int n_providers, cons
                                 uint64_t count, uint64_t *found, uint64_t *hashes_done, const volatile int *cancel) {
     if (!providers || n_providers <= 0 || !p || !found || !clamp_range(start, count)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     if (n_providers == 1) return b200post_k2pow_search(providers[0], p, start, count, found, hashes_done, cancel);
-    std::vector<RandomxEngine *> eng(n_providers);
+    std::vector<RandomxEngine *> eng;
+    if (int rc = randomx_engines(providers, n_providers, &eng)) return rc;
     uint64_t batch = UINT64_MAX;
-    for (int i = 0; i < n_providers; i++) {
-        eng[i] = randomx_engine_for(providers[i]);
-        if (!eng[i]) return providers[i] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    for (RandomxEngine *e : eng) {
         uint64_t b = 0;
-        eng[i]->batch_size(&b);
+        e->batch_size(&b);
         batch = std::min(batch, b);
     }
     // device i takes batches i, i+n, i+2n, ... of `batch` nonces; everyone stops after the round in which a hit appears
     const std::string key = key_of(p->cache_key, p->cache_key_len);
     const rx::K2powTemplate tmpl = template_of(p);
-    std::vector<int> rcs(n_providers, B200POST_OK);
     std::vector<uint64_t> hits(n_providers, UINT64_MAX), dones(n_providers, 0);
-    std::vector<std::string> errs(n_providers);
     volatile int any_hit = 0;
-    std::vector<std::thread> th;
-    for (int i = 0; i < n_providers; i++)
-        th.emplace_back([&, i] {
-            const uint64_t first = start + (uint64_t)i * batch;
-            if ((uint64_t)i * batch >= count) return;
-            rcs[i] = eng[i]->k2pow(key, tmpl, p->difficulty, first, count - (uint64_t)i * batch, nullptr, &hits[i], &dones[i], cancel,
-                                   batch * (uint64_t)n_providers, &any_hit);
-            if (rcs[i] != B200POST_OK) errs[i] = last_error();
-            if (hits[i] != UINT64_MAX) any_hit = 1;
-        });
-    for (auto &t : th) t.join();
+    const int rc = fan_out((size_t)n_providers, [&](size_t i) -> int {
+        if ((uint64_t)i * batch >= count) return B200POST_OK;
+        const int r = eng[i]->k2pow(key, tmpl, p->difficulty, start + (uint64_t)i * batch, count - (uint64_t)i * batch, nullptr, &hits[i],
+                                    &dones[i], cancel, batch * (uint64_t)n_providers, &any_hit);
+        if (hits[i] != UINT64_MAX) any_hit = 1;
+        return r;
+    });
     *found = UINT64_MAX;
     uint64_t total = 0;
     for (int i = 0; i < n_providers; i++) { total += dones[i]; if (hits[i] < *found) *found = hits[i]; }
     if (hashes_done) *hashes_done = total;
-    for (int i = 0; i < n_providers; i++) if (rcs[i] != B200POST_OK) { set_error(errs[i]); return rcs[i]; }
-    return B200POST_OK;
+    return rc;
 }
 
 int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params *p, uint32_t n_groups, uint64_t max_nonces_per_group,
@@ -157,8 +156,8 @@ int b200post_k2pow_search_groups(uint32_t provider, const b200post_k2pow_params 
 int b200post_k2pow_search_group_range(uint32_t provider, const b200post_k2pow_params *p, uint32_t first_group, uint32_t n_groups,
                                       uint64_t max_nonces_per_group, uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel) {
     if (!p || !pows || n_groups == 0 || (uint64_t)first_group + n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     const std::string key = key_of(p->cache_key, p->cache_key_len);
     uint64_t batch = 0;
     e->batch_size(&batch);
@@ -200,11 +199,8 @@ int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_pro
         return B200POST_ERR_INVALID_ARGUMENT;
     }
     if (n_providers == 1) return b200post_k2pow_search_group_range(providers[0], p, first_group, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
-    std::vector<RandomxEngine *> eng(n_providers);
-    for (int i = 0; i < n_providers; i++) {
-        eng[i] = randomx_engine_for(providers[i]);
-        if (!eng[i]) return providers[i] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
-    }
+    std::vector<RandomxEngine *> eng;
+    if (int rc = randomx_engines(providers, n_providers, &eng)) return rc;
     for (uint32_t g = 0; g < n_groups; g++) pows[g] = B200POST_K2POW_NOT_FOUND;
     const std::string key = key_of(p->cache_key, p->cache_key_len);
     const uint64_t cap = max_nonces_per_group == 0 || max_nonces_per_group > kNonceSpace ? kNonceSpace : max_nonces_per_group;
@@ -214,40 +210,37 @@ int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_pro
     std::mutex mu;
     uint64_t next = 0, total = 0;
     std::vector<uint64_t> best(n_groups, B200POST_K2POW_NOT_FOUND);
-    std::vector<int> rcs(n_providers, B200POST_OK);
-    std::vector<std::string> errs(n_providers);
     std::atomic<bool> stop{false};
-    std::vector<std::thread> th;
-    for (int i = 0; i < n_providers; i++)
-        th.emplace_back([&, i] {
-            uint64_t batch = 0;
-            eng[i]->batch_size(&batch);
-            std::vector<uint8_t> in, out;
-            std::vector<uint64_t> hit;
-            std::vector<uint32_t> groups;
-            while (!stop) {
-                if (cancel && *cancel) { set_error("cancelled"); rcs[i] = B200POST_ERR_CANCELLED; break; }
-                uint64_t lo, per;
-                {
-                    std::lock_guard<std::mutex> lk(mu);
-                    groups.clear();
-                    for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(first_group + g);
-                    if (groups.empty() || next >= cap) break;
-                    // one device batch: `per` consecutive nonces for each group still searching, as on one device
-                    per = std::min<uint64_t>(std::max<uint64_t>(1, batch / groups.size()), cap - next);
-                    lo = next;
-                    next += per;
-                }
-                if ((rcs[i] = search_window(eng[i], key, p, groups, lo, per, in, out, hit)) != B200POST_OK) break;
+    const int rc = fan_out((size_t)n_providers, [&](size_t i) {
+        uint64_t batch = 0;
+        eng[i]->batch_size(&batch);
+        std::vector<uint8_t> in, out;
+        std::vector<uint64_t> hit;
+        std::vector<uint32_t> groups;
+        int r = B200POST_OK;
+        while (!stop) {
+            if (cancel && *cancel) { set_error("cancelled"); r = B200POST_ERR_CANCELLED; break; }
+            uint64_t lo, per;
+            {
                 std::lock_guard<std::mutex> lk(mu);
-                total += groups.size() * per;
-                for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi] - first_group] = std::min(best[groups[gi] - first_group], hit[gi]);
+                groups.clear();
+                for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(first_group + g);
+                if (groups.empty() || next >= cap) break;
+                // one device batch: `per` consecutive nonces for each group still searching, as on one device
+                per = std::min<uint64_t>(std::max<uint64_t>(1, batch / groups.size()), cap - next);
+                lo = next;
+                next += per;
             }
-            if (rcs[i] != B200POST_OK) { errs[i] = last_error(); stop = true; }
-        });
-    for (auto &t : th) t.join();
+            if ((r = search_window(eng[i], key, p, groups, lo, per, in, out, hit)) != B200POST_OK) break;
+            std::lock_guard<std::mutex> lk(mu);
+            total += groups.size() * per;
+            for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi] - first_group] = std::min(best[groups[gi] - first_group], hit[gi]);
+        }
+        if (r != B200POST_OK) stop = true;
+        return r;
+    });
     if (hashes_done) *hashes_done = total;
-    for (int i = 0; i < n_providers; i++) if (rcs[i] != B200POST_OK) { set_error(errs[i]); return rcs[i]; }
+    if (rc) return rc;
     for (uint32_t g = 0; g < n_groups; g++) pows[g] = best[g];
     return B200POST_OK;
 }
@@ -256,8 +249,8 @@ int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uin
     if (!p || !valid) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     *valid = 0;
     if (pow >= kNonceSpace) return B200POST_OK;     // does not fit the 7 input bytes: cannot be what the prover hashed
-    RandomxEngine *e = randomx_engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    RandomxEngine *e;
+    if (int rc = randomx_engine(provider, &e)) return rc;
     uint64_t found = UINT64_MAX;
     const int rc = e->k2pow(key_of(p->cache_key, p->cache_key_len), template_of(p), p->difficulty, pow, 1, nullptr, &found, nullptr, nullptr);
     if (rc == B200POST_OK) *valid = found == pow;

@@ -13,6 +13,7 @@
 
 #include "../../include/b200post.h"
 #include "engine.h"
+#include "host_hash.h"
 
 using namespace b200post;
 
@@ -88,7 +89,7 @@ int b200post_vrf_comm_unique_id(uint8_t out128[128]) {
 int b200post_vrf_comm_init(uint32_t provider, int rank, int world, const uint8_t id128[128], b200post_vrf_comm **out) {
     if (!out || !id128 || world < 1 || rank < 0 || rank >= world) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     *out = nullptr;
-    if (!engine_for(provider)) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engine(provider)) return rc;
     Nccl *n = nccl();                  // loaded only once a device is there to use it
     if (!n) return B200POST_ERR_UNSUPPORTED;
     if (cudaSetDevice((int)provider) != cudaSuccess) { set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
@@ -123,11 +124,10 @@ int b200post_vrf_comm_min(b200post_vrf_comm *c, const b200post_vrf_nonce *mine, 
     if (cudaMemcpyAsync(c->host.data(), c->d_recv.get(), sizeof(Record) * (size_t)c->world, cudaMemcpyDeviceToHost, c->stream.get()) != cudaSuccess ||
         cudaStreamSynchronize(c->stream.get()) != cudaSuccess) { set_error("VRF exchange failed"); return B200POST_ERR_CUDA; }
     memset(best, 0, sizeof *best);
-    for (const Record &x : c->host) {
-        if (!x.found) continue;
-        const int cmp = best->found ? memcmp(x.label32, best->label32, 32) : -1;
-        if (cmp < 0 || (cmp == 0 && x.index < best->index)) { best->found = 1; best->index = x.index; memcpy(best->label32, x.label32, 32); }
-    }
+    for (const Record &x : c->host)
+        if (x.found && (!best->found || vrf_less(x.label32, x.index, best->label32, best->index))) {
+            best->found = 1; best->index = x.index; memcpy(best->label32, x.label32, 32);
+        }
     return B200POST_OK;
 }
 

@@ -137,8 +137,8 @@ int b200post_poet_pow_find(uint32_t provider, const uint8_t *pc, size_t pc_len, 
                            uint32_t difficulty, uint64_t start_nonce, uint64_t max_nonces, uint64_t *nonce, uint64_t *hashes,
                            const volatile int *cancel) {
     if ((!pc && pc_len) || (!ch && ch_len) || !node_id || !nonce || difficulty > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     PowJob job;
     if (!build_job(pc, pc_len, ch, ch_len, node_id, difficulty, &job)) {
         set_error("unsupported message layout: challenge lengths must add up to a multiple of 4 bytes");

@@ -140,8 +140,8 @@ __global__ void __launch_bounds__(256) prove_lazy_kernel(const uint4 *__restrict
 
 int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonces, const uint64_t *pows, uint32_t k1, uint32_t k2,
                   uint64_t num_labels, uint64_t chunk, bool keep_stored, uint32_t first_nonce) {
-    DeviceEngine *e = engine_for(provider);
-    if (!e) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(provider, &e)) return rc;
     if (nonces == 0 || nonces % 16 || first_nonce % 16 || (uint64_t)first_nonce + nonces > 4096 || k1 == 0 || k2 == 0 ||
         num_labels == 0 || chunk == 0 || chunk > (1u << 28)) {
         set_error("invalid proving parameters (nonces must be a positive multiple of 16, <= 4096)");
@@ -263,8 +263,6 @@ namespace {
 struct Shard {
     Scanner sc;
     uint64_t lo = 0, hi = 0;
-    int rc = B200POST_OK;
-    std::string err;
 };
 
 // The labels [0, total) in contiguous shards of whole chunks, one per provider in list order, sized within one chunk of
@@ -302,15 +300,11 @@ public:
     // list order, once every thread has joined
     int run(const Fill &fill, uint64_t chunk, uint64_t base, const volatile int *cancel) {
         if (shards_.size() == 1) return run_shard(0, fill, chunk, base, cancel);
-        std::vector<std::thread> th;
-        for (size_t s = 0; s < shards_.size(); s++)
-            th.emplace_back([&, s] {
-                Shard &sh = *shards_[s];
-                if ((sh.rc = run_shard(s, fill, chunk, base, cancel)) != B200POST_OK) { sh.err = last_error(); abort_ = true; }
-            });
-        for (auto &t : th) t.join();
-        for (auto &sh : shards_) if (sh->rc != B200POST_OK) { set_error(sh->err); return sh->rc; }
-        return B200POST_OK;
+        return fan_out(shards_.size(), [&](size_t s) {
+            const int rc = run_shard(s, fill, chunk, base, cancel);
+            if (rc != B200POST_OK) abort_ = true;
+            return rc;
+        });
     }
 
 private:

@@ -258,6 +258,12 @@ RandomxEngine *randomx_engine_for(uint32_t provider) {
     return it->second.get();
 }
 
+int randomx_engine(uint32_t provider, RandomxEngine **e) {
+    *e = randomx_engine_for(provider);
+    if (*e) return B200POST_OK;
+    return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+}
+
 void randomx_shutdown_all() {
     std::lock_guard<std::mutex> lk(g_rx_mu);
     g_rx.clear();

@@ -58,6 +58,8 @@ private:
 };
 
 RandomxEngine *randomx_engine_for(uint32_t provider);
+// randomx_engine_for as a B200POST_* code, as device_engine (engine.h) does for the label engine
+int randomx_engine(uint32_t provider, RandomxEngine **e);
 void randomx_shutdown_all();
 // release() of the engine on `device`, if one was created: its HBM goes back to the device, the engine stays usable
 void randomx_release(int device);

@@ -19,6 +19,7 @@
 
 #include "../../include/b200post_prove.h"
 #include "engine.h"
+#include "host_hash.h"
 #include "initial_proof.h"
 #include "postdata_io.h"
 #include "prove_internal.h"
@@ -130,7 +131,7 @@ extern "C" int b200post_merge_range_records(const char *data_dir, const b200post
     std::vector<uint32_t> devs;
     if (int rc = provider_devices(o->provider_id, &devs)) return rc;
     const uint32_t dev = devs[0];
-    if (!engine_for(dev)) return B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engine(dev)) return rc;
     out->ranges = (uint32_t)recs.size();
 
     // ---- the nonce: the least of the ranges' bests under (label32, index), then the rule of an init
@@ -141,8 +142,7 @@ extern "C" int b200post_merge_range_records(const char *data_dir, const b200post
     for (const auto &r : recs) {
         const b200post_vrf_nonce &v = r->vrf();
         if (!v.found) continue;
-        const int c = memcmp(v.label32, best32, 32);
-        if (!any || c < 0 || (c == 0 && v.index < best_index)) { memcpy(best32, v.label32, 32); best_index = v.index; any = true; }
+        if (!any || vrf_less(v.label32, v.index, best32, best_index)) { memcpy(best32, v.label32, 32); best_index = v.index; any = true; }
     }
     bool past_end = false;
     if (int rc = settle_nonce(dir, &md, best_index, best32, o->provider_id, o->compute_batch_size ? o->compute_batch_size : 1ull << 20,

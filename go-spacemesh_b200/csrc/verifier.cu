@@ -124,24 +124,13 @@ int b200post_verify_batch_multi(const uint32_t *providers, int n_providers, size
                                 uint64_t *invalid_indices) {
     if (!providers || n_providers <= 0) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     if (n_providers == 1 || n < 2) return b200post_verify_batch(providers[0], n, proofs, metas, params, options, opts, statuses, invalid_indices);
-    for (int d = 0; d < n_providers; d++)
-        if (!engine_for(providers[d])) return providers[d] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engines(providers, n_providers)) return rc;
     const size_t parts = std::min<size_t>((size_t)n_providers, n);
-    std::vector<int> rcs(parts, B200POST_OK);
-    std::vector<std::string> errs(parts);
-    std::vector<std::thread> th;
-    for (size_t d = 0; d < parts; d++) {
+    return fan_out(parts, [=](size_t d) {
         const size_t lo = n * d / parts, hi = n * (d + 1) / parts;
-        th.emplace_back([=, &rcs, &errs] {
-            rcs[d] = b200post_verify_batch(providers[d], hi - lo, proofs + lo, metas + lo, params, options ? options + lo : nullptr,
-                                           opts, statuses + lo, invalid_indices ? invalid_indices + lo : nullptr);
-            if (rcs[d] != B200POST_OK) errs[d] = b200post_last_error();   // the error text is thread-local
-        });
-    }
-    for (auto &t : th) t.join();
-    for (size_t d = 0; d < parts; d++)
-        if (rcs[d] != B200POST_OK) { set_error(errs[d]); return rcs[d]; }
-    return B200POST_OK;
+        return b200post_verify_batch(providers[d], hi - lo, proofs + lo, metas + lo, params, options ? options + lo : nullptr, opts,
+                                     statuses + lo, invalid_indices ? invalid_indices + lo : nullptr);
+    });
 }
 
 }  // extern "C"
@@ -541,7 +530,7 @@ extern "C" {
 int b200post_verifier_new(uint32_t provider, const b200post_verifier_opts *opts, b200post_verifier **out) {
     if (!out) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     *out = nullptr;
-    if (!engine_for(provider)) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engine(provider)) return rc;
     return b200post_verifier_new_multi(&provider, 1, opts, out);
 }
 
@@ -549,8 +538,7 @@ int b200post_verifier_new_multi(const uint32_t *providers, int n_providers, cons
                                 b200post_verifier **out) {
     if (!out || !providers || n_providers <= 0) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     *out = nullptr;
-    for (int d = 0; d < n_providers; d++)
-        if (!engine_for(providers[d])) return providers[d] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engines(providers, n_providers)) return rc;
     if (opts && (opts->pow_mode > B200POST_POW_SKIP || (opts->pow_mode == B200POST_POW_CALLBACK && !opts->pow_verify))) {
         set_error("pow_mode CALLBACK needs a pow_verify function; to run without the k2pow check ask for B200POST_POW_SKIP explicitly");
         return B200POST_ERR_UNSUPPORTED;
@@ -648,7 +636,7 @@ int b200post_verify_batch(uint32_t provider, size_t n, const b200post_proof *pro
                           const b200post_verify_params *params, const b200post_verify_options *options,
                           const b200post_verifier_opts *opts, int *statuses, uint64_t *invalid_indices) {
     if (n && (!proofs || !metas || !params || !statuses)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    if (!engine_for(provider)) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engine(provider)) return rc;
     b200post_verifier_opts vo{};
     if (opts) vo = *opts;
     if (vo.pow_mode > B200POST_POW_SKIP || (vo.pow_mode == B200POST_POW_CALLBACK && !vo.pow_verify)) {
@@ -675,7 +663,7 @@ int b200post_verify_batch(uint32_t provider, size_t n, const b200post_proof *pro
 int b200post_verify_vrf_nonces(uint32_t provider, size_t n, const b200post_vrf_check *checks, int *statuses, int *valid,
                                uint8_t *labels32) {
     if (n && (!checks || !statuses || !valid)) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    if (!engine_for(provider)) return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engine(provider)) return rc;
     if (n == 0) return B200POST_OK;
     std::vector<Job> jobs(n);
     std::vector<Job *> ptrs(n);
@@ -702,25 +690,14 @@ int b200post_verify_vrf_nonces(uint32_t provider, size_t n, const b200post_vrf_c
 int b200post_verify_vrf_nonces_multi(const uint32_t *providers, int n_providers, size_t n, const b200post_vrf_check *checks,
                                      int *statuses, int *valid, uint8_t *labels32) {
     if (!providers || n_providers <= 0 || (n && (!checks || !statuses || !valid))) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
-    for (int d = 0; d < n_providers; d++)
-        if (!engine_for(providers[d])) return providers[d] == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+    if (int rc = device_engines(providers, n_providers)) return rc;
     if (n_providers == 1 || n < 2) return b200post_verify_vrf_nonces(providers[0], n, checks, statuses, valid, labels32);
     const size_t parts = std::min<size_t>((size_t)n_providers, n);
-    std::vector<int> rcs(parts, B200POST_OK);
-    std::vector<std::string> errs(parts);
-    std::vector<std::thread> th;
-    for (size_t d = 0; d < parts; d++) {
+    return fan_out(parts, [=](size_t d) {
         const size_t lo = n * d / parts, hi = n * (d + 1) / parts;
-        th.emplace_back([=, &rcs, &errs] {
-            rcs[d] = b200post_verify_vrf_nonces(providers[d], hi - lo, checks + lo, statuses + lo, valid + lo,
-                                                labels32 ? labels32 + 32 * lo : nullptr);
-            if (rcs[d] != B200POST_OK) errs[d] = b200post_last_error();   // the error text is thread-local
-        });
-    }
-    for (auto &t : th) t.join();
-    for (size_t d = 0; d < parts; d++)
-        if (rcs[d] != B200POST_OK) { set_error(errs[d]); return rcs[d]; }
-    return B200POST_OK;
+        return b200post_verify_vrf_nonces(providers[d], hi - lo, checks + lo, statuses + lo, valid + lo,
+                                          labels32 ? labels32 + 32 * lo : nullptr);
+    });
 }
 
 }  // extern "C"

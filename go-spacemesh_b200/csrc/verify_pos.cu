@@ -12,7 +12,6 @@
 #include <future>
 #include <memory>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "../../include/b200post_setup.h"
@@ -111,11 +110,6 @@ struct DevResult {
     VrfResult best;              // full check: VRF arg-min over the device's share
 };
 
-bool vrf_less(const VrfResult &a, const VrfResult &b) {
-    const int c = memcmp(a.label32, b.label32, 32);
-    return c ? c < 0 : a.index < b.index;
-}
-
 void add_progress(volatile uint64_t *p, uint64_t n) {
     if (p) __atomic_fetch_add(p, n, __ATOMIC_RELAXED);
 }
@@ -155,7 +149,7 @@ void run_chunks(DeviceEngine *e, size_t n_chunks, Load load, const uint8_t commi
         }
         res->labels += cur.count;
         add_progress(o.progress, cur.count);
-        if (diff && vr.found && (!res->best.found || vrf_less(vr, res->best))) res->best = vr;
+        if (diff && vr.found && (!res->best.found || vrf_less(vr.label32, vr.index, res->best.label32, res->best.index))) res->best = vr;
     }
 }
 
@@ -302,7 +296,7 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
     std::vector<uint32_t> devs;
     if ((rc = provider_devices(o->provider_id, &devs))) return rc;
     std::vector<DeviceEngine *> engines;
-    for (uint32_t d : devs) if (!engines.emplace_back(engine_for(d))) return B200POST_ERR_NO_DEVICE;
+    if ((rc = device_engines(devs.data(), (int)devs.size(), &engines))) return rc;
 
     uint8_t commitment[32], diff[32];
     commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
@@ -325,13 +319,8 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
             check_sampled(engines[g], lay, dir, a, b, seed, o->fraction, commitment, N, *o, cancel, &res[g]);
         }
     };
-    if (G == 1) {
-        work(0);
-    } else {
-        std::vector<std::thread> th;
-        for (size_t g = 0; g < G; g++) th.emplace_back(work, g);
-        for (auto &t : th) t.join();
-    }
+    if (G == 1) work(0);
+    else fan_out(G, [&](size_t g) { work(g); return B200POST_OK; });   // the parts' outcomes are in res, merged below
 
     // ---- merge
     int status = B200POST_OK;
@@ -345,7 +334,7 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
         }
         out->labels_checked += r.labels; out->mismatches += r.mismatches;
         bad.insert(bad.end(), r.bad.begin(), r.bad.end());
-        if (r.best.found && (!best.found || vrf_less(r.best, best))) best = r.best;
+        if (r.best.found && (!best.found || vrf_less(r.best.label32, r.best.index, best.label32, best.index))) best = r.best;
     }
     out->files_checked = full ? last + 1 - o->from_file : 0;
     for (size_t g = 0; g < G && !full; g++) out->files_checked += res[g].files;
@@ -361,12 +350,9 @@ int b200post_verify_pos(const char *data_dir, const b200post_verify_pos_opts *o,
 
     // ---- the VRF nonce: its label recomputed and compared with NonceValue; for a whole-POST check also the arg-min
     if (md.has_nonce) {
-        uint8_t all[32];
-        memset(all, 0xff, 32);
-        VrfResult nv;
-        if ((rc = engines[0]->labels_range(commitment, N, md.nonce, 1, nullptr, nullptr, all, &nv, nullptr))) return rc;
-        if (!nv.found) memset(nv.label32, 0xff, 32);   // found is 0 only for the all-ones label
-        out->nonce_ok = memcmp(nv.label32, md.nonce_value, 32) == 0;
+        uint8_t l32[32];
+        if ((rc = label32_at(engines[0], commitment, N, md.nonce, l32))) return rc;
+        out->nonce_ok = memcmp(l32, md.nonce_value, 32) == 0;
     }
     if (whole && md.has_nonce) {
         out->argmin_checked = 1;

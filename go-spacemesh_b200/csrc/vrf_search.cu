@@ -231,8 +231,8 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     // ---- device: the scan runs on one (it is bound by storage, not by the GPU)
     std::vector<uint32_t> devs;
     if (int rc = provider_devices(o.provider_id, &devs)) return rc;
-    DeviceEngine *e = engine_for(devs[0]);
-    if (!e) return B200POST_ERR_NO_DEVICE;
+    DeviceEngine *e;
+    if (int rc = device_engine(devs[0], &e)) return rc;
     chunk = std::min(chunk, num_labels);
 
     Running best;
@@ -276,18 +276,16 @@ int stored_vrf_search(const std::string &dir, b200post_post_metadata *md, const 
     for (int j = 0; j < 8; j++) { prefix[j] = (uint8_t)(best.hi >> (56 - 8 * j)); prefix[8 + j] = (uint8_t)(best.lo >> (56 - 8 * j)); }
     std::vector<uint64_t> pos{best.index};
     if (best.next != ~0ull) pos.push_back(best.next);
-    uint8_t commitment[32], all[32], best32[32];
+    uint8_t commitment[32], best32[32];
     commitment_bytes(md->node_id, md->commitment_atx_id, commitment);
-    memset(all, 0xff, 32);
     uint64_t best_index = 0;
     for (size_t j = 0; j < pos.size(); j++) {
-        VrfResult vr;
-        if (int rc = e->labels_range(commitment, N, pos[j], 1, nullptr, nullptr, all, &vr, nullptr)) return rc;
-        if (!vr.found) memset(vr.label32, 0xff, 32);   // found is 0 only for the all-ones label
-        if (memcmp(vr.label32, prefix, 16))
+        uint8_t l32[32];
+        if (int rc = label32_at(e, commitment, N, pos[j], l32)) return rc;
+        if (memcmp(l32, prefix, 16))
             return fail(B200POST_ERR_LABEL_MISMATCH, "the stored label at index " + std::to_string(pos[j]) +
                                                          " differs from its recomputation: the POST data is damaged");
-        if (j == 0 || memcmp(vr.label32, best32, 32) < 0) { memcpy(best32, vr.label32, 32); best_index = pos[j]; }
+        if (j == 0 || memcmp(l32, best32, 32) < 0) { memcpy(best32, l32, 32); best_index = pos[j]; }
     }
     if (best.n_ties > pos.size())
         return fail(B200POST_ERR_LABEL_MISMATCH, std::to_string(best.n_ties) + " stored labels share the smallest 16-byte prefix: the POST data is damaged");
