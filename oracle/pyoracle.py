@@ -393,17 +393,22 @@ def py_label_passes(label16: bytes, challenge: bytes, nonce: int, pow_: int, dif
     return (int.from_bytes(out[:8], "little") & ((1 << 56) - 1)) < (difficulty & ((1 << 56) - 1))
 
 
-def py_subset_positions(values, seed: bytes, nonce: int, packed: bytes, pow_: int, k3: int, with_positions: bool = False):
+def py_subset_positions(values, seed: bytes, nonce: int, packed: bytes, pow_: int, k3: int, with_positions: bool = False,
+                        stream_bytes: int = 256):
     """RandomValuesIterator: BLAKE3-XOF driven partial Fisher-Yates; returns the first k3 selected values
-    (with_positions: pairs (value, position in `values`))."""
+    (with_positions: pairs (value, position in `values`)).  The XOF stream starts at `stream_bytes` and doubles
+    whenever the next draw would run past its end, so any number of draws reads real stream bytes."""
     import blake3
-    stream = blake3.blake3(seed + nonce.to_bytes(4, "little") + packed + pow_.to_bytes(8, "little")).digest(8192)
+    xof = blake3.blake3(seed + nonce.to_bytes(4, "little") + packed + pow_.to_bytes(8, "little"))
+    stream = xof.digest(stream_bytes)
     vals, pos, out, idx = list(values), 0, [], 0
     where = list(range(len(vals)))
     while len(out) < min(k3, len(vals)):
         remaining = len(vals) - idx
         max_allowed = 0xFFFF - 0xFFFF % remaining
         while True:
+            while pos + 2 > len(stream):
+                stream = xof.digest(max(2 * len(stream), 2))
             r = int.from_bytes(stream[pos:pos + 2], "little")
             pos += 2
             if r < max_allowed:

@@ -209,6 +209,45 @@ def test_vectorised_prove_oracle_matches_scalar(orc, regime):
         assert exp_hits == [0] and sum(1 for h in hits.values() if list(h) == [0]) > 1
 
 
+def _plain_subset(values, msg: bytes, stream_len: int):
+    """Partial Fisher-Yates over one fixed XOF stream, read with bounds checks: the whole shuffle, and the bytes used."""
+    import blake3
+    stream = blake3.blake3(msg).digest(stream_len)
+    vals, where, pos, out = list(values), list(range(len(values))), 0, []
+    for idx in range(len(vals)):
+        remaining = len(vals) - idx
+        while True:
+            assert pos + 2 <= len(stream), "fixed reference stream too short"
+            r = int.from_bytes(stream[pos:pos + 2], "little")
+            pos += 2
+            if r < 0xFFFF - 0xFFFF % remaining:
+                break
+        j = idx + r % remaining
+        vals[idx], vals[j] = vals[j], vals[idx]
+        where[idx], where[j] = where[j], where[idx]
+        out.append((vals[idx], where[idx]))
+    return out, pos
+
+
+def test_subset_positions_grow_the_stream(orc):
+    """Subset selection with up to k2 = 65535 draws: the stream py_subset_positions grows on demand gives the same
+    selections as one drawn 64 KiB up front and as a plain shuffle over a fixed 1 MiB stream, every prefix of the
+    selection order is the selection for a smaller k3, and no position is selected twice."""
+    rng = np.random.default_rng(41)
+    k2 = 65535
+    values = [int(v) for v in rng.integers(0, 2**34, k2)]
+    seed, nonce, packed, pow_ = b"peer", 77, bytes(rng.integers(0, 256, 40, dtype=np.uint8)), 2**50 + 9
+    full = orc.py_subset_positions(values, seed, nonce, packed, pow_, k2, with_positions=True)
+    assert len(full) == k2 and len({w for _, w in full}) == k2
+    assert all(values[w] == v for v, w in full)
+    assert orc.py_subset_positions(values, seed, nonce, packed, pow_, k2, with_positions=True, stream_bytes=1 << 16) == full
+    plain, used = _plain_subset(values, seed + nonce.to_bytes(4, "little") + packed + pow_.to_bytes(8, "little"), 1 << 20)
+    assert plain == full
+    assert used > 2 * 8192          # well past the fixed 8 KiB stream the oracle used to stop at
+    for k in (1, 127, 128, 129, 300, 4095, 4096, 4097, 20000, 40000, 65534):
+        assert orc.py_subset_positions(values, seed, nonce, packed, pow_, k, with_positions=True) == full[:k], k
+
+
 def test_simd_and_scalar_romix_agree(orc):
     """The vectorised ROMix paths used for the timed CPU baseline (1 = SSE2, 2 = AVX2 with two labels per thread in
     lock-step, 3 = AVX-512 with four, where the CPU has it) are the same function as the scalar restatement, ragged
