@@ -2,11 +2,14 @@
 #include <algorithm>
 #include <atomic>
 #include <cstring>
+#include <functional>
+#include <mutex>
 #include <string>
 #include <vector>
 
 #include "../../include/b200post_k2pow.h"
 #include "engine.h"
+#include "k2pow_jobs.h"
 #include "proof_common.h"
 #include "randomx_engine.h"
 
@@ -36,39 +39,67 @@ bool clamp_range(uint64_t start, uint64_t &count) {
     return true;
 }
 
-// One window of the prover's search: pows [next, next + per) of every group in `groups`, in one device call.  hit[i] =
-// the smallest valid pow of groups[i] in the window, or B200POST_K2POW_NOT_FOUND.
-int search_window(RandomxEngine *e, const std::string &key, const b200post_k2pow_params *p, const std::vector<uint32_t> &groups,
-                  uint64_t next, uint64_t per, std::vector<uint8_t> &in, std::vector<uint8_t> &out, std::vector<uint64_t> &hit) {
-    const size_t n = groups.size() * per;
-    in.resize(n * 48); out.resize(n * 32);
-    for (size_t gi = 0; gi < groups.size(); gi++)
-        for (uint64_t k = 0; k < per; k++) {
-            uint8_t *d = &in[(gi * per + k) * 48];
-            const uint64_t pow = next + k;
-            for (int b = 0; b < 7; b++) d[b] = (uint8_t)(pow >> (8 * b));
-            d[7] = (uint8_t)groups[gi];
-            memcpy(d + 8, p->challenge8, 8);
-            memcpy(d + 16, p->node_id, 32);
-        }
-    const int rc = e->hash_inputs(key, in.data(), 48, n, out.data());
-    if (rc != B200POST_OK) return rc;
-    hit.assign(groups.size(), B200POST_K2POW_NOT_FOUND);
-    for (size_t gi = 0; gi < groups.size(); gi++)
-        for (uint64_t k = 0; k < per && hit[gi] == B200POST_K2POW_NOT_FOUND; k++)
-            if (memcmp(&out[(gi * per + k) * 32], p->difficulty, 32) < 0) hit[gi] = next + k;
-    return B200POST_OK;
-}
-
-// randomx_engine of every entry in list order; the first failing entry's code (and text) answers
-int randomx_engines(const uint32_t *providers, int n, std::vector<RandomxEngine *> *out) {
-    out->assign((size_t)n, nullptr);
-    for (int i = 0; i < n; i++)
-        if (int rc = randomx_engine(providers[i], &(*out)[(size_t)i])) return rc;
-    return B200POST_OK;
+// The jobs of groups first_group .. first_group + n_groups - 1 of one identity (p->nonce_group is not used)
+std::vector<K2powJob> group_jobs(const b200post_k2pow_params *p, uint32_t first_group, uint32_t n_groups) {
+    std::vector<K2powJob> jobs(n_groups);
+    for (uint32_t g = 0; g < n_groups; g++) {
+        rx::K2powTemplate t = template_of(p);
+        t.tail[0] = (uint8_t)(first_group + g);   // the absolute group number is the k2pow input's group byte
+        memcpy(jobs[g].tail, t.tail, 41);
+        memcpy(jobs[g].difficulty, p->difficulty, 32);
+    }
+    return jobs;
 }
 
 }  // namespace
+
+namespace b200post {
+
+int k2pow_search_jobs(const std::vector<RandomxEngine *> &eng, const std::string &key, const std::vector<K2powJob> &jobs, uint64_t cap,
+                      uint64_t *pows, uint64_t *hashes_done, const volatile int *cancel, const std::function<void(uint32_t, uint64_t)> &on_final) {
+    JobSchedule sched(jobs.size(), cap);
+    std::mutex mu;                     // guards sched and orders the on_final calls
+    std::atomic<bool> stop{false};
+    for (RandomxEngine *e : eng) e->reset_timing();
+    const auto report = [&](const std::vector<uint32_t> &done) { if (on_final) for (uint32_t j : done) on_final(j, sched.pow(j)); };
+    const auto part = [&](size_t i) -> int {
+        uint64_t batch = 0;
+        eng[i]->batch_size(&batch);
+        JobSchedule::Window w;
+        std::vector<uint64_t> hits;
+        std::vector<uint32_t> slot;
+        while (!stop) {
+            if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
+            {
+                std::lock_guard<std::mutex> lk(mu);
+                if (!sched.take(batch, &w)) { report(sched.settle()); break; }
+            }
+            hits.assign(w.jobs.size(), B200POST_K2POW_NOT_FOUND);
+            for (const std::vector<JobSegment> &segs : JobSchedule::batches(w, batch)) {
+                slot.resize(segs.size());
+                if (int rc = eng[i]->search_segments(key, jobs.data(), jobs.size(), segs.data(), segs.size(), slot.data())) return rc;
+                for (size_t s = 0; s < segs.size(); s++) {
+                    if (slot[s] == 0xffffffffu) continue;
+                    const size_t k = (size_t)(std::lower_bound(w.jobs.begin(), w.jobs.end(), segs[s].job) - w.jobs.begin());
+                    hits[k] = std::min(hits[k], segs[s].first_pow + slot[s]);
+                }
+            }
+            std::lock_guard<std::mutex> lk(mu);
+            report(sched.finish(w, hits));
+        }
+        return B200POST_OK;
+    };
+    const int rc = eng.size() == 1 ? part(0) : fan_out(eng.size(), [&](size_t i) {
+        const int r = part(i);
+        if (r != B200POST_OK) stop = true;
+        return r;
+    });
+    for (size_t j = 0; j < jobs.size(); j++) pows[j] = sched.final(j) ? sched.pow(j) : B200POST_K2POW_NOT_FOUND;
+    if (hashes_done) *hashes_done = sched.hashes();
+    return rc;
+}
+
+}  // namespace b200post
 
 extern "C" {
 
@@ -158,31 +189,8 @@ int b200post_k2pow_search_group_range(uint32_t provider, const b200post_k2pow_pa
     if (!p || !pows || n_groups == 0 || (uint64_t)first_group + n_groups > 256) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     RandomxEngine *e;
     if (int rc = randomx_engine(provider, &e)) return rc;
-    const std::string key = key_of(p->cache_key, p->cache_key_len);
-    uint64_t batch = 0;
-    e->batch_size(&batch);
-    for (uint32_t g = 0; g < n_groups; g++) pows[g] = B200POST_K2POW_NOT_FOUND;
-    if (max_nonces_per_group == 0 || max_nonces_per_group > kNonceSpace) max_nonces_per_group = kNonceSpace;
-    std::vector<uint32_t> pending(n_groups);   // absolute group numbers: they are the k2pow input's group byte
-    for (uint32_t g = 0; g < n_groups; g++) pending[g] = first_group + g;
-    std::vector<uint8_t> in, out;
-    std::vector<uint64_t> hit;
-    uint64_t next = 0, total = 0;      // every pending group has tried nonces [0, next)
-    while (!pending.empty() && next < max_nonces_per_group) {
-        if (cancel && *cancel) { set_error("cancelled"); return B200POST_ERR_CANCELLED; }
-        // one device batch shared by all groups still searching: `per` consecutive nonces each
-        const uint64_t per = std::min<uint64_t>(std::max<uint64_t>(1, batch / pending.size()), max_nonces_per_group - next);
-        const int rc = search_window(e, key, p, pending, next, per, in, out, hit);
-        if (rc != B200POST_OK) return rc;
-        total += pending.size() * per;
-        std::vector<uint32_t> still;
-        for (size_t gi = 0; gi < pending.size(); gi++)
-            if (hit[gi] == B200POST_K2POW_NOT_FOUND) still.push_back(pending[gi]); else pows[pending[gi] - first_group] = hit[gi];
-        pending.swap(still);
-        next += per;
-    }
-    if (hashes_done) *hashes_done = total;
-    return B200POST_OK;
+    return k2pow_search_jobs({e}, key_of(p->cache_key, p->cache_key_len), group_jobs(p, first_group, n_groups), max_nonces_per_group, pows,
+                             hashes_done, cancel);
 }
 
 int b200post_k2pow_search_groups_multi(const uint32_t *providers, int n_providers, const b200post_k2pow_params *p,
@@ -201,48 +209,24 @@ int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_pro
     if (n_providers == 1) return b200post_k2pow_search_group_range(providers[0], p, first_group, n_groups, max_nonces_per_group, pows, hashes_done, cancel);
     std::vector<RandomxEngine *> eng;
     if (int rc = randomx_engines(providers, n_providers, &eng)) return rc;
-    for (uint32_t g = 0; g < n_groups; g++) pows[g] = B200POST_K2POW_NOT_FOUND;
-    const std::string key = key_of(p->cache_key, p->cache_key_len);
-    const uint64_t cap = max_nonces_per_group == 0 || max_nonces_per_group > kNonceSpace ? kNonceSpace : max_nonces_per_group;
-    // Windows go out in ascending nonce order from one cursor, each to every group without a hit yet.  So every group
-    // has been handed out the contiguous nonces [0, cursor at its first reported hit), and once all threads have
-    // joined, the smallest hit reported for it is its smallest valid pow.
-    std::mutex mu;
-    uint64_t next = 0, total = 0;
-    std::vector<uint64_t> best(n_groups, B200POST_K2POW_NOT_FOUND);
-    std::atomic<bool> stop{false};
-    const int rc = fan_out((size_t)n_providers, [&](size_t i) {
-        uint64_t batch = 0;
-        eng[i]->batch_size(&batch);
-        std::vector<uint8_t> in, out;
-        std::vector<uint64_t> hit;
-        std::vector<uint32_t> groups;
-        int r = B200POST_OK;
-        while (!stop) {
-            if (cancel && *cancel) { set_error("cancelled"); r = B200POST_ERR_CANCELLED; break; }
-            uint64_t lo, per;
-            {
-                std::lock_guard<std::mutex> lk(mu);
-                groups.clear();
-                for (uint32_t g = 0; g < n_groups; g++) if (best[g] == B200POST_K2POW_NOT_FOUND) groups.push_back(first_group + g);
-                if (groups.empty() || next >= cap) break;
-                // one device batch: `per` consecutive nonces for each group still searching, as on one device
-                per = std::min<uint64_t>(std::max<uint64_t>(1, batch / groups.size()), cap - next);
-                lo = next;
-                next += per;
-            }
-            if ((r = search_window(eng[i], key, p, groups, lo, per, in, out, hit)) != B200POST_OK) break;
-            std::lock_guard<std::mutex> lk(mu);
-            total += groups.size() * per;
-            for (size_t gi = 0; gi < groups.size(); gi++) best[groups[gi] - first_group] = std::min(best[groups[gi] - first_group], hit[gi]);
-        }
-        if (r != B200POST_OK) stop = true;
-        return r;
-    });
-    if (hashes_done) *hashes_done = total;
-    if (rc) return rc;
-    for (uint32_t g = 0; g < n_groups; g++) pows[g] = best[g];
-    return B200POST_OK;
+    return k2pow_search_jobs(eng, key_of(p->cache_key, p->cache_key_len), group_jobs(p, first_group, n_groups), max_nonces_per_group, pows,
+                             hashes_done, cancel);
+}
+
+int b200post_k2pow_search_jobs(const uint32_t *providers, int n_providers, const uint8_t *cache_key, size_t cache_key_len,
+                               size_t n_jobs, const b200post_k2pow_job *jobs, uint64_t max_nonces_per_job, uint64_t *pows,
+                               uint64_t *hashes_done, const volatile int *cancel) {
+    if (!providers || n_providers <= 0 || n_jobs == 0 || !jobs || !pows) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::vector<RandomxEngine *> eng;
+    if (int rc = randomx_engines(providers, n_providers, &eng)) return rc;
+    std::vector<K2powJob> table(n_jobs);
+    for (size_t j = 0; j < n_jobs; j++) {
+        table[j].tail[0] = jobs[j].nonce_group;
+        memcpy(table[j].tail + 1, jobs[j].challenge8, 8);
+        memcpy(table[j].tail + 9, jobs[j].node_id, 32);
+        memcpy(table[j].difficulty, jobs[j].difficulty, 32);
+    }
+    return k2pow_search_jobs(eng, key_of(cache_key, cache_key_len), table, max_nonces_per_job, pows, hashes_done, cancel);
 }
 
 int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uint64_t pow, int *valid) {

@@ -6,6 +6,7 @@
 
 #include <cstdint>
 #include <mutex>
+#include <string>
 #include <vector>
 
 #include "../../include/b200post_prove.h"
@@ -85,5 +86,9 @@ int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const u
 // rejection clears *out and returns B200POST_ERR_INVALID_PROOF with the verifier's reason.
 int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o,
                const b200post_proof_metadata &meta, b200post_proof_out *out);
+// The same gate over n proofs of one scrypt N in one b200post_verify_batch call: rcs[i] / errs[i] are proof i's code and
+// text (a failure of the call itself is every proof's), and a rejected proof's *outs[i] is cleared.
+void gate_proofs(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o, size_t n,
+                 const b200post_proof_metadata *metas, b200post_proof_out *const *outs, int *rcs, std::string *errs);
 
 }  // namespace b200post

@@ -16,11 +16,18 @@
 // Nonce windows (b200post_prove_opts.max_windows): generate() runs passes over the data, each scanning windows_per_pass
 // windows of nonces with their own pows, until a window has a proof; the kernels only ever see pass-relative nonces.
 //
+// Several identities (b200post_generate_proofs): prove_items runs every identity's pass loop; the pows of all identities
+// waiting for a pass come from one k2pow job search, and each identity's scan starts as soon as its pows are final.  The
+// single calls are its one-item case.
+//
 // The scanner, the proof record, the pow step and the verifier gate are declared in prove_internal.h: the setup
 // session's initial proof (initial_proof.cu) runs the same scan over the labels as it writes them.
 #include <algorithm>
 #include <atomic>
+#include <condition_variable>
+#include <cstdio>
 #include <functional>
+#include <map>
 #include <memory>
 #include <mutex>
 #include <set>
@@ -36,6 +43,7 @@
 #include "postdata_io.h"
 #include "proof_common.h"
 #include "prove_internal.h"
+#include "randomx_engine.h"
 
 namespace b200post {
 namespace {
@@ -415,25 +423,36 @@ int find_pows(const b200post_prove_opts &o, const uint8_t challenge[32], const u
     return B200POST_OK;
 }
 
-int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o,
-               const b200post_proof_metadata &meta, b200post_proof_out *out) {
+void gate_proofs(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o, size_t n,
+                 const b200post_proof_metadata *metas, b200post_proof_out *const *outs, int *rcs, std::string *errs) {
     b200post_verify_params vp{};
     vp.k1 = cfg.k1; vp.k2 = cfg.k2; vp.scrypt_n = scrypt_n;
     memcpy(vp.pow_difficulty, cfg.pow_difficulty, 32);
     b200post_verifier_opts vo{};
     vo.pow_mode = o.pow_mode == B200POST_POW_BUILTIN ? B200POST_POW_BUILTIN : B200POST_POW_SKIP;
     vo.pow_cache_key = o.pow_cache_key; vo.pow_cache_key_len = o.pow_cache_key_len;
-    const b200post_proof proof{out->nonce, out->indices, out->indices_len, out->pow};
-    int status = B200POST_OK;
-    uint64_t bad = 0;
-    const int rc = b200post_verify_batch(provider, 1, &proof, &meta, &vp, nullptr, &vo, &status, &bad);
-    if (rc) return rc;
-    if (status != B200POST_OK) {
-        memset(out, 0, sizeof *out);
-        set_error(bad == ~0ull ? "the proof failed the verifier's k2pow check" : "the proof failed the verifier at position " + std::to_string(bad));
-        return B200POST_ERR_INVALID_PROOF;
+    std::vector<b200post_proof> proofs(n);
+    for (size_t i = 0; i < n; i++) proofs[i] = b200post_proof{outs[i]->nonce, outs[i]->indices, outs[i]->indices_len, outs[i]->pow};
+    std::vector<int> status(n, B200POST_OK);
+    std::vector<uint64_t> bad(n, 0);
+    const int rc = b200post_verify_batch(provider, n, proofs.data(), metas, &vp, nullptr, &vo, status.data(), bad.data());
+    for (size_t i = 0; i < n; i++) {
+        rcs[i] = rc ? rc : status[i] != B200POST_OK ? B200POST_ERR_INVALID_PROOF : B200POST_OK;
+        if (rc) errs[i] = last_error();
+        else if (status[i] != B200POST_OK) {
+            memset(outs[i], 0, sizeof *outs[i]);
+            errs[i] = bad[i] == ~0ull ? "the proof failed the verifier's k2pow check" : "the proof failed the verifier at position " + std::to_string(bad[i]);
+        }
     }
-    return B200POST_OK;
+}
+
+int gate_proof(uint32_t provider, const b200post_post_config &cfg, uint64_t scrypt_n, const b200post_prove_opts &o,
+               const b200post_proof_metadata &meta, b200post_proof_out *out) {
+    int rc = B200POST_OK;
+    std::string err;
+    gate_proofs(provider, cfg, scrypt_n, o, 1, &meta, &out, &rc, &err);
+    if (rc) set_error(err);
+    return rc;
 }
 
 }  // namespace b200post
@@ -458,9 +477,257 @@ void parallel_copy(uint8_t *dst, const uint8_t *src, size_t bytes) {
 }  // namespace
 
 namespace {
+
+// One identity's proof in progress: its host checks' results and what the pass loop keeps between passes.  out, meta_out
+// and check are the caller's (check is set for a checked proof).
+struct ItemProof {
+    const char *data_dir = nullptr;
+    const uint8_t *challenge = nullptr;
+    b200post_proof_out *out = nullptr;
+    b200post_proof_metadata *meta_out = nullptr;
+    b200post_prove_check *check = nullptr;
+    b200post_post_metadata md{};
+    uint64_t num_labels = 0, per_file = 0, chunk = 0;
+    uint32_t n = 0, windows = 0, per_pass = 0;
+    std::vector<std::pair<uint64_t, uint64_t>> ranges;
+    uint8_t commitment[32] = {0};
+    uint32_t a = 0;                    // the next pass starts at window a
+    uint64_t scanned = 0;              // over every pass
+    std::set<uint64_t> damaged;        // the checked report's, over every pass
+    bool have = false;
+    std::vector<uint64_t> pows;        // the current pass's, one per nonce group
+    b200post_proof_metadata meta{};
+    int status = B200POST_OK;          // the single call's code and text once `done`
+    std::string error;
+    bool done = false;
+
+    uint32_t pass_windows() const { return std::min(per_pass, windows - a); }
+    uint32_t first_group() const { return a * n / 16; }
+    uint32_t groups() const { return pass_windows() * n / 16; }
+    void finish(int rc, const std::string &err) { status = rc; error = rc ? err : std::string(); done = true; }
+};
+
+// The host checks of one proof, in the single call's order: metadata, nonce count, scrypt N (checked), pow mode,
+// MaxFileSize.  Then the pass plan.
+int open_item(ItemProof &it, const b200post_prove_opts &o, int n_providers) {
+    int rc = b200post_load_metadata(it.data_dir, &it.md);
+    if (rc) return rc;
+    const b200post_post_metadata &md = it.md;
+    it.num_labels = (uint64_t)md.num_units * md.labels_per_unit;
+    if (it.num_labels == 0 || o.nonces % 16 || o.nonces > 4096) { set_error("invalid metadata or nonce count"); return B200POST_ERR_INVALID_ARGUMENT; }
+    if (it.check && (md.scrypt_n < 2 || md.scrypt_n > (1ull << 20) || (md.scrypt_n & (md.scrypt_n - 1)))) {
+        set_error("corrupt metadata: Scrypt.N out of range");
+        return B200POST_ERR_IO;
+    }
+    if ((rc = check_pow_mode(o))) return rc;
+    it.per_file = md.max_file_size / 16;
+    if (it.per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
+    // the nonce windows [w*n, (w+1)*n) to try, `per_pass` of them per read of the data (b200post_prove_opts)
+    it.n = o.nonces;
+    it.windows = std::min(std::max(o.max_windows, 1u), 4096 / it.n);
+    it.per_pass = std::max(o.windows_per_pass, 1u);
+    it.chunk = std::min<uint64_t>(o.chunk_labels, it.num_labels);
+    it.ranges = split_shards(it.num_labels, it.chunk, (size_t)n_providers);
+    if (it.check) commitment_bytes(md.node_id, md.commitment_atx_id, it.commitment);
+    return B200POST_OK;
+}
+
+// One pass of an item with its pows found: the scan of windows [a, a + m), its rule's decision and the checked report.
+// Marks the item done when it has a proof (before the gate) or no window is left.
+int scan_pass(ItemProof &it, const b200post_post_config &cfg, const uint32_t *providers, int n_providers, const volatile int *cancel) {
+    const uint32_t m = it.pass_windows(), first = it.a * it.n;
+    // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
+    ShardedScan scan(it.ranges, first, it.n, m, cfg.k2, it.check ? it.commitment : nullptr, it.md.scrypt_n, cancel);
+    int rc;
+    for (int s = 0; s < n_providers; s++)
+        if ((rc = scan.scanner((size_t)s).init(providers[s], it.challenge, m * it.n, it.pows.data(), cfg.k1, cfg.k2, it.num_labels, it.chunk,
+                                               it.check != nullptr, first)))
+            return rc;
+    std::vector<std::unique_ptr<PostDataReader>> readers;
+    for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(it.data_dir, it.per_file));
+    rc = scan.run([&](size_t s, uint64_t pos, uint64_t cnt, uint8_t *dst) { return readers[s]->read(pos, cnt, dst); }, it.chunk, 0, cancel);
+    if (rc) return rc;
+    metrics().prove_passes_total++;
+    ProveRule &rule = scan.rule();
+    it.scanned += rule.scanned();
+    uint32_t nonce = 0;
+    std::vector<uint64_t> idx;
+    it.have = rule.decide(&nonce, &idx, &rc);
+    if (b200post_prove_check *check = it.check) {   // the report adds up over the passes (`damaged`: every distinct damaged index so far)
+        const size_t before = it.damaged.size();
+        it.damaged.insert(rule.damaged().begin(), rule.damaged().end());
+        check->labels_rechecked += rule.rechecked(); check->rounds += rule.rounds(); check->damaged = it.damaged.size();
+        check->n_reported = 0;
+        for (uint64_t i : it.damaged) {   // ascending
+            if (check->n_reported == 64) break;
+            check->damaged_index[check->n_reported++] = i;
+        }
+        metrics().prove_labels_rechecked_total += rule.rechecked();
+        metrics().prove_damaged_labels_total += it.damaged.size() - before;
+    }
+    if (rc) return rc;
+    if (it.have && (rc = write_proof(it.scanned, nonce, idx, it.pows.data(), first, it.num_labels, it.out))) return rc;
+    it.a += m;
+    if (!it.have && it.a < it.windows) return B200POST_OK;   // another pass
+    if (!it.have) return no_proof(it.windows, it.n);
+    memcpy(it.meta.node_id, it.md.node_id, 32);
+    memcpy(it.meta.commitment_atx_id, it.md.commitment_atx_id, 32);
+    memcpy(it.meta.challenge, it.challenge, 32);
+    it.meta.num_units = it.md.num_units; it.meta.labels_per_unit = it.md.labels_per_unit;
+    it.done = true;
+    return B200POST_OK;
+}
+
+// The pass loop of every item (b200post_generate_proofs; the single calls are its one-item case).  The pows of every
+// item waiting for a pass go into one search (BUILTIN: one k2pow job search over the devices; CALLBACK / SKIP: per item
+// on this thread).  An item's scan starts on one of the scan threads as soon as its pows are final, while the search
+// goes on for the others, and an item that needs another pass joins the next search.  Checked proofs then pass the
+// verifier gate together.  Each item ends with its single call's status and text; the return value is the call's own:
+// UNSUPPORTED for the pow mode, NO_DEVICE / UNSUPPORTED of the device list, CANCELLED, else OK.
+int prove_items(std::vector<ItemProof> &items, const b200post_post_config &cfg, const b200post_prove_opts &o, const uint32_t *providers,
+                int n_providers, uint32_t parallel_scans, const volatile int *cancel) {
+    for (ItemProof &it : items)
+        if (int rc = open_item(it, o, n_providers)) it.finish(rc, last_error());
+    if (int rc = check_pow_mode(o)) return rc;   // every item that got this far answers the same
+    std::mutex mu;                               // guards everything below and every item's done / status
+    std::condition_variable cv;
+    std::vector<size_t> waiting, ready;          // items needing the pows of their next pass; items to scan
+    size_t left = 0;                             // items not done
+    for (size_t i = 0; i < items.size(); i++) if (!items[i].done) { waiting.push_back(i); left++; }
+    const auto end_item = [&](size_t i, int rc, const std::string &err) {   // under mu
+        items[i].finish(rc, err);
+        left--;
+        cv.notify_all();
+    };
+    const auto scan_loop = [&] {
+        std::unique_lock<std::mutex> lk(mu);
+        for (;;) {
+            cv.wait(lk, [&] { return !ready.empty() || left == 0; });
+            if (ready.empty()) return;
+            const size_t i = ready.front();
+            ready.erase(ready.begin());
+            lk.unlock();
+            const int rc = scan_pass(items[i], cfg, providers, n_providers, cancel);
+            const std::string err = rc ? last_error() : std::string();
+            lk.lock();
+            if (rc || items[i].done) end_item(i, rc, err);
+            else { waiting.push_back(i); cv.notify_all(); }
+        }
+    };
+    std::vector<std::thread> scanners;
+    int call_rc = B200POST_OK;
+    bool devices_checked = false;
+    std::unique_lock<std::mutex> lk(mu);
+    while (left) {
+        cv.wait(lk, [&] { return !waiting.empty() || left == 0; });
+        if (!left) break;
+        std::vector<size_t> batch;
+        batch.swap(waiting);
+        std::sort(batch.begin(), batch.end());
+        lk.unlock();
+        std::vector<int> rcs(batch.size(), B200POST_OK);
+        std::vector<std::string> errs(batch.size());
+        std::vector<bool> handed(batch.size(), false);   // pows final: the item went to `ready`
+        // the single call's pow step for the items without BUILTIN: their hooks, before any device is touched
+        if (o.pow_mode != B200POST_POW_BUILTIN)
+            for (size_t b = 0; b < batch.size(); b++) {
+                ItemProof &it = items[batch[b]];
+                if ((rcs[b] = find_pows(o, it.challenge, it.md.node_id, it.md.num_units, cfg.pow_difficulty, providers, n_providers,
+                                        it.first_group(), it.groups(), &it.pows, cancel)))
+                    errs[b] = last_error();
+            }
+        // the devices answer once, where the single call first touches them: the search (BUILTIN) or the first scan
+        int rc = B200POST_OK;
+        std::vector<RandomxEngine *> eng;
+        if (!devices_checked) {
+            devices_checked = true;
+            if (o.pow_mode == B200POST_POW_BUILTIN) rc = randomx_engines(providers, n_providers, &eng);
+            if (!rc) rc = device_engines(providers, n_providers);
+            if (rc) call_rc = rc;
+            else for (size_t t = std::min<size_t>(left, parallel_scans ? parallel_scans : 4); t; t--) scanners.emplace_back(scan_loop);
+        }
+        if (!rc && o.pow_mode == B200POST_POW_BUILTIN) {
+            // one job search over the pass's nonce groups of every item in the batch
+            std::vector<K2powJob> jobs;
+            std::vector<size_t> owner, first_job(batch.size()), unfinal(batch.size());
+            for (size_t b = 0; b < batch.size(); b++) {
+                ItemProof &it = items[batch[b]];
+                uint8_t scaled[32];
+                div256_u32(cfg.pow_difficulty, it.md.num_units, scaled);
+                first_job[b] = jobs.size();
+                unfinal[b] = it.groups();
+                it.pows.assign(it.groups(), B200POST_K2POW_NOT_FOUND);
+                for (uint32_t g = 0; g < it.groups(); g++) {
+                    K2powJob j;
+                    j.tail[0] = (uint8_t)(it.first_group() + g);
+                    memcpy(j.tail + 1, it.challenge, 8);
+                    memcpy(j.tail + 9, it.md.node_id, 32);
+                    memcpy(j.difficulty, scaled, 32);
+                    jobs.push_back(j);
+                    owner.push_back(b);
+                }
+            }
+            if (eng.empty()) randomx_engines(providers, n_providers, &eng);
+            const std::string key = o.pow_cache_key ? std::string(reinterpret_cast<const char *>(o.pow_cache_key), o.pow_cache_key_len)
+                                                    : std::string(B200POST_K2POW_DEFAULT_KEY);
+            std::vector<uint64_t> pows(jobs.size());
+            rc = k2pow_search_jobs(eng, key, jobs, 0, pows.data(), nullptr, cancel, [&](uint32_t j, uint64_t pow) {
+                const size_t b = owner[j];
+                ItemProof &it = items[batch[b]];
+                it.pows[j - first_job[b]] = pow;
+                if (--unfinal[b]) return;
+                std::lock_guard<std::mutex> g(mu);
+                handed[b] = true;
+                if (std::find(it.pows.begin(), it.pows.end(), B200POST_K2POW_NOT_FOUND) != it.pows.end()) {
+                    end_item(batch[b], B200POST_ERR_INVALID_PROOF, "k2pow: nonce space exhausted");
+                    return;
+                }
+                ready.push_back(batch[b]);
+                cv.notify_all();
+            });
+        }
+        const std::string err = rc ? last_error() : std::string();
+        lk.lock();
+        for (size_t b = 0; b < batch.size(); b++) {
+            if (handed[b]) continue;
+            if (rcs[b]) end_item(batch[b], rcs[b], errs[b]);       // its hook failed
+            else if (rc) end_item(batch[b], rc, err);              // the devices or the search failed before its pows were final
+            else { ready.push_back(batch[b]); cv.notify_all(); }   // CALLBACK / SKIP pows
+        }
+    }
+    lk.unlock();
+    for (std::thread &t : scanners) t.join();
+    // the gate: the checked proofs of each scrypt N in one b200post_verify_batch call on the first device
+    std::map<uint64_t, std::vector<size_t>> gate;
+    for (size_t i = 0; i < items.size(); i++)
+        if (items[i].status == B200POST_OK && items[i].check) gate[items[i].md.scrypt_n].push_back(i);
+    for (const auto &kv : gate) {
+        const size_t k = kv.second.size();
+        std::vector<b200post_proof_metadata> metas(k);
+        std::vector<b200post_proof_out *> outs(k);
+        std::vector<int> rcs(k);
+        std::vector<std::string> errs(k);
+        for (size_t g = 0; g < k; g++) { metas[g] = items[kv.second[g]].meta; outs[g] = items[kv.second[g]].out; }
+        gate_proofs(providers[0], cfg, kv.first, o, k, metas.data(), outs.data(), rcs.data(), errs.data());
+        for (size_t g = 0; g < k; g++) {
+            ItemProof &it = items[kv.second[g]];
+            if (rcs[g]) it.finish(rcs[g], errs[g]);
+            else it.check->proof_verified = 1;
+        }
+    }
+    for (ItemProof &it : items) {
+        if (it.status == B200POST_OK && it.meta_out) *it.meta_out = it.meta;
+        if (it.status == B200POST_ERR_CANCELLED && !call_rc) call_rc = B200POST_ERR_CANCELLED;
+    }
+    if (call_rc == B200POST_ERR_CANCELLED) set_error("cancelled");
+    return call_rc;
+}
+
 int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
              const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
              b200post_prove_check *check, const volatile int *cancel);
+b200post_prove_opts prove_opts(const b200post_prove_opts *opts);
+
 }  // namespace
 
 extern "C" {
@@ -506,91 +773,52 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
     return generate(data_dir, challenge, cfg, opts, providers, n_providers, out, meta_out, check, cancel);
 }
 
+int b200post_generate_proofs(b200post_prove_item *items, size_t n, const b200post_post_config *cfg, const b200post_prove_opts *opts,
+                             const uint32_t *providers, int n_providers, uint32_t checked, uint32_t parallel_scans,
+                             const volatile int *cancel) {
+    if (!items || n == 0 || !cfg || !providers || n_providers <= 0) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    for (size_t i = 0; i < n; i++)
+        if (!items[i].data_dir) { set_error("invalid argument: item " + std::to_string(i) + " has no data_dir"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::vector<ItemProof> its(n);
+    for (size_t i = 0; i < n; i++) {
+        b200post_prove_item &x = items[i];
+        x.status = B200POST_OK;
+        memset(x.error, 0, sizeof x.error);
+        memset(&x.proof, 0, sizeof x.proof); memset(&x.meta, 0, sizeof x.meta); memset(&x.check, 0, sizeof x.check);
+        its[i].data_dir = x.data_dir; its[i].challenge = x.challenge; its[i].out = &x.proof; its[i].meta_out = &x.meta;
+        its[i].check = checked ? &x.check : nullptr;
+    }
+    const int rc = prove_items(its, *cfg, prove_opts(opts), providers, n_providers, parallel_scans, cancel);
+    for (size_t i = 0; i < n; i++) {
+        items[i].status = its[i].status;
+        snprintf(items[i].error, sizeof items[i].error, "%s", its[i].error.c_str());
+    }
+    return rc;
+}
+
 }  // extern "C"
 
 namespace {
-// b200post_generate_proof_multi (check == nullptr) and b200post_generate_proof_checked: they differ only in the scan's
-// hit records, whether hits are born pending (the ShardedScan's commitment), the report and the final verifier gate
-int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
-             const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
-             b200post_prove_check *check, const volatile int *cancel) {
+// b200post_prove_opts with its defaults filled in
+b200post_prove_opts prove_opts(const b200post_prove_opts *opts) {
     b200post_prove_opts o{};
     if (opts) o = *opts;
     if (o.nonces == 0) o.nonces = 16;
     if (o.chunk_labels == 0) o.chunk_labels = 1ull << 22;
-    b200post_post_metadata md;
-    int rc = b200post_load_metadata(data_dir, &md);
-    if (rc) return rc;
-    const uint64_t num_labels = (uint64_t)md.num_units * md.labels_per_unit;
-    if (num_labels == 0 || o.nonces % 16 || o.nonces > 4096) { set_error("invalid metadata or nonce count"); return B200POST_ERR_INVALID_ARGUMENT; }
-    if (check && (md.scrypt_n < 2 || md.scrypt_n > (1ull << 20) || (md.scrypt_n & (md.scrypt_n - 1)))) {
-        set_error("corrupt metadata: Scrypt.N out of range");
-        return B200POST_ERR_IO;
-    }
-    if ((rc = check_pow_mode(o))) return rc;
-    const uint64_t per_file = md.max_file_size / 16;
-    if (per_file == 0) { set_error("corrupt metadata: MaxFileSize"); return B200POST_ERR_IO; }
-    // the nonce windows [w*n, (w+1)*n) to try, `per_pass` of them per read of the data (b200post_prove_opts)
-    const uint32_t n = o.nonces, windows = std::min(std::max(o.max_windows, 1u), 4096 / n);
-    const uint32_t per_pass = std::max(o.windows_per_pass, 1u);
-    const uint64_t chunk = std::min<uint64_t>(o.chunk_labels, num_labels);
-    const auto ranges = split_shards(num_labels, chunk, (size_t)n_providers);
-    uint8_t commitment[32];
-    if (check) commitment_bytes(md.node_id, md.commitment_atx_id, commitment);
-    uint64_t scanned = 0;              // over every pass
-    std::set<uint64_t> damaged;        // the checked report's, over every pass
-    bool have = false;
-    for (uint32_t a = 0; a < windows && !have;) {
-        const uint32_t m = std::min(per_pass, windows - a), first = a * n;
-        // k2pow per nonce group of the pass (RandomX upstream; or the caller's hook)
-        std::vector<uint64_t> pows;
-        if ((rc = find_pows(o, challenge, md.node_id, md.num_units, cfg->pow_difficulty, providers, n_providers, first / 16, m * n / 16,
-                            &pows, cancel)))
-            return rc;
-        // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
-        ShardedScan scan(ranges, first, n, m, cfg->k2, check ? commitment : nullptr, md.scrypt_n, cancel);
-        for (int s = 0; s < n_providers; s++)
-            if ((rc = scan.scanner((size_t)s).init(providers[s], challenge, m * n, pows.data(), cfg->k1, cfg->k2, num_labels, chunk,
-                                                   check != nullptr, first)))
-                return rc;
-        std::vector<std::unique_ptr<PostDataReader>> readers;
-        for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(data_dir, per_file));
-        rc = scan.run([&](size_t s, uint64_t pos, uint64_t cnt, uint8_t *dst) { return readers[s]->read(pos, cnt, dst); }, chunk, 0, cancel);
-        if (rc) return rc;
-        metrics().prove_passes_total++;
-        ProveRule &rule = scan.rule();
-        scanned += rule.scanned();
-        uint32_t nonce = 0;
-        std::vector<uint64_t> idx;
-        have = rule.decide(&nonce, &idx, &rc);
-        if (check) {   // the checked report adds up over the passes (`damaged`: every distinct damaged index so far)
-            const size_t before = damaged.size();
-            damaged.insert(rule.damaged().begin(), rule.damaged().end());
-            check->labels_rechecked += rule.rechecked(); check->rounds += rule.rounds(); check->damaged = damaged.size();
-            check->n_reported = 0;
-            for (uint64_t i : damaged) {   // ascending
-                if (check->n_reported == 64) break;
-                check->damaged_index[check->n_reported++] = i;
-            }
-            metrics().prove_labels_rechecked_total += rule.rechecked();
-            metrics().prove_damaged_labels_total += damaged.size() - before;
-        }
-        if (rc) return rc;
-        if (have && (rc = write_proof(scanned, nonce, idx, pows.data(), first, num_labels, out))) return rc;
-        a += m;
-    }
-    if (!have) return no_proof(windows, n);
-    b200post_proof_metadata meta;
-    memcpy(meta.node_id, md.node_id, 32);
-    memcpy(meta.commitment_atx_id, md.commitment_atx_id, 32);
-    memcpy(meta.challenge, challenge, 32);
-    meta.num_units = md.num_units; meta.labels_per_unit = md.labels_per_unit;
-    if (check) {
-        // the gate: a proof this library's own verifier rejects is never handed out
-        if ((rc = gate_proof(providers[0], *cfg, md.scrypt_n, o, meta, out))) return rc;
-        check->proof_verified = 1;
-    }
-    if (meta_out) *meta_out = meta;
-    return B200POST_OK;
+    return o;
+}
+
+// b200post_generate_proof_multi (check == nullptr) and b200post_generate_proof_checked: the one-item case of
+// prove_items.  They differ only in the scan's hit records, whether hits are born pending (the ShardedScan's
+// commitment), the report and the final verifier gate.
+int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
+             const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
+             b200post_prove_check *check, const volatile int *cancel) {
+    std::vector<ItemProof> items(1);
+    ItemProof &it = items[0];
+    it.data_dir = data_dir; it.challenge = challenge; it.out = out; it.meta_out = meta_out; it.check = check;
+    prove_items(items, *cfg, prove_opts(opts), providers, n_providers, 1, cancel);
+    if (it.status) set_error(it.error);
+    return it.status;
 }
 }  // namespace

@@ -241,6 +241,44 @@ int RandomxEngine::k2pow(const std::string &key, const rx::K2powTemplate &tmpl, 
     return B200POST_OK;
 }
 
+void RandomxEngine::reset_timing() {
+    std::lock_guard<std::mutex> lk(mu_);
+    total_ms_ = vm_ms_ = 0; hashes_ = vm_launches_ = 0;
+}
+
+int RandomxEngine::search_segments(const std::string &key, const K2powJob *jobs, size_t n_jobs, const JobSegment *segs, size_t n_segs,
+                                   uint32_t *hit) {
+    std::lock_guard<std::mutex> lk(mu_);
+    int rc = ensure_dataset(key);
+    if (rc != B200POST_OK) return rc;
+    if (n_segs == 0) return B200POST_OK;
+    const uint64_t n = (uint64_t)segs[n_segs - 1].off + segs[n_segs - 1].cnt;
+    rc = ensure_batch((uint32_t)std::min<uint64_t>(n, desired_batch()));
+    if (rc != B200POST_OK) return rc;
+    CUDA_TRY(d_jobs_.grow(n_jobs));
+    CUDA_TRY(d_segs_.grow(n_segs));
+    CUDA_TRY(d_hit_.grow(n_segs));
+    CUDA_TRY(cudaEventRecord(ev_[0].get(), stream_.get()));
+    CUDA_TRY(cudaMemcpyAsync(d_jobs_.get(), jobs, n_jobs * sizeof(K2powJob), cudaMemcpyHostToDevice, stream_.get()));
+    CUDA_TRY(cudaMemcpyAsync(d_segs_.get(), segs, n_segs * sizeof(JobSegment), cudaMemcpyHostToDevice, stream_.get()));
+    CUDA_TRY(cudaMemsetAsync(d_hit_.get(), 0xff, n_segs * 4, stream_.get()));
+    const uint32_t step = std::min<uint32_t>(cap_, desired_batch());   // cap_ may be short of the batch (HBM) or left over from a larger one
+    for (uint64_t base = 0; base < n; base += step) {
+        const uint32_t m = (uint32_t)std::min<uint64_t>(step, n - base);
+        CUDA_TRY(rx::launch_seed_k2pow_jobs(buf_, m, (uint32_t)base, d_jobs_.get(), d_segs_.get(), (uint32_t)n_segs, stream_.get()));
+        rc = run_chain(m);
+        if (rc != B200POST_OK) return rc;
+        CUDA_TRY(rx::launch_find_below_jobs(buf_, m, (uint32_t)base, d_jobs_.get(), d_segs_.get(), (uint32_t)n_segs, d_hit_.get(), stream_.get()));
+    }
+    CUDA_TRY(cudaMemcpyAsync(hit, d_hit_.get(), n_segs * 4, cudaMemcpyDeviceToHost, stream_.get()));
+    CUDA_TRY(cudaEventRecord(ev_[1].get(), stream_.get()));
+    CUDA_TRY(cudaStreamSynchronize(stream_.get()));
+    float ms = 0;
+    CUDA_TRY(cudaEventElapsedTime(&ms, ev_[0].get(), ev_[1].get()));
+    total_ms_ += ms; hashes_ += n;
+    return B200POST_OK;
+}
+
 // ------------------------------------------------------------------------------------------------ registry
 static std::mutex g_rx_mu;
 static std::map<int, std::unique_ptr<RandomxEngine>> &g_rx = *new std::map<int, std::unique_ptr<RandomxEngine>>();
@@ -262,6 +300,13 @@ int randomx_engine(uint32_t provider, RandomxEngine **e) {
     *e = randomx_engine_for(provider);
     if (*e) return B200POST_OK;
     return provider == B200POST_CPU_PROVIDER_ID ? B200POST_ERR_UNSUPPORTED : B200POST_ERR_NO_DEVICE;
+}
+
+int randomx_engines(const uint32_t *providers, int n, std::vector<RandomxEngine *> *out) {
+    out->assign((size_t)n, nullptr);
+    for (int i = 0; i < n; i++)
+        if (int rc = randomx_engine(providers[i], &(*out)[(size_t)i])) return rc;
+    return B200POST_OK;
 }
 
 void randomx_shutdown_all() {

@@ -171,18 +171,37 @@ __global__ void seed_inputs_kernel(u64 *__restrict__ seed, u32 stride, u32 n, co
     b2_compress(h, m, len, true);
     for (int i = 0; i < 8; i++) seed[(size_t)i * stride + vm] = h[i];
 }
-__global__ void seed_k2pow_kernel(u64 *__restrict__ seed, u32 stride, u32 n, K2powTemplate t) {
-    const u32 vm = blockIdx.x * blockDim.x + threadIdx.x;
-    if (vm >= n) return;
+// seed of VM `vm` = Blake2b-512(LE56(pow) || tail[0:41]), the k2pow input layout
+__device__ __forceinline__ void seed_k2pow(u64 *__restrict__ seed, u32 stride, u32 vm, u64 pow, const uint8_t *tail) {
     uint8_t in[48];
-    const u64 pow = t.start + vm;
     for (int i = 0; i < 7; i++) in[i] = (uint8_t)(pow >> (8 * i));
-    for (int i = 0; i < 41; i++) in[7 + i] = t.tail[i];
+    for (int i = 0; i < 41; i++) in[7 + i] = tail[i];
     u64 h[8], m[16];
     b2_init(h, 64);
     for (int i = 0; i < 16; i++) { u64 w = 0; if (i < 6) for (int b = 0; b < 8; b++) w |= (u64)in[8 * i + b] << (8 * b); m[i] = w; }
     b2_compress(h, m, 48, true);
     for (int i = 0; i < 8; i++) seed[(size_t)i * stride + vm] = h[i];
+}
+__global__ void seed_k2pow_kernel(u64 *__restrict__ seed, u32 stride, u32 n, K2powTemplate t) {
+    const u32 vm = blockIdx.x * blockDim.x + threadIdx.x;
+    if (vm >= n) return;
+    seed_k2pow(seed, stride, vm, t.start + vm, t.tail);
+}
+// the segment holding batch VM v: the last one whose first VM is <= v (segments ascend and cover the batch)
+__device__ __forceinline__ u32 segment_of(const JobSegment *__restrict__ segs, u32 n_segs, u32 v) {
+    u32 lo = 0, hi = n_segs;
+    while (hi - lo > 1) { const u32 mid = (lo + hi) / 2; if (segs[mid].off <= v) lo = mid; else hi = mid; }
+    return lo;
+}
+// Job search: VM vm of this launch is VM vm_base + vm of the batch; it hashes its segment's job at the segment's next pow
+__global__ void __launch_bounds__(128) seed_k2pow_jobs_kernel(u64 *__restrict__ seed, u32 stride, u32 n, u32 vm_base,
+                                                              const K2powJob *__restrict__ jobs, const JobSegment *__restrict__ segs,
+                                                              u32 n_segs) {
+    const u32 vm = blockIdx.x * blockDim.x + threadIdx.x;
+    if (vm >= n) return;
+    const u32 v = vm_base + vm;
+    const JobSegment s = segs[segment_of(segs, n_segs, v)];
+    seed_k2pow(seed, stride, vm, s.first_pow + (v - s.off), jobs[s.job].tail);
 }
 
 // ---------------------------------------------------------------------------------------------- scratchpad fill / hash
@@ -633,6 +652,21 @@ __global__ void find_below_kernel(const uint8_t *__restrict__ hashes, u32 n, con
     }
 }
 
+// Job search: a VM whose hash is below its job's difficulty takes the minimum of its offset into its segment in the
+// segment's hit slot (pre-set to 0xffffffff by the caller), so only n_segs words come back
+__global__ void __launch_bounds__(256) find_below_jobs_kernel(const uint8_t *__restrict__ hashes, u32 n, u32 vm_base,
+                                                              const K2powJob *__restrict__ jobs, const JobSegment *__restrict__ segs,
+                                                              u32 n_segs, u32 *__restrict__ hit) {
+    const u32 vm = blockIdx.x * blockDim.x + threadIdx.x;
+    if (vm >= n) return;
+    const u32 v = vm_base + vm, s = segment_of(segs, n_segs, v);
+    const uint8_t *h = hashes + (size_t)vm * 32, *d = jobs[segs[s].job].difficulty;
+    for (int i = 0; i < 32; i++) {               // big-endian byte order: the first differing byte decides
+        const uint8_t a = h[i], b = d[i];
+        if (a != b) { if (a < b) atomicMin(&hit[s], v - segs[s].off); return; }
+    }
+}
+
 inline u32 blocks_for(u64 n, u32 per) { return (u32)((n + per - 1) / per); }
 
 }  // namespace
@@ -724,6 +758,16 @@ cudaError_t launch_finalize(const BatchBuffers &b, uint32_t n, cudaStream_t s) {
 }
 cudaError_t launch_find_below(const BatchBuffers &b, uint32_t n, const uint8_t *d_difficulty, uint32_t *d_found, cudaStream_t s) {
     find_below_kernel<<<blocks_for(n, 256), 256, 0, s>>>(b.hashes, n, d_difficulty, d_found);
+    return cudaGetLastError();
+}
+cudaError_t launch_seed_k2pow_jobs(const BatchBuffers &b, uint32_t n, uint32_t vm_base, const K2powJob *d_jobs, const JobSegment *d_segs,
+                                   uint32_t n_segs, cudaStream_t s) {
+    seed_k2pow_jobs_kernel<<<blocks_for(n, 128), 128, 0, s>>>(reinterpret_cast<u64 *>(b.seed), b.stride, n, vm_base, d_jobs, d_segs, n_segs);
+    return cudaGetLastError();
+}
+cudaError_t launch_find_below_jobs(const BatchBuffers &b, uint32_t n, uint32_t vm_base, const K2powJob *d_jobs, const JobSegment *d_segs,
+                                   uint32_t n_segs, uint32_t *d_hit, cudaStream_t s) {
+    find_below_jobs_kernel<<<blocks_for(n, 256), 256, 0, s>>>(b.hashes, n, vm_base, d_jobs, d_segs, n_segs, d_hit);
     return cudaGetLastError();
 }
 

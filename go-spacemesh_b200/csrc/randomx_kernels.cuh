@@ -4,6 +4,7 @@
 
 #include <cstdint>
 
+#include "k2pow_jobs.h"
 #include "randomx_host.h"
 
 namespace b200post {
@@ -56,6 +57,13 @@ cudaError_t launch_chain_seed(const BatchBuffers &b, uint32_t n, cudaStream_t s)
 cudaError_t launch_finalize(const BatchBuffers &b, uint32_t n, cudaStream_t s);
 // k2pow: smallest VM index whose hash < difficulty (32 bytes big-endian), or 0xffffffff, into *d_found (pre-set by the caller)
 cudaError_t launch_find_below(const BatchBuffers &b, uint32_t n, const uint8_t *d_difficulty, uint32_t *d_found, cudaStream_t s);
+// k2pow job search over a batch described by segments (k2pow_jobs.h); this launch runs the batch's VMs
+// [vm_base, vm_base + n) in buffer slots 0..n-1.  Seeds: each VM's input from its segment's job and pow.
+cudaError_t launch_seed_k2pow_jobs(const BatchBuffers &b, uint32_t n, uint32_t vm_base, const K2powJob *d_jobs, const JobSegment *d_segs,
+                                   uint32_t n_segs, cudaStream_t s);
+// hit[s] = min(hit[s], offset into segment s) of every VM whose hash is below its job's difficulty
+cudaError_t launch_find_below_jobs(const BatchBuffers &b, uint32_t n, uint32_t vm_base, const K2powJob *d_jobs, const JobSegment *d_segs,
+                                   uint32_t n_segs, uint32_t *d_hit, cudaStream_t s);
 // one-time: uploads the AES tables / opcode map the kernels read
 cudaError_t upload_tables();
 

@@ -196,3 +196,54 @@ func RandomxHash(provider uint32, key []byte, inputs [][]byte) ([][32]byte, erro
 	copy(unsafe.Slice((*byte)(unsafe.Pointer(&res[0])), 32*n), unsafe.Slice((*byte)(out), 32*n))
 	return res, nil
 }
+
+// K2powJob is one k2pow of a job search: any identity, challenge and nonce group, with its own difficulty (the
+// PowDifficulty divided by that identity's NumUnits, ScaleDifficulty).
+type K2powJob struct {
+	NodeID     [32]byte
+	Challenge8 [8]byte
+	NonceGroup uint8
+	Difficulty [32]byte
+}
+
+// K2powSearchJobs runs several identities' k2pows in one search (b200post_k2pow_search_jobs): their windows of
+// nonces share device batches.  pows[j] is job j's smallest valid pow below maxNoncesPerJob (0 = the whole nonce space)
+// or K2powNotFound, whatever the other jobs and the device list (repeats allowed).  ctx cancels between windows.
+func K2powSearchJobs(ctx context.Context, providers []uint32, cacheKey []byte, jobs []K2powJob, maxNoncesPerJob uint64) (pows []uint64, hashes uint64, err error) {
+	if len(providers) == 0 {
+		return nil, 0, ErrNoProvider
+	}
+	if len(jobs) == 0 {
+		return nil, 0, nil
+	}
+	cj := (*C.b200post_k2pow_job)(C.calloc(C.size_t(len(jobs)), C.size_t(unsafe.Sizeof(C.b200post_k2pow_job{}))))
+	defer C.free(unsafe.Pointer(cj))
+	for i, j := range jobs {
+		x := &unsafe.Slice(cj, len(jobs))[i]
+		C.memcpy(unsafe.Pointer(&x.node_id[0]), unsafe.Pointer(&j.NodeID[0]), 32)
+		C.memcpy(unsafe.Pointer(&x.challenge8[0]), unsafe.Pointer(&j.Challenge8[0]), 8)
+		x.nonce_group = C.uint8_t(j.NonceGroup)
+		C.memcpy(unsafe.Pointer(&x.difficulty[0]), unsafe.Pointer(&j.Difficulty[0]), 32)
+	}
+	var key unsafe.Pointer
+	if cacheKey != nil {
+		key = C.CBytes(cacheKey)
+		defer C.free(key)
+	}
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	out := (*C.uint64_t)(C.calloc(C.size_t(len(jobs)), 8))
+	defer C.free(unsafe.Pointer(out))
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	var done C.uint64_t
+	if err := statusErr(checked(func() C.int {
+		return C.b200post_k2pow_search_jobs(provs, C.int(len(providers)), (*C.uint8_t)(key), C.size_t(len(cacheKey)), C.size_t(len(jobs)), cj,
+			C.uint64_t(maxNoncesPerJob), out, &done, flag)
+	})); err != nil {
+		return nil, uint64(done), err
+	}
+	pows = make([]uint64, len(jobs))
+	copy(pows, unsafe.Slice((*uint64)(unsafe.Pointer(out)), len(jobs)))
+	return pows, uint64(done), nil
+}

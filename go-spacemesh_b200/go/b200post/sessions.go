@@ -731,3 +731,78 @@ func SearchVRFNonce(ctx context.Context, dataDir string, o VRFSearchOpts) (nonce
 	C.memcpy(unsafe.Pointer(&label[0]), unsafe.Pointer(&out.label32[0]), 32)
 	return uint64(out.index), label, nil
 }
+
+// ProveItem is one identity's POST in GenerateProofs.
+type ProveItem struct {
+	DataDir   string
+	Challenge [32]byte // per identity: identities registered at different PoETs get different challenges
+}
+
+// ProveResult is one identity's outcome in GenerateProofs: Err is what GenerateProofCheckedWindows (checked) or
+// GenerateProofOn returns for that identity alone, Proof is set when Err is nil, and Check (checked) holds the report,
+// also for an item whose proof failed after its scan.
+type ProveResult struct {
+	Proof *Proof
+	Check *ProveCheck
+	Err   error
+}
+
+// GenerateProofs proves for several identities in one call (b200post_generate_proofs), the way a node that runs one
+// post-service per identity needs them at the same PoET round: their k2pow searches share device batches, one
+// identity's scan overlaps the others' searches, and at most parallelScans scans run at once (0 = min(len(items), 4)).
+// Each result equals the one-identity call for that item, whatever the other items.  An item's failure is its
+// result's Err; the returned error is the call's own (no providers, the device list, ctx cancelled).
+func GenerateProofs(ctx context.Context, providers []uint32, items []ProveItem, cfg SetupConfig, nonces uint32, w NonceWindows,
+	checkedProofs bool, parallelScans uint32) ([]ProveResult, error) {
+	if len(providers) == 0 {
+		return nil, ErrNoProvider
+	}
+	if len(items) == 0 {
+		return nil, nil
+	}
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), max_windows: C.uint32_t(w.Max), windows_per_pass: C.uint32_t(w.PerPass)}
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	// the items live in C memory: the library keeps pointers into them for the whole call
+	arr := (*C.b200post_prove_item)(C.calloc(C.size_t(len(items)), C.size_t(unsafe.Sizeof(C.b200post_prove_item{}))))
+	defer C.free(unsafe.Pointer(arr))
+	cs := unsafe.Slice(arr, len(items))
+	for i, it := range items {
+		cs[i].data_dir = C.CString(it.DataDir)
+		defer C.free(unsafe.Pointer(cs[i].data_dir))
+		C.memcpy(unsafe.Pointer(&cs[i].challenge[0]), unsafe.Pointer(&it.Challenge[0]), 32)
+	}
+	var chk C.uint32_t
+	if checkedProofs {
+		chk = 1
+	}
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	if err := statusErr(checked(func() C.int {
+		return C.b200post_generate_proofs(arr, C.size_t(len(items)), &c, &o, provs, C.int(len(providers)), chk, C.uint32_t(parallelScans), flag)
+	})); err != nil {
+		return nil, err
+	}
+	out := make([]ProveResult, len(items))
+	for i := range cs {
+		x := &cs[i]
+		if checkedProofs {
+			rep := &ProveCheck{LabelsRechecked: uint64(x.check.labels_rechecked), Damaged: uint64(x.check.damaged),
+				ProofVerified: x.check.proof_verified != 0, Rounds: uint32(x.check.rounds)}
+			for k := 0; k < int(x.check.n_reported); k++ {
+				rep.DamagedIndex = append(rep.DamagedIndex, uint64(x.check.damaged_index[k]))
+			}
+			out[i].Check = rep
+		}
+		if err := statusErr(C.int(x.status), C.GoString(&x.error[0])); err != nil {
+			out[i].Err = err
+			continue
+		}
+		out[i].Proof = &Proof{Nonce: uint32(x.proof.nonce), Pow: uint64(x.proof.pow),
+			Indices: C.GoBytes(unsafe.Pointer(&x.proof.indices[0]), C.int(x.proof.indices_len))}
+	}
+	return out, nil
+}

@@ -18,6 +18,11 @@ class _Params(ctypes.Structure):
                 ("challenge8", ctypes.c_uint8 * 8), ("node_id", ctypes.c_uint8 * 32), ("difficulty", ctypes.c_uint8 * 32)]
 
 
+class _Job(ctypes.Structure):
+    _fields_ = [("node_id", ctypes.c_uint8 * 32), ("challenge8", ctypes.c_uint8 * 8), ("nonce_group", ctypes.c_uint8),
+                ("difficulty", ctypes.c_uint8 * 32)]
+
+
 _bound = False
 
 
@@ -40,6 +45,8 @@ def _bind():
         L.b200post_k2pow_search_group_range.argtypes = [u32, ctypes.POINTER(_Params), u32, u32, u64, vp, ctypes.POINTER(u64), vp]
         L.b200post_k2pow_search_group_range_multi.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.POINTER(_Params), u32, u32,
                                                               u64, vp, ctypes.POINTER(u64), vp]
+        L.b200post_k2pow_search_jobs.argtypes = [ctypes.POINTER(u32), ctypes.c_int, ctypes.c_char_p, sz, sz, ctypes.POINTER(_Job), u64,
+                                                 vp, ctypes.POINTER(u64), vp]
         L.b200post_k2pow_verify.argtypes = [u32, ctypes.POINTER(_Params), u64, ctypes.POINTER(ctypes.c_int)]
         L.b200post_randomx_dataset_read.argtypes = [u32, ctypes.c_char_p, sz, u64, u64, vp]
         L.b200post_randomx_last_timing.argtypes = [u32, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
@@ -143,6 +150,26 @@ def search_group_range(challenge8: bytes, node_id: bytes, difficulty: bytes, fir
         _check(_bind().b200post_k2pow_search_group_range(provider, ctypes.byref(p), first_group, n_groups, max_nonces_per_group,
                                                          pows.ctypes.data, ctypes.byref(done), cptr))
     return [None if int(v) == NOT_FOUND else int(v) for v in pows[:n_groups]], done.value
+
+
+def search_jobs(jobs, max_nonces_per_job: int = 0, *, key: bytes | None = None, providers=(0,), cancel=None):
+    """Several identities' k2pows in one search sharing device batches (b200post_k2pow_search_jobs).  jobs: a list of
+    (node_id, challenge8, nonce_group, difficulty) with the difficulty already scaled by the identity's num_units.
+    -> (pows, hashes computed), pows[j] being job j's smallest valid pow below max_nonces_per_job (0 = the whole nonce
+    space) or None."""
+    arr = (_Job * max(len(jobs), 1))()
+    for a, (node_id, challenge8, group, difficulty) in zip(arr, jobs):
+        a.node_id = (ctypes.c_uint8 * 32)(*node_id)
+        a.challenge8 = (ctypes.c_uint8 * 8)(*challenge8[:8])
+        a.nonce_group = group
+        a.difficulty = (ctypes.c_uint8 * 32)(*difficulty)
+    pows = np.zeros(max(len(jobs), 1), dtype=np.uint64)
+    done = ctypes.c_uint64(0)
+    provs = (ctypes.c_uint32 * max(len(providers), 1))(*providers)
+    _check(_bind().b200post_k2pow_search_jobs(provs if len(providers) else None, len(providers), key, len(key) if key is not None else 0,
+                                              len(jobs), arr, max_nonces_per_job, pows.ctypes.data, ctypes.byref(done),
+                                              ctypes.addressof(cancel) if cancel is not None else None))
+    return [None if int(v) == NOT_FOUND else int(v) for v in pows[:len(jobs)]], done.value
 
 
 def dataset(first: int, count: int, key: bytes | None = None, *, provider: int = 0) -> np.ndarray:

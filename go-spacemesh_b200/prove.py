@@ -51,6 +51,24 @@ class ProveCheck:
     rounds: int = 0
 
 
+class _ProveItem(ctypes.Structure):
+    _fields_ = [("data_dir", ctypes.c_char_p), ("challenge", ctypes.c_uint8 * 32), ("status", ctypes.c_int32),
+                ("error", ctypes.c_char * 256), ("proof", _ProofOut), ("meta", _Meta), ("check", _ProveCheck)]
+
+
+@dataclass
+class ItemResult:
+    """One identity's outcome in generate_proofs: status and error are what the one-identity call returns and sets
+    (OK and "" on success); proof, metadata, labels scanned and (checked) the report are set when status is OK, and the
+    report also when a checked proof failed later."""
+    status: int
+    error: str
+    proof: Proof | None
+    meta: ProofMetadata | None
+    labels_scanned: int
+    check: ProveCheck | None
+
+
 def _bind():
     L = lib()
     if getattr(L, "_prove_bound", False):
@@ -65,6 +83,9 @@ def _bind():
     L.b200post_generate_proof_checked.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
                                                   ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_ProofOut),
                                                   ctypes.POINTER(_Meta), ctypes.POINTER(_ProveCheck), ctypes.c_void_p]
+    L.b200post_generate_proofs.argtypes = [ctypes.POINTER(_ProveItem), ctypes.c_size_t, ctypes.POINTER(_PostConfig),
+                                           ctypes.POINTER(_ProveOpts), ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.c_uint32,
+                                           ctypes.c_uint32, ctypes.c_void_p]
     L._prove_bound = True
     return L
 
@@ -109,6 +130,41 @@ def _results(out, meta):
     pm = ProofMetadata(bytes(meta.node_id), bytes(meta.commitment_atx_id), bytes(meta.challenge), int(meta.num_units),
                        int(meta.labels_per_unit))
     return proof, pm, int(out.labels_scanned)
+
+
+def _report(chk) -> ProveCheck:
+    return ProveCheck(int(chk.labels_rechecked), int(chk.damaged), [int(v) for v in chk.damaged_index[: chk.n_reported]],
+                      bool(chk.proof_verified), int(chk.rounds))
+
+
+def generate_proofs(items, cfg: PostConfig, *, providers=(0,), checked: bool = True, parallel_scans: int = 0,
+                    nonces: int = 16, chunk_labels: int = 0, pow="builtin", cancel=None, max_windows=1,
+                    windows_per_pass: int = 1):
+    """Proofs of several identities' POSTs in one call (b200post_generate_proofs): items is a list of (data_dir,
+    challenge).  Their k2pow searches share device batches and one identity's scan overlaps the others' searches; each
+    result equals generate_proof_checked (checked) or generate_proof(providers=...) for that item alone.
+    -> (the call's status, [ItemResult]).  The call's status is OK unless the arguments, the pow mode or the device
+    list are refused, or `cancel` was set; an item's own failure is its ItemResult's, not an exception."""
+    L = _bind()
+    opts, providers = _opts(None, list(providers) if not isinstance(providers, str) else providers, nonces, chunk_labels, pow,
+                            max_windows, windows_per_pass)
+    arr = (_ProveItem * max(len(items), 1))()
+    dirs = [d.encode() if d is not None else None for d, _ in items]   # kept alive for the call
+    for a, d, (_, ch) in zip(arr, dirs, items):
+        a.data_dir = d
+        a.challenge = (ctypes.c_uint8 * 32)(*ch)
+    c = _c_cfg(cfg)
+    provs = (ctypes.c_uint32 * max(len(providers), 1))(*providers)
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    rc = L.b200post_generate_proofs(arr, len(items), ctypes.byref(c), ctypes.byref(opts), provs if len(providers) else None,
+                                    len(providers), int(checked), parallel_scans, cptr)
+    out = []
+    for a in arr[: len(items)]:
+        ok = a.status == OK
+        proof, meta, scanned = _results(a.proof, a.meta) if ok else (None, None, 0)
+        out.append(ItemResult(int(a.status), a.error.decode(errors="replace"), proof, meta, scanned,
+                              _report(a.check) if checked else None))
+    return rc, out
 
 
 def generate_proof_checked(data_dir: str, challenge: bytes, cfg: PostConfig, *, providers=(0,), nonces: int = 16,

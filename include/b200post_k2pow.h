@@ -104,6 +104,30 @@ int b200post_k2pow_search_group_range_multi(const uint32_t *providers, int n_pro
                                             uint32_t first_group, uint32_t n_groups, uint64_t max_nonces_per_group, uint64_t *pows,
                                             uint64_t *hashes_done, const volatile int *cancel);
 
+/* One k2pow of a job search: any identity, challenge and nonce group, with its own difficulty (already divided by the
+ * identity's num_units). */
+typedef struct b200post_k2pow_job {
+    uint8_t node_id[32];
+    uint8_t challenge8[8];
+    uint8_t nonce_group;
+    uint8_t difficulty[32];        /* big-endian */
+} b200post_k2pow_job;
+
+/* Several identities' k2pows in one search, sharing device batches (what a node proving for several identities needs).
+ * pows[j] is job j's smallest valid pow in [0, max_nonces_per_job) (0 = the whole 56-bit space), or
+ * B200POST_K2POW_NOT_FOUND, whatever the other jobs, their order and the device list; the group searches above are the
+ * one-identity case of this search.  Windows of `per` consecutive nonces go out in ascending order from one cursor, each
+ * to every job without a hit yet, `per` = a device batch / the jobs pending (at least 1); a window wider than a batch runs
+ * as several device batches.  A job's pow is final once every window below its lowest hit has finished.  One host thread
+ * per list entry (repeats allowed) takes windows; *hashes_done (may be NULL) = the sum over windows of jobs x per.
+ * `cancel` is polled between windows.  Errors: arguments (n_jobs 0 included), then NO_DEVICE / UNSUPPORTED of the first
+ * failing list entry; a device error or CANCELLED of any thread fails the call once all have joined (the first failing
+ * entry in list order gives the status and text), and then only final pows are given.  b200post_randomx_last_timing of
+ * each device covers the whole search. */
+int b200post_k2pow_search_jobs(const uint32_t *providers, int n_providers, const uint8_t *cache_key, size_t cache_key_len,
+                               size_t n_jobs, const b200post_k2pow_job *jobs, uint64_t max_nonces_per_job, uint64_t *pows,
+                               uint64_t *hashes_done, const volatile int *cancel);
+
 /* The verifier's check: *valid = 1 iff RandomX(input(pow)) < p->difficulty. */
 int b200post_k2pow_verify(uint32_t provider, const b200post_k2pow_params *p, uint64_t pow, int *valid);
 

@@ -138,6 +138,39 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
                                     b200post_proof_out *out, b200post_proof_metadata *meta_out, b200post_prove_check *check,
                                     const volatile int *cancel);
 
+/* One identity's proof in b200post_generate_proofs. */
+typedef struct b200post_prove_item {
+    const char *data_dir;              /* in                                                                          */
+    uint8_t challenge[32];             /* in: per identity (identities registered at different PoETs differ)          */
+    int32_t status;                    /* out: what the one-identity call returns for this item                       */
+    char error[256];                   /* out: that call's b200post_last_error() text (truncated), "" when OK         */
+    b200post_proof_out proof;          /* out: valid when status is OK                                                */
+    b200post_proof_metadata meta;      /* out: valid when status is OK                                                */
+    b200post_prove_check check;        /* out: filled when `checked`                                                  */
+} b200post_prove_item;
+
+/* Proofs of several identities' POSTs in one call (a node that proves for several identities at once, DESIGN.md §5).
+ * Contract: for every item, (nonce, indices, pow), labels_scanned, the check report and status equal those of
+ * b200post_generate_proof_checked (checked = 1) or b200post_generate_proof_multi (checked = 0) called for that item
+ * alone with the same opts and provider list, whatever the other items, their order and parallel_scans.
+ *   k2pow (BUILTIN): the pows of the current pass of every item still proving go into ONE b200post_k2pow_search_jobs
+ *     search over `providers`, so identities share device batches.  CALLBACK and SKIP behave per item as in the single call.
+ *   scans: an item's scan (the single call's, over `providers`) starts as soon as all of its pass's pows are final,
+ *     while the search goes on for the others; at most parallel_scans scans run at once (0 = min(n, 4)), which bounds
+ *     pinned staging at parallel_scans x n_providers x 2 x chunk_labels x 16 bytes.  An item that needs another pass
+ *     (max_windows) joins the next search.
+ *   gate (checked): the proofs go through b200post_verify_batch on providers[0] together, one call per scrypt N among
+ *     them, instead of one call each.
+ * Errors: an item's failure stays with that item (missing or corrupt metadata, a read error, "no proof found", a gate
+ * rejection, a device error of its scan or search).  The call itself returns, in the single call's order:
+ * B200POST_ERR_INVALID_ARGUMENT for bad call arguments (items NULL, n 0, cfg NULL, no providers, an item without
+ * data_dir; no item is touched), B200POST_ERR_UNSUPPORTED for opts' pow mode, B200POST_ERR_NO_DEVICE / UNSUPPORTED
+ * for the device list (checked once some item passed its host checks; those items get the same code and text), and
+ * B200POST_ERR_CANCELLED when `cancel` stopped any item (those items report CANCELLED and no proof); else B200POST_OK. */
+int b200post_generate_proofs(b200post_prove_item *items, size_t n, const b200post_post_config *cfg,
+                             const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                             uint32_t checked, uint32_t parallel_scans, const volatile int *cancel);
+
 /*
  * The initial proof of a POST, produced by its setup session (DESIGN.md §3e).  go-spacemesh asks for it right after
  * initialisation (BuildInitialPost: PostClient.Proof(ctx, nodeID, shared.ZeroChallenge, nil)); a proof over 32 zero bytes
