@@ -57,6 +57,9 @@ extern "C" size_t b200post_metrics_text(char *buf, size_t cap) {
     line("b200post_setup_label_mismatch_total", "reference-label cross-check failures", "counter", m.setup_label_mismatch_total);
     line("b200post_post_data_labels_verified_total", "stored POST labels recomputed and compared (verify_pos)", "counter", m.post_data_labels_verified_total);
     line("b200post_post_data_label_mismatch_total", "stored POST labels that differed from their recomputation (verify_pos)", "counter", m.post_data_label_mismatch_total);
+    line("b200post_sums_blocks_checked_total", "1 MiB label blocks hashed and compared with their checksums (check_sums, write_sums)", "counter", m.sums_blocks_checked_total);
+    line("b200post_sums_blocks_bad_total", "label blocks whose stored bytes differed from their checksum or recomputation", "counter", m.sums_blocks_bad_total);
+    line("b200post_sums_blocks_repaired_total", "damaged label blocks recomputed and written back (check_sums -repair)", "counter", m.sums_blocks_repaired_total);
     if (buf && cap) {
         const size_t n = o.size() < cap - 1 ? o.size() : cap - 1;
         memcpy(buf, o.data(), n);

@@ -30,6 +30,14 @@
 // with -rangeRecord.
 // -nonceWindows W scans the nonces [0, W x nonces) in the same pass: the proof comes from the lowest window of -nonces
 // nonces that has one, as a prover trying W windows would find it.
+// Block checksums (postdata_N.sum, one BLAKE3 digest per 1 MiB of labels; DESIGN.md §3g):
+//   b200postcli <init flags> -checksums                  init writes the sidecars from the labels it computes
+//   b200postcli -checkSums -datadir D [-fromFile A -toFile B] [-provider P] [-repair]
+//   b200postcli -verify -fraction 100 -writeSums -datadir D [-fromFile A -toFile B] [-provider 0|all]
+// -checkSums reads the covered labels and compares them with their checksums at storage speed, printing
+// `file N labels [a, b)` for each bad block; -repair recomputes those blocks and writes them back.  -writeSums gives
+// sidecars to data that has none, after recomputing and matching every label.  Exit codes: 0 clean, 1 damaged or
+// incomplete, 2 usage, 130 stopped.
 // Exit codes: 0 ok (-mergeRanges: the nonce is settled, with or without the initial proof), 1 error or damaged data,
 // 2 usage, 130 stopped.
 #include <signal.h>
@@ -110,6 +118,56 @@ static int run_verify(const std::string &datadir, const std::string &provider, d
     return 1;
 }
 
+static int run_sums(const std::string &datadir, const std::string &provider, uint64_t from_file, int64_t to_file, bool write, bool repair) {
+    b200post_sums_opts o;
+    b200post_default_sums_opts(&o);
+    o.provider_id = provider == "all" ? B200POST_PROVIDER_ALL : (int64_t)strtoull(provider.c_str(), nullptr, 10);
+    if (o.provider_id == (int64_t)B200POST_CPU_PROVIDER_ID) { fprintf(stderr, "provider 4294967295 (CPU) is not served: this build has no CPU path\n"); return 2; }
+    if (!write && o.provider_id == B200POST_PROVIDER_ALL) { fprintf(stderr, "-checkSums runs on one device: -provider takes a CUDA ordinal\n"); return 2; }
+    o.from_file = from_file; o.to_file = to_file; o.repair = repair;
+    uint64_t per_file = 0;
+    b200post_post_metadata md;
+    if (b200post_load_metadata(datadir.c_str(), &md) == 0 && md.max_file_size >= 16) per_file = md.max_file_size / 16;
+    volatile uint64_t progress = 0;
+    o.progress = &progress;
+    signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
+    volatile int done = 0;
+    std::thread show([&] {
+        const auto t0 = std::chrono::steady_clock::now();
+        while (!done) {
+            for (int k = 0; k < 20 && !done; k++) std::this_thread::sleep_for(std::chrono::milliseconds(100));
+            const double el = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+            const uint64_t p = progress;
+            fprintf(stderr, "\r%llu labels %s, %.0f labels/s   ", (unsigned long long)p, write ? "recomputed and compared" : "hashed", el > 0 ? p / el : 0.0);
+        }
+        fprintf(stderr, "\n");
+    });
+    b200post_sums_result r;
+    const int rc = write ? b200post_write_sums(datadir.c_str(), &o, &r, &g_cancel) : b200post_check_sums(datadir.c_str(), &o, &r, &g_cancel);
+    done = 1;
+    show.join();
+    if (rc == B200POST_ERR_CANCELLED) { fprintf(stderr, "stopped\n"); return 130; }
+    if (rc != 0 && rc != B200POST_ERR_LABEL_MISMATCH && !(rc == B200POST_ERR_STATE && r.labels_checked)) {
+        fprintf(stderr, "%s failed: %s (%d)\n", write ? "writeSums" : "checkSums", b200post_last_error(), rc);
+        return 1;
+    }
+    printf("%s %llu labels (%llu bytes read) in %llu files: %llu bad blocks\n", write ? "verified" : "checked", (unsigned long long)r.labels_checked,
+           (unsigned long long)r.bytes_read, (unsigned long long)(r.files_checked + (write ? r.files_unchecked : 0)), (unsigned long long)r.bad_blocks);
+    for (uint32_t i = 0; i < r.n_reported && per_file; i++)
+        printf("file %llu labels [%llu, %llu)\n", (unsigned long long)(r.bad[i].first_label / per_file),
+               (unsigned long long)r.bad[i].first_label, (unsigned long long)(r.bad[i].first_label + r.bad[i].count));
+    if (write) printf("checksums written for %llu files; %llu files damaged, none written for them\n", (unsigned long long)r.files_checked,
+                      (unsigned long long)r.files_unchecked);
+    else {
+        if (repair) printf("repaired %llu blocks\n", (unsigned long long)r.repaired_blocks);
+        if (r.labels_unchecked) printf("%llu labels in %llu files have no checksum\n", (unsigned long long)r.labels_unchecked, (unsigned long long)r.files_unchecked);
+    }
+    if (rc == 0) { printf("POST data matches its checksums\n"); return 0; }
+    if (rc == B200POST_ERR_LABEL_MISMATCH) fprintf(stderr, "%s\n", b200post_last_error());
+    printf(rc == B200POST_ERR_STATE ? "the check is incomplete\n" : "POST data is DAMAGED\n");
+    return 1;
+}
+
 static int run_merge(const std::string &datadir, const std::string &provider, uint64_t batch, const b200post_post_config &cfg_in) {
     b200post_merge_opts o{};
     o.provider_id = provider == "all" ? B200POST_PROVIDER_ALL : (int64_t)strtoull(provider.c_str(), nullptr, 10);
@@ -169,7 +227,7 @@ int main(int argc, char **argv) {
     std::string id, atx, datadir = "./post-data", provider = "0";
     uint64_t num_units = 0, labels_per_unit = 0, scrypt_n = 8192, max_file_size = 4ull << 30, batch = 1ull << 20;
     bool print_providers = false, verify = false, print_num_files = false, search = false, range = false, initial = false;
-    bool range_record = false, merge = false;
+    bool range_record = false, merge = false, checksums = false, check_sums = false, repair = false, write_sums = false;
     uint32_t nonces = 288, windows = 1, k1 = 0, k2 = 0;
     std::string pow_difficulty;
     double fraction = 0.2;
@@ -207,6 +265,10 @@ int main(int argc, char **argv) {
         else if (a == "k1") k1 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "k2") k2 = (uint32_t)strtoul(val().c_str(), nullptr, 10);
         else if (a == "powDifficulty") pow_difficulty = val();
+        else if (a == "checksums") checksums = true;
+        else if (a == "checkSums") check_sums = true;
+        else if (a == "repair") repair = true;
+        else if (a == "writeSums") write_sums = true;
         else { fprintf(stderr, "unknown flag -%s\n", a.c_str()); return 2; }
     }
     if (print_providers) {
@@ -222,6 +284,12 @@ int main(int argc, char **argv) {
         printf("%llu\n", (unsigned long long)((nl + per_file - 1) / per_file));
         return 0;
     }
+    if (repair && !check_sums) { fprintf(stderr, "-repair needs -checkSums\n"); return 2; }
+    if (write_sums && (!verify || fraction != 100.0)) { fprintf(stderr, "-writeSums needs -verify -fraction 100: checksums are written only for labels that were all recomputed\n"); return 2; }
+    if (check_sums && (verify || checksums)) { fprintf(stderr, "-checkSums does not combine with -verify or -checksums\n"); return 2; }
+    if (checksums && (verify || search || merge)) { fprintf(stderr, "-checksums is an init flag\n"); return 2; }
+    if (check_sums) return run_sums(datadir, provider, from_file, to_file, false, repair);
+    if (write_sums) return run_sums(datadir, provider, from_file, to_file, true, false);
     if (verify) return run_verify(datadir, provider, fraction, from_file, to_file, seed);
     if (search) return run_search(datadir, provider, batch);
     b200post_post_config cfg;
@@ -263,6 +331,7 @@ int main(int argc, char **argv) {
             return rc == B200POST_ERR_INVALID_ARGUMENT || rc == B200POST_ERR_STATE ? 2 : 1;
         }
     }
+    if (checksums && b200post_setup_request_checksums(mgr)) { fprintf(stderr, "checksums: %s\n", b200post_last_error()); return 1; }
     signal(SIGINT, on_signal); signal(SIGTERM, on_signal);
     const uint64_t per_file = o.max_file_size / 16, all = (uint64_t)o.num_units * cfg.labels_per_unit;
     const uint64_t total = range ? std::min<uint64_t>(to_file < 0 ? all : (uint64_t)(to_file + 1) * per_file, all) - from_file * per_file : all;

@@ -121,6 +121,8 @@ std::string range_record_path(const std::string &dir, uint64_t from_file, uint64
     return join(dir, "range_" + std::to_string(from_file) + "_" + std::to_string(to_file) + ".rec");
 }
 
+std::string sums_path(const std::string &dir, uint64_t file) { return join(dir, "postdata_" + std::to_string(file) + ".sum"); }
+
 PostFile post_file_kind(const std::string &name, bool *tmp) {
     const bool t = ends_with(name, ".tmp");
     if (tmp) *tmp = t;
@@ -130,6 +132,7 @@ PostFile post_file_kind(const std::string &name, bool *tmp) {
     if (base == kInitialProofFile) return PostFile::kInitialProof;
     if (base == kInitialScanFile) return PostFile::kInitialScan;
     if (base.size() > 4 && base.rfind("range_", 0) == 0 && ends_with(base, ".rec")) return PostFile::kRangeRecord;
+    if (base.size() > 13 && base.rfind("postdata_", 0) == 0 && ends_with(base, ".sum")) return PostFile::kSums;
     return PostFile::kNone;
 }
 
@@ -360,6 +363,63 @@ int load_initial_proof_file(const std::string &dir, const b200post_post_metadata
     *out = p;
     if (pm) *pm = m;
     return B200POST_OK;
+}
+
+// ---- postdata_<N>.sum: "B2PSUMS1" | version u32 | block labels u32 | NodeId | CommitmentAtxId | Scrypt.N u64 |
+// labels per file u64 | file u64 | covered u64 | digests | FNV-1a 64 of everything before it (little endian)
+namespace {
+
+const char kSumsMagic[] = "B2PSUMS1";
+const uint32_t kSumsVersion = 1;
+const size_t kSumsHeader = 8 + 4 + 4 + 32 + 32 + 8 * 4;
+
+uint64_t fnv1a64(const char *p, size_t n) {
+    uint64_t h = 0xcbf29ce484222325ull;
+    for (size_t i = 0; i < n; i++) { h ^= (unsigned char)p[i]; h *= 0x100000001b3ull; }
+    return h;
+}
+template <class T> void put(std::string *s, T v) { s->append(reinterpret_cast<const char *>(&v), sizeof v); }
+template <class T> T at(const std::string &s, size_t off) { T v; memcpy(&v, s.data() + off, sizeof v); return v; }
+
+}  // namespace
+
+PostSums PostSums::of(const b200post_post_metadata &md, uint64_t file) {
+    PostSums s;
+    memcpy(s.node_id, md.node_id, 32);
+    memcpy(s.commitment_atx_id, md.commitment_atx_id, 32);
+    s.scrypt_n = md.scrypt_n; s.labels_per_file = md.max_file_size / 16; s.file = file;
+    return s;
+}
+
+int save_post_sums(const std::string &dir, const PostSums &s) {
+    if (s.digests.size() != s.blocks() * 32) return fail(B200POST_ERR_INVALID_ARGUMENT, "sidecar: digest count does not match its coverage");
+    std::string b(kSumsMagic, 8);
+    put<uint32_t>(&b, kSumsVersion);
+    put<uint32_t>(&b, (uint32_t)kSumBlockLabels);
+    b.append(reinterpret_cast<const char *>(s.node_id), 32);
+    b.append(reinterpret_cast<const char *>(s.commitment_atx_id), 32);
+    put<uint64_t>(&b, s.scrypt_n);
+    put<uint64_t>(&b, s.labels_per_file);
+    put<uint64_t>(&b, s.file);
+    put<uint64_t>(&b, s.covered);
+    b += s.digests;
+    put<uint64_t>(&b, fnv1a64(b.data(), b.size()));
+    return write_file_atomic(sums_path(dir, s.file), b);
+}
+
+bool load_post_sums(const std::string &dir, const b200post_post_metadata &md, uint64_t file, uint64_t max_labels, PostSums *out) {
+    std::string b;
+    if (!read_file(sums_path(dir, file), &b) || b.size() < kSumsHeader + 8) return false;
+    if (fnv1a64(b.data(), b.size() - 8) != at<uint64_t>(b, b.size() - 8)) return false;
+    PostSums s = PostSums::of(md, file);
+    if (b.compare(0, 8, kSumsMagic, 8) != 0 || at<uint32_t>(b, 8) != kSumsVersion || at<uint32_t>(b, 12) != kSumBlockLabels) return false;
+    if (memcmp(b.data() + 16, s.node_id, 32) || memcmp(b.data() + 48, s.commitment_atx_id, 32)) return false;
+    if (at<uint64_t>(b, 80) != s.scrypt_n || at<uint64_t>(b, 88) != s.labels_per_file || at<uint64_t>(b, 96) != file) return false;
+    s.covered = at<uint64_t>(b, 104);
+    if (s.covered > max_labels || s.covered > s.labels_per_file || b.size() != kSumsHeader + s.blocks() * 32 + 8) return false;
+    s.digests = b.substr(kSumsHeader, s.blocks() * 32);
+    *out = std::move(s);
+    return true;
 }
 
 }  // namespace b200post

@@ -22,10 +22,11 @@ extern const uint8_t kZeroChallenge[32];   // shared.ZeroChallenge: the challeng
 std::string join(const std::string &dir, const std::string &name);
 std::string postdata_path(const std::string &dir, uint64_t file);
 std::string range_record_path(const std::string &dir, uint64_t from_file, uint64_t to_file);
+std::string sums_path(const std::string &dir, uint64_t file);   // postdata_<file>.sum
 
 // Which of the directory's files a directory entry is.  *tmp (may be NULL): the entry is the ".tmp" of one of them,
 // left by an atomic write that did not finish.
-enum class PostFile { kNone, kLabels, kMetadata, kInitialProof, kInitialScan, kRangeRecord };
+enum class PostFile { kNone, kLabels, kMetadata, kInitialProof, kInitialScan, kRangeRecord, kSums };
 PostFile post_file_kind(const std::string &name, bool *tmp);
 
 // ---- layout: numLabels in files of MaxFileSize / 16 labels, the last one possibly shorter
@@ -89,5 +90,25 @@ int save_initial_proof_file(const std::string &dir, const b200post_proof_metadat
 // "no initial proof: <why>" otherwise
 int load_initial_proof_file(const std::string &dir, const b200post_post_metadata &md, const b200post_post_config &cfg, uint32_t nonces,
                             b200post_proof_out *out, b200post_proof_metadata *pm);
+
+// ---- postdata_<N>.sum (DESIGN.md §3g): BLAKE3 digests of one postdata file's labels in blocks of kSumBlockLabels,
+// aligned to the file's first label.  `covered` labels [0, covered) are described: every digest covers a whole block
+// except possibly the last, which covers [floor((covered - 1) / B) * B, covered).  Written only from labels computed
+// on a device (or, by b200post_write_sums, from stored bytes a full recomputation has just matched), never from bytes
+// read back: labels are deterministic, so no session makes a sidecar wrong, and labels past `covered` are unchecked.
+constexpr uint64_t kSumBlockLabels = 1ull << 16;   // 1 MiB of labels
+struct PostSums {
+    uint8_t node_id[32] = {0}, commitment_atx_id[32] = {0};
+    uint64_t scrypt_n = 0, labels_per_file = 0, file = 0, covered = 0;
+    std::string digests;   // ceil(covered / kSumBlockLabels) x 32 bytes
+    // the header of `file` of the POST md describes, covering nothing
+    static PostSums of(const b200post_post_metadata &md, uint64_t file);
+    uint64_t blocks() const { return (covered + kSumBlockLabels - 1) / kSumBlockLabels; }
+};
+int save_post_sums(const std::string &dir, const PostSums &s);
+// The sidecar of `file`: true with *out filled when it is intact (magic, version, block size, checksum, length), made
+// for this POST (NodeId, CommitmentAtxId, Scrypt.N, labels per file) and this file, and covers at most max_labels.
+// False when it is absent or unusable.
+bool load_post_sums(const std::string &dir, const b200post_post_metadata &md, uint64_t file, uint64_t max_labels, PostSums *out);
 
 }  // namespace b200post

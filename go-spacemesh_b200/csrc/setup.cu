@@ -17,6 +17,7 @@
 #include "engine.h"
 #include "host_hash.h"
 #include "initial_proof.h"
+#include "label_sums.h"
 #include "metrics.h"
 #include "postdata_io.h"
 #include "setup_internal.h"
@@ -80,6 +81,8 @@ struct b200post_setup_manager {
     std::string proof_err;
     b200post_proof_out proof{};
     b200post_proof_metadata proof_meta{};
+    // block checksums (b200post_setup_request_checksums): asked for between prepare and start
+    bool want_sums = false;
 };
 
 namespace {
@@ -89,6 +92,91 @@ int fail_state(b200post_setup_manager *m, int code, const std::string &msg) {
     set_error(msg);
     return code;
 }
+
+// The self-check of a batch: label `pick`, recomputed on the host CPU, against the device's label16
+int reference_check(const uint8_t commitment[32], uint64_t N, uint64_t pick, const uint8_t *label16) {
+    uint8_t ref[32];
+    reference_label32(commitment, pick, (uint32_t)N, ref);
+    if (memcmp(ref, label16, 16) == 0) return B200POST_OK;
+    metrics().setup_label_mismatch_total++;
+    return fail(B200POST_ERR_LABEL_MISMATCH, "reference label mismatch at index " + std::to_string(pick));
+}
+
+// The sidecars (postdata_<N>.sum, DESIGN.md §3g) of a session that asked for them.  They are built from the labels
+// the session computes, on its first device; labels already on disk are recomputed for them, never read back.
+class SessionSums {
+public:
+    SessionSums(std::string dir, const b200post_post_metadata &md, uint64_t num_labels)
+        : dir_(std::move(dir)), md_(md), lay_(num_labels, md.max_file_size / 16) {}
+
+    // Before the first batch: each file of the range with labels below `written` gets a sidecar covering them.  The
+    // whole blocks of a usable sidecar below the labels on disk are kept, and the rest, from the start of the block
+    // that holds its end (from label 0 of the file when the sidecar is absent or unusable), is recomputed and hashed.
+    // The initial-proof scan, the VRF scan and a range record never see these labels.
+    int begin(int64_t provider_id, uint64_t from_file, uint64_t written, uint64_t batch, const uint8_t commitment[32],
+              const volatile int *cancel) {
+        std::vector<uint32_t> devs;
+        if (int rc = provider_devices(provider_id, &devs)) return rc;
+        if (int rc = device_engine(devs[0])) return rc;
+        hasher_.reset(new BlockHasher((int)devs[0]));
+        std::vector<uint8_t> buf;
+        for (uint64_t f = from_file; f * lay_.per_file < written; f++) {
+            const uint64_t base = f * lay_.per_file, have = std::min<uint64_t>(lay_.labels_in(f), written - base);
+            PostSums old;
+            const bool usable = load_post_sums(dir_, md_, f, lay_.per_file, &old);
+            if (!usable) old = PostSums::of(md_, f);
+            const bool whole_file = have == lay_.labels_in(f);
+            if (usable && whole_file && old.covered == have) continue;   // nothing to add, nothing left open
+            open_.reset(new FileSums(old, std::min(old.covered, have) / kSumBlockLabels * kSumBlockLabels));
+            for (uint64_t at = open_->covered(); at < have;) {
+                if (cancel && *cancel) { save(); return fail(B200POST_ERR_CANCELLED, "cancelled"); }
+                const uint64_t n = std::min(batch, have - at);
+                buf.resize((size_t)n * 16);
+                int rc = compute_labels(provider_id, md_.scrypt_n, commitment, base + at, n, buf.data(), nullptr, nullptr, cancel);
+                if (!rc) rc = self_check(commitment, base + at, n, buf.data());
+                if (!rc) rc = open_->feed(*hasher_, buf.data(), n);
+                if (rc) { if (rc == B200POST_ERR_CANCELLED) save(); return rc; }
+                at += n;
+            }
+            if (int rc = save()) return rc;
+            if (whole_file) open_.reset();
+        }
+        return B200POST_OK;
+    }
+
+    // labels [pos, pos + count) of one file, as the session writes them.  The sidecar is saved when they complete a
+    // block and at the end of the file.
+    int batch(uint64_t pos, const uint8_t *labels, uint64_t count) {
+        const uint64_t f = pos / lay_.per_file, in_file = pos % lay_.per_file;
+        if (!open_ || open_->file() != f) open_.reset(new FileSums(PostSums::of(md_, f), 0));
+        if (open_->covered() != in_file) return fail(B200POST_ERR_STATE, "checksums: batch at label " + std::to_string(pos) + " does not continue the sidecar");
+        bool completed = false;
+        if (int rc = open_->feed(*hasher_, labels, count, &completed)) return rc;
+        const bool file_end = in_file + count == lay_.labels_in(f);
+        if (completed || file_end) {
+            if (int rc = save()) return rc;
+        }
+        if (file_end) open_.reset();
+        return B200POST_OK;
+    }
+
+    // the sidecar of the file the session is writing, as far as it got
+    int save() { return open_ ? open_->save(*hasher_, dir_) : B200POST_OK; }
+
+private:
+    // the session's self-check applied to one recomputed piece
+    int self_check(const uint8_t commitment[32], uint64_t start, uint64_t count, const uint8_t *labels) {
+        const uint64_t pick = start + (n_checked_++ * 2654435761ull) % count;
+        return reference_check(commitment, md_.scrypt_n, pick, labels + (pick - start) * 16);
+    }
+
+    std::string dir_;
+    b200post_post_metadata md_;
+    Layout lay_;
+    std::unique_ptr<BlockHasher> hasher_;
+    std::unique_ptr<FileSums> open_;
+    uint64_t n_checked_ = 0;
+};
 
 }  // namespace
 
@@ -134,7 +222,7 @@ int b200post_setup_prepare_files(b200post_setup_manager *m, const b200post_setup
         return B200POST_ERR_STATE;
     }
     // a request belongs to one prepared session, and so does its outcome
-    m->want_proof = m->proof_done = m->want_record = false;
+    m->want_proof = m->proof_done = m->want_record = m->want_sums = false;
     m->proof_rc = B200POST_OK; m->proof_err.clear();
     m->proof = b200post_proof_out{}; m->proof_meta = b200post_proof_metadata{};
     // ---- option validation (initialization.NewInitializer / config.Validate upstream; errors -> state Error, post.go:362-365)
@@ -224,7 +312,8 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
     // a range with a record scans its labels for the VRF into the record, not into the metadata
     const bool record = range && m->want_record;
     uint64_t written = lo + m->labels_written.load();   // the next label to write
-    const bool need_work = written < hi || (!range && (!m->meta.has_nonce || m->meta.vrf_scan_pending));
+    // a session with checksums may have sidecars to complete even when every label is on disk
+    const bool need_work = written < hi || (!range && (!m->meta.has_nonce || m->meta.vrf_scan_pending)) || m->want_sums;
     if (need_work && m->opts.provider_id == B200POST_PROVIDER_UNSET) {
         set_error("no provider specified");
         return finish(B200POST_SETUP_ERROR, B200POST_ERR_NO_PROVIDER);
@@ -254,8 +343,26 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
             if (ip->vrf().found) memcpy(diff, ip->vrf().label32, 32);
         }
     }
-    // from here on a stop or failure first saves the initial proof's scan state
-    auto end = [&](int32_t state, int rc) { if (ip) ip->stop(); return finish(state, rc); };
+    // the sidecars: completed up to the resume point before the first batch
+    std::unique_ptr<SessionSums> sums;
+    if (m->want_sums) {
+        sums.reset(new SessionSums(m->data_dir, m->meta, lay.num_labels));
+        const int rc = sums->begin(m->opts.provider_id, m->range_from, written, batch, commitment, cancel);
+        if (rc) {
+            if (ip) ip->stop();
+            return finish(rc == B200POST_ERR_CANCELLED ? B200POST_SETUP_STOPPED : B200POST_SETUP_ERROR, rc);
+        }
+    }
+    // from here on a stop or failure first saves the initial proof's scan state and the open sidecar
+    auto end = [&](int32_t state, int rc) {
+        if (ip) ip->stop();
+        if (sums) {
+            const std::string err = last_error();
+            sums->save();   // best effort: the session's own outcome is what it reports
+            set_error(err);
+        }
+        return finish(state, rc);
+    };
 
     std::vector<uint8_t> buf;
     uint64_t n_batches = 0;
@@ -285,23 +392,18 @@ int b200post_setup_start_session(b200post_setup_manager *m, const volatile int *
         // host) and compared with what the device wrote — independent of the device, its kernels' scheduling and memory.
         if (options().debug_corrupt_next_batch.exchange(0) != 0 && count) labels[((n_batches * 7) % count) * 16 + 3] ^= 0x40;   // fault injection (tests)
         if (n_batches % m->opts.self_check_every == 0) {
-            uint8_t ref[32];
             uint64_t pick = written + (n_batches * 2654435761ull) % count;
             if (options().debug_corrupt_check_all.load() != 0) {
                 // test hook: check the label the injected fault hit (the sampled one is elsewhere with probability 1 - 1/count)
                 pick = written + (n_batches * 7) % count;
             }
-            reference_label32(commitment, pick, (uint32_t)m->opts.scrypt_n, ref);
-            if (memcmp(ref, labels + (pick - written) * 16, 16)) {
-                metrics().setup_label_mismatch_total++;
-                set_error("reference label mismatch at index " + std::to_string(pick));
-                return end(B200POST_SETUP_ERROR, B200POST_ERR_LABEL_MISMATCH);
-            }
+            if ((rc = reference_check(commitment, m->opts.scrypt_n, pick, labels + (pick - written) * 16))) return end(B200POST_SETUP_ERROR, rc);
         }
         n_batches++;
         // a record's VRF best covers every batch that its scan folds: it is noted before the batch goes to the scan
         if (record && nn.found) { ip->note_vrf(nn); memcpy(diff, nn.label32, 32); }
         if ((rc = write_labels(m->data_dir, file_idx, in_file, labels, count))) return end(B200POST_SETUP_ERROR, rc);
+        if (sums && (rc = sums->batch(written, labels, count))) return end(B200POST_SETUP_ERROR, rc);
         // the scan of this batch overlaps the computation of the next one
         if (ip && (rc = ip->scan(written, count, labels))) return end(B200POST_SETUP_ERROR, rc);
         written += count;
@@ -370,7 +472,7 @@ int b200post_setup_reset(b200post_setup_manager *m) {
     }
     m->labels_written.store(0);
     memset(&m->meta, 0, sizeof m->meta);
-    m->want_proof = m->proof_done = m->want_record = false;
+    m->want_proof = m->proof_done = m->want_record = m->want_sums = false;
     m->state = B200POST_SETUP_NOT_STARTED;
     return B200POST_OK;
 }
@@ -435,6 +537,14 @@ int b200post_setup_request_range_record(b200post_setup_manager *m, const b200pos
     }
     m->want_record = true;
     m->record_proof = proof != nullptr;
+    return B200POST_OK;
+}
+
+int b200post_setup_request_checksums(b200post_setup_manager *m) {
+    if (!m) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    std::lock_guard<std::mutex> lk(m->mu);
+    if (m->state != B200POST_SETUP_PREPARED) { set_error("post session not prepared"); return B200POST_ERR_STATE; }
+    m->want_sums = true;
     return B200POST_OK;
 }
 

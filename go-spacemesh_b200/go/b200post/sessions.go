@@ -806,3 +806,125 @@ func GenerateProofs(ctx context.Context, providers []uint32, items []ProveItem, 
 	}
 	return out, nil
 }
+
+// ---------------------------------------------------------------------------------------------------------
+// Block checksums: postdata_<N>.sum, one BLAKE3 digest per 1 MiB block of labels (DESIGN.md §3g)
+// ---------------------------------------------------------------------------------------------------------
+
+// SumBlockLabels is the number of labels in one checksummed block (1 MiB).
+const SumBlockLabels = 1 << 16
+
+// RequestChecksums asks the prepared session (whole POST or file range) to write postdata_<N>.sum for every file it
+// writes, from the labels it computes.  Labels already on disk that no usable sidecar covers are recomputed for it,
+// not read back.  Call it between PrepareInitializer (or PrepareFiles) and StartSession.
+func (m *SetupManager) RequestChecksums() error {
+	return setupErr(checked(func() C.int { return C.b200post_setup_request_checksums(m.h) }))
+}
+
+// LabelBlockDigests returns the BLAKE3 digest of each block of SumBlockLabels labels of labels (16 bytes each), the
+// last block possibly short, hashed on one GPU.
+func LabelBlockDigests(provider uint32, labels []byte) ([][32]byte, error) {
+	if len(labels)%16 != 0 {
+		return nil, fmt.Errorf("labels are 16 bytes each, got %d bytes", len(labels))
+	}
+	n := uint64(len(labels) / 16)
+	if n == 0 {
+		return nil, nil
+	}
+	out := make([][32]byte, (n+SumBlockLabels-1)/SumBlockLabels)
+	rc, msg := checked(func() C.int {
+		return C.b200post_label_block_digests(C.uint32_t(provider), (*C.uint8_t)(unsafe.Pointer(&labels[0])), C.uint64_t(n),
+			(*C.uint8_t)(unsafe.Pointer(&out[0][0])))
+	})
+	if err := setupErr(rc, msg); err != nil {
+		return nil, err
+	}
+	return out, nil
+}
+
+type SumsOpts struct {
+	ProviderID uint32  // CheckSums: a CUDA ordinal; WriteSums: a CUDA ordinal or AllProviders
+	FromFile   uint64
+	ToFile     int64   // inclusive; -1 = the last file
+	Progress   *uint64 // optional: labels hashed (CheckSums) or recomputed and compared (WriteSums) so far
+	Repair     bool    // CheckSums: rewrite each bad block from its recomputation, once that matches its checksum
+}
+
+// SumsBlock is one bad block: the global index of its first label and its label count.
+type SumsBlock struct{ FirstLabel, Count uint64 }
+
+type SumsResult struct {
+	FilesChecked, FilesUnchecked              uint64      // CheckSums: files with / without a usable sidecar; WriteSums: files given one / with a mismatch
+	LabelsChecked, LabelsUnchecked, BytesRead uint64
+	BlocksChecked, BadBlocks, RepairedBlocks  uint64
+	Bad                                       []SumsBlock // the lowest bad blocks, ascending (<= 64)
+}
+
+func sumsCall(ctx context.Context, dataDir string, o SumsOpts, write bool) (*SumsResult, error) {
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var co C.b200post_sums_opts
+	C.b200post_default_sums_opts(&co)
+	if o.ProviderID == AllProviders {
+		co.provider_id = C.B200POST_PROVIDER_ALL
+	} else {
+		co.provider_id = C.int64_t(o.ProviderID)
+	}
+	co.from_file, co.to_file = C.uint64_t(o.FromFile), C.int64_t(o.ToFile)
+	if o.Repair {
+		co.repair = 1
+	}
+	if o.Progress != nil {
+		var pin runtime.Pinner
+		pin.Pin(o.Progress)
+		defer pin.Unpin()
+		co.progress = (*C.uint64_t)(unsafe.Pointer(o.Progress))
+	}
+	var cancel int32
+	done := make(chan struct{})
+	defer close(done)
+	go func() {
+		select {
+		case <-ctx.Done():
+			atomic.StoreInt32(&cancel, 1)
+		case <-done:
+		}
+	}()
+	var out C.b200post_sums_result
+	rc, msg := checked(func() C.int {
+		if write {
+			return C.b200post_write_sums(dir, &co, &out, (*C.int)(unsafe.Pointer(&cancel)))
+		}
+		return C.b200post_check_sums(dir, &co, &out, (*C.int)(unsafe.Pointer(&cancel)))
+	})
+	r := &SumsResult{FilesChecked: uint64(out.files_checked), FilesUnchecked: uint64(out.files_unchecked),
+		LabelsChecked: uint64(out.labels_checked), LabelsUnchecked: uint64(out.labels_unchecked), BytesRead: uint64(out.bytes_read),
+		BlocksChecked: uint64(out.blocks_checked), BadBlocks: uint64(out.bad_blocks), RepairedBlocks: uint64(out.repaired_blocks)}
+	for i := 0; i < int(out.n_reported); i++ {
+		r.Bad = append(r.Bad, SumsBlock{uint64(out.bad[i].first_label), uint64(out.bad[i].count)})
+	}
+	switch {
+	case rc == C.B200POST_OK, rc == C.B200POST_ERR_LABEL_MISMATCH, rc == C.B200POST_ERR_CANCELLED,
+		rc == C.B200POST_ERR_STATE && out.labels_checked > 0:
+		return r, setupErr(rc, msg)
+	}
+	return nil, setupErr(rc, msg)
+}
+
+// CheckSums reads the covered labels of the files and compares each 1 MiB block with its postdata_<N>.sum at storage
+// speed.  Bad blocks return the result with ErrLabelMismatch (none left after a successful Repair); labels without a
+// checksum return the result with an ErrState-class error (the check is incomplete); a range with no checksum at all
+// is an error without a result.
+func CheckSums(ctx context.Context, dataDir string, o SumsOpts) (*SumsResult, error) {
+	return sumsCall(ctx, dataDir, o, false)
+}
+
+// WriteSums gives sidecars to data that has none: VerifyPos at fraction 100 over the files, and a sidecar for each file
+// whose labels all match, byte-identical to the one an init with RequestChecksums writes.  A file with a mismatch gets
+// none: the result with ErrLabelMismatch.  It costs one full check.
+func WriteSums(ctx context.Context, dataDir string, o SumsOpts) (*SumsResult, error) {
+	if o.Repair {
+		return nil, fmt.Errorf("WriteSums does not repair: use CheckSums")
+	}
+	return sumsCall(ctx, dataDir, o, true)
+}

@@ -56,6 +56,22 @@ class _VrfSearchOpts(ctypes.Structure):
                 ("progress", ctypes.c_void_p)]
 
 
+class _SumsOpts(ctypes.Structure):
+    _fields_ = [("provider_id", ctypes.c_int64), ("from_file", ctypes.c_uint64), ("to_file", ctypes.c_int64),
+                ("progress", ctypes.c_void_p), ("repair", ctypes.c_uint32)]
+
+
+class _SumsBlock(ctypes.Structure):
+    _fields_ = [("first_label", ctypes.c_uint64), ("count", ctypes.c_uint64)]
+
+
+class _SumsResult(ctypes.Structure):
+    _fields_ = [("files_checked", ctypes.c_uint64), ("files_unchecked", ctypes.c_uint64), ("labels_checked", ctypes.c_uint64),
+                ("labels_unchecked", ctypes.c_uint64), ("bytes_read", ctypes.c_uint64), ("blocks_checked", ctypes.c_uint64),
+                ("bad_blocks", ctypes.c_uint64), ("repaired_blocks", ctypes.c_uint64), ("n_reported", ctypes.c_uint32),
+                ("reserved", ctypes.c_uint32), ("bad", _SumsBlock * 64)]
+
+
 class _MergeOpts(ctypes.Structure):
     _fields_ = [("provider_id", ctypes.c_int64), ("compute_batch_size", ctypes.c_uint64)]
 
@@ -90,6 +106,23 @@ class VerifyPosResult:       # b200post_verify_pos_result; `code` is the call's 
     argmin_checked: bool
     argmin_ok: bool
     bad_index: list[int]
+
+
+@dataclass
+class SumsResult:            # b200post_sums_result; `code` is the call's status (OK, ERR_LABEL_MISMATCH, ERR_STATE, ERR_CANCELLED)
+    code: int
+    files_checked: int       # check: files with a usable sidecar; write_sums: files given one
+    files_unchecked: int     # check: files without one; write_sums: files with a mismatch (no sidecar)
+    labels_checked: int
+    labels_unchecked: int
+    bytes_read: int
+    blocks_checked: int
+    bad_blocks: int
+    repaired_blocks: int
+    bad: list[tuple[int, int]]   # the lowest bad blocks: (first global label, label count), ascending
+
+
+SUM_BLOCK_LABELS = 1 << 16   # labels per checksummed block (1 MiB)
 
 
 @dataclass
@@ -149,6 +182,10 @@ def _bind():
     L.b200post_load_initial_proof.argtypes = [ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.c_uint32, vp, vp]
     L.b200post_setup_request_range_record.argtypes = [vp, vp]
     L.b200post_merge_range_records.argtypes = [ctypes.c_char_p, vp, ctypes.POINTER(_MergeOpts), vp, vp]
+    L.b200post_label_block_digests.argtypes = [ctypes.c_uint32, vp, ctypes.c_uint64, vp]
+    L.b200post_setup_request_checksums.argtypes = [vp]
+    L.b200post_check_sums.argtypes = [ctypes.c_char_p, ctypes.POINTER(_SumsOpts), ctypes.POINTER(_SumsResult), vp]
+    L.b200post_write_sums.argtypes = [ctypes.c_char_p, ctypes.POINTER(_SumsOpts), ctypes.POINTER(_SumsResult), vp]
     L._setup_bound = True
     return L
 
@@ -194,6 +231,46 @@ def verify_pos(data_dir: str, *, fraction: float = 0.2, provider_id: int = 0, fr
         _err(rc)
     return VerifyPosResult(rc, r.files_checked, r.labels_checked, r.mismatches, r.seed, bool(r.nonce_ok), bool(r.argmin_checked),
                            bool(r.argmin_ok), [int(r.bad_index[i]) for i in range(r.n_reported)])
+
+
+def label_block_digests(labels, provider_id: int = 0):
+    """BLAKE3 digests of labels (bytes or a uint8 array of n x 16 bytes) in blocks of SUM_BLOCK_LABELS from the first,
+    the last one possibly short, hashed on CUDA ordinal provider_id: an (ceil(n / 2^16), 32) uint8 array."""
+    import numpy as np
+    a = np.ascontiguousarray(np.frombuffer(labels, dtype=np.uint8) if isinstance(labels, (bytes, bytearray)) else labels, dtype=np.uint8).reshape(-1)
+    if a.size % 16:
+        raise ValueError("labels are 16 bytes each")
+    n = a.size // 16
+    out = np.empty(((n + SUM_BLOCK_LABELS - 1) // SUM_BLOCK_LABELS, 32), dtype=np.uint8)
+    _err(_bind().b200post_label_block_digests(provider_id, a.ctypes.data, n, out.ctypes.data))
+    return out
+
+
+def _sums_call(fn, data_dir, provider_id, from_file, to_file, repair, progress, cancel) -> SumsResult:
+    o = _SumsOpts(provider_id, from_file, to_file, ctypes.addressof(progress) if progress is not None else None, int(repair))
+    r = _SumsResult()
+    rc = fn(data_dir.encode(), ctypes.byref(o), ctypes.byref(r), ctypes.addressof(cancel) if cancel is not None else None)
+    if rc not in (OK, ERR_LABEL_MISMATCH, ERR_STATE, ERR_CANCELLED) or (rc == ERR_STATE and r.labels_checked == 0):
+        _err(rc)
+    return SumsResult(rc, r.files_checked, r.files_unchecked, r.labels_checked, r.labels_unchecked, r.bytes_read, r.blocks_checked,
+                      r.bad_blocks, r.repaired_blocks, [(int(r.bad[i].first_label), int(r.bad[i].count)) for i in range(r.n_reported)])
+
+
+def check_sums(data_dir: str, *, provider_id: int = 0, from_file: int = 0, to_file: int = -1, repair: bool = False,
+               progress: ctypes.c_uint64 | None = None, cancel: ctypes.c_int | None = None) -> SumsResult:
+    """b200postcli -checkSums: read the covered labels of files [from_file, to_file], hash them on the GPU and compare
+    every 1 MiB block with its postdata_<N>.sum.  repair=True rewrites each bad block from its recomputation once that
+    matches the checksum.  Returns the result for OK, ERR_LABEL_MISMATCH (bad blocks left), ERR_STATE (labels without a
+    checksum) and ERR_CANCELLED; raises on other errors, and on ERR_STATE "no checksums" when nothing is covered."""
+    return _sums_call(_bind().b200post_check_sums, data_dir, provider_id, from_file, to_file, repair, progress, cancel)
+
+
+def write_sums(data_dir: str, *, provider_id: int = 0, from_file: int = 0, to_file: int = -1,
+               progress: ctypes.c_uint64 | None = None, cancel: ctypes.c_int | None = None) -> SumsResult:
+    """b200postcli -verify -fraction 100 -writeSums: the full check of verify_pos over files [from_file, to_file]; every
+    file whose labels all match gets its postdata_<N>.sum from the verified bytes.  Returns the result for OK,
+    ERR_LABEL_MISMATCH (files with a mismatch got none) and ERR_CANCELLED; raises on other errors."""
+    return _sums_call(_bind().b200post_write_sums, data_dir, provider_id, from_file, to_file, False, progress, cancel)
 
 
 def load_initial_proof(data_dir: str, cfg: PostConfig, nonces: int = 16):
@@ -305,6 +382,12 @@ class PostSetupManager:
             opts.pow_cache_key, opts.pow_cache_key_len = pow_cache_key, len(pow_cache_key)
         self._initial_opts = opts   # keeps a pow callback alive for the session
         _err(_bind().b200post_setup_request_range_record(self._h, ctypes.byref(opts)))
+
+    def request_checksums(self) -> None:
+        """Ask the prepared session to write postdata_<N>.sum (block checksums) for every file it writes, from the
+        labels it computes; labels already on disk are recomputed for them, not read back.  Call between prepare and
+        start_session."""
+        _err(_bind().b200post_setup_request_checksums(self._h))
 
     def initial_proof(self):
         """After a completed session that asked for it: (Proof, ProofMetadata, labels scanned).  Raises ERR_INVALID_PROOF

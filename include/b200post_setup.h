@@ -191,6 +191,81 @@ void b200post_default_vrf_search_opts(b200post_vrf_search_opts *o);
 int b200post_search_vrf_nonce(const char *data_dir, const b200post_vrf_search_opts *o, b200post_vrf_nonce *out,
                               const volatile int *cancel);
 
+/*
+ * Block checksums (DESIGN.md §3g).  A block is B = 2^16 labels (1 MiB) of one postdata_N.bin, aligned to the file's
+ * first label; the file's last block may be shorter.  Its digest is unkeyed BLAKE3 of its bytes (32 bytes).  The
+ * sidecar postdata_N.sum holds the digests of the file's labels [0, covered): whole blocks, except possibly the last,
+ * which covers [floor((covered - 1) / B) * B, covered).  Sidecars are made only from labels computed on a device, never
+ * from bytes read back (b200post_write_sums: only after every label of the file was recomputed and matched), so no
+ * session makes one wrong; labels past `covered` are unchecked.  libpost's readers look only at postdata_<N>.bin
+ * (recalled, unpinned), so the sidecars do not disturb them.
+ */
+
+/* The digests of `count` labels (count x 16 bytes, host memory) split into blocks of 2^16 labels from the first, the
+ * last one short: ceil(count / 2^16) x 32 bytes into digests32, hashed on CUDA ordinal `provider`. */
+int b200post_label_block_digests(uint32_t provider, const uint8_t *labels16, uint64_t count, uint8_t *digests32);
+
+/* Ask the prepared session (whole POST or file range, with or without an initial proof or a range record) to write
+ * postdata_N.sum for every file it writes, from the labels it computes, hashed on its first device after the
+ * self-check.  A sidecar is saved after every batch that completes a block, at the end of each file, and when the
+ * session stops or fails.  On resume, the whole blocks of a usable sidecar below the labels on disk are kept and the
+ * rest of those labels (from label 0 when the sidecar is absent, damaged or made for another identity, N, file size or
+ * file) is recomputed and hashed first, not read back; the initial-proof scan, the VRF scan and a range record never
+ * see them.  The labels, the metadata, initial_post.json and range records are byte-identical to a session without
+ * the request.  Call between prepare and start; prepare clears the request. */
+int b200post_setup_request_checksums(b200post_setup_manager *mgr);
+
+typedef struct b200post_sums_opts {
+    int64_t provider_id;         /* check: a CUDA ordinal; write: a CUDA ordinal or B200POST_PROVIDER_ALL      */
+    uint64_t from_file;          /* first postdata_N.bin                                                      */
+    int64_t to_file;             /* last file, inclusive; -1 = the POST's last file                           */
+    volatile uint64_t *progress; /* optional: labels hashed (check) or recomputed and compared (write) so far */
+    uint32_t repair;             /* check only: 1 = rewrite each bad block from its recomputation             */
+} b200post_sums_opts;
+
+typedef struct b200post_sums_block {
+    uint64_t first_label;        /* global label index of the block's first label */
+    uint64_t count;              /* its labels                                     */
+} b200post_sums_block;
+
+typedef struct b200post_sums_result {
+    uint64_t files_checked;      /* check: files with a usable sidecar; write: files given one                */
+    uint64_t files_unchecked;    /* check: files without a usable sidecar; write: files with a mismatch       */
+    uint64_t labels_checked, labels_unchecked;
+    uint64_t bytes_read;
+    uint64_t blocks_checked, bad_blocks, repaired_blocks;
+    uint32_t n_reported;
+    uint32_t reserved;
+    b200post_sums_block bad[64]; /* the lowest bad blocks, ascending                                          */
+} b200post_sums_result;
+
+/* provider 0, all files, no progress, no repair */
+void b200post_default_sums_opts(b200post_sums_opts *o);
+
+/*
+ * Check stored labels against their sidecars at storage speed: the covered labels of files [from_file, to_file] are
+ * read (pinned, double-buffered), hashed on the device and compared block by block.  Host checks first, in order:
+ * bad arguments -> INVALID_ARGUMENT; no metadata -> ERR_IO; a missing or short file -> ERR_IO "incomplete"; a file
+ * without a usable sidecar is counted unchecked, and when no label of the range is covered -> ERR_STATE "no checksums";
+ * then UNSUPPORTED for the CPU id or NO_DEVICE.  Returns LABEL_MISMATCH when a block differs (the lowest 64 reported),
+ * else ERR_STATE when labels were unchecked, else OK; `out` is filled in each case.
+ * repair = 1: each bad block is recomputed under the metadata's N and hashed; its digest must equal the sidecar's (else
+ * LABEL_MISMATCH "recomputed block disagrees with its checksum", nothing written), then it is written with pwrite,
+ * fdatasync'ed, read back and hashed again.  Repaired blocks no longer count towards LABEL_MISMATCH.  Repair never
+ * touches the metadata, the nonce, initial_post.json or records; a missing or short file is a range session's job.
+ */
+int b200post_check_sums(const char *data_dir, const b200post_sums_opts *o, b200post_sums_result *out, const volatile int *cancel);
+
+/*
+ * Sidecars for data that has none (written by libpost, earlier sessions, or without the request): the full check of
+ * b200post_verify_pos (fraction 100, every label recomputed and compared) over files [from_file, to_file], and for each
+ * file whose labels all match, the sidecar from the digests of those verified bytes, byte-identical to the one an init
+ * with checksums writes.  A file with a mismatch gets none and is counted in files_unchecked, its damaged blocks
+ * reported (from the lowest mismatching labels of each compare call): LABEL_MISMATCH.  Host checks as above (no
+ * sidecar needed).  Costs one full check.
+ */
+int b200post_write_sums(const char *data_dir, const b200post_sums_opts *o, b200post_sums_result *out, const volatile int *cancel);
+
 #ifdef __cplusplus
 }
 #endif
