@@ -62,14 +62,10 @@ __device__ __forceinline__ void load_iv(uint32_t cv[8]) {
     cv[4] = 0x510E527Fu; cv[5] = 0x9B05688Cu; cv[6] = 0x1F83D9ABu; cv[7] = 0x5BE0CD19u;
 }
 
-// Blocks [0, full_blocks) of 1 MiB, then, when last_bytes > 0, one short block of last_bytes (a multiple of 16) bytes:
-// the digest of block b goes to out[32 b, 32 b + 32).
-__global__ void __launch_bounds__(kSumThreads) label_block_digests_kernel(const uint8_t *__restrict__ labels, uint32_t full_blocks,
-                                                                          uint32_t last_bytes, uint8_t *__restrict__ out) {
+// The digest of one block of `bytes` (a positive multiple of 16, at most kBlockBytes) at base, by the whole CTA, into
+// out[0, 32).  Shared by the kernel over host-copied blocks and the one over ranges of a device-resident chunk.
+__device__ __forceinline__ void hash_block(const uint8_t *__restrict__ base, uint32_t bytes, uint8_t *__restrict__ out) {
     __shared__ uint32_t cvs[kMaxChunks][8];
-    const uint32_t b = blockIdx.x;
-    const uint32_t bytes = b < full_blocks ? kBlockBytes : last_bytes;
-    const uint8_t *base = labels + (size_t)b * kBlockBytes;
     const uint32_t n_chunks = (bytes + kChunkBytes - 1) / kChunkBytes;
     const uint32_t root_chunk = n_chunks == 1 ? ROOT : 0;
 
@@ -126,7 +122,23 @@ __global__ void __launch_bounds__(kSumThreads) label_block_digests_kernel(const 
         }
         __syncthreads();
     }
-    if (threadIdx.x < 8) reinterpret_cast<uint32_t *>(out + (size_t)b * 32)[threadIdx.x] = cvs[0][threadIdx.x];
+    if (threadIdx.x < 8) reinterpret_cast<uint32_t *>(out)[threadIdx.x] = cvs[0][threadIdx.x];
+}
+
+// Blocks [0, full_blocks) of 1 MiB, then, when last_bytes > 0, one short block of last_bytes (a multiple of 16) bytes:
+// the digest of block b goes to out[32 b, 32 b + 32).
+__global__ void __launch_bounds__(kSumThreads) label_block_digests_kernel(const uint8_t *__restrict__ labels, uint32_t full_blocks,
+                                                                          uint32_t last_bytes, uint8_t *__restrict__ out) {
+    const uint32_t b = blockIdx.x;
+    hash_block(labels + (size_t)b * kBlockBytes, b < full_blocks ? kBlockBytes : last_bytes, out + (size_t)b * 32);
+}
+
+// One CTA per range of a chunk already in device memory: range b is desc[b] (byte offset into chunk, bytes), its
+// digest goes to out[32 b, 32 b + 32).  The proving scan's digests (b200post_generate_proof_sums).
+__global__ void __launch_bounds__(kSumThreads) label_range_digests_kernel(const uint8_t *__restrict__ chunk, const DigestDesc *__restrict__ desc,
+                                                                          uint8_t *__restrict__ out) {
+    const DigestDesc d = desc[blockIdx.x];
+    hash_block(chunk + d.offset, d.bytes, out + (size_t)blockIdx.x * 32);
 }
 
 }  // namespace
@@ -203,6 +215,13 @@ int FileSums::save(BlockHasher &h, const std::string &dir) {
     PostSums s;
     if (int rc = sums(h, &s)) return rc;
     return save_post_sums(dir, s);
+}
+
+cudaError_t launch_range_digests(cudaStream_t st, const uint8_t *d_chunk, const DigestDesc *d_desc, uint32_t n, uint8_t *d_out) {
+    if (n == 0) return cudaSuccess;
+    label_range_digests_kernel<<<n, kSumThreads, 0, st>>>(d_chunk, d_desc, d_out);
+    g_launches++;
+    return cudaGetLastError();
 }
 
 }  // namespace b200post

@@ -25,6 +25,13 @@ private:
     DeviceBuffer<uint8_t> d_in_, d_out_;
 };
 
+// One digest range of a chunk already in device memory: `bytes` (a positive multiple of 16, at most 1 MiB) from byte
+// `offset` of the chunk
+struct DigestDesc { uint64_t offset; uint32_t bytes, pad; };
+// Enqueues on `st` the digests of the n ranges d_desc[0, n) (device) of the chunk at d_chunk, one CTA each: range i's
+// digest into d_out[32 i, 32 i + 32).  The proving scan's check of each chunk against its sidecars.
+cudaError_t launch_range_digests(cudaStream_t st, const uint8_t *d_chunk, const DigestDesc *d_desc, uint32_t n, uint8_t *d_out);
+
 // The sidecar of one file under construction: feed() takes the file's labels in order from sums().covered on, hashes
 // every block they complete, and keeps the bytes of a block they leave open; save() hashes that open block as the
 // sidecar's short last one and writes the file.  The bytes fed are hashed, never read back from disk.

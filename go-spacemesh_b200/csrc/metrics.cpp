@@ -60,6 +60,9 @@ extern "C" size_t b200post_metrics_text(char *buf, size_t cap) {
     line("b200post_sums_blocks_checked_total", "1 MiB label blocks hashed and compared with their checksums (check_sums, write_sums)", "counter", m.sums_blocks_checked_total);
     line("b200post_sums_blocks_bad_total", "label blocks whose stored bytes differed from their checksum or recomputation", "counter", m.sums_blocks_bad_total);
     line("b200post_sums_blocks_repaired_total", "damaged label blocks recomputed and written back (check_sums -repair)", "counter", m.sums_blocks_repaired_total);
+    line("b200post_prove_sum_blocks_checked_total", "label blocks the proving scan hashed and compared with their checksums (checksummed proofs)", "counter", m.prove_sum_blocks_checked_total);
+    line("b200post_prove_sum_blocks_bad_total", "label blocks of checksummed proofs whose stored digest differed from their checksum", "counter", m.prove_sum_blocks_bad_total);
+    line("b200post_prove_sum_blocks_healed_total", "bad label blocks a checksummed proof recomputed and scanned from the recomputation", "counter", m.prove_sum_blocks_healed_total);
     if (buf && cap) {
         const size_t n = o.size() < cap - 1 ? o.size() : cap - 1;
         memcpy(buf, o.data(), n);

@@ -25,6 +25,8 @@ struct Metrics {
     std::atomic<uint64_t> post_data_labels_verified_total{0}, post_data_label_mismatch_total{0};   // b200post_verify_pos
     // block checksums: blocks hashed and compared (check_sums, write_sums), found damaged, rewritten by a repair
     std::atomic<uint64_t> sums_blocks_checked_total{0}, sums_blocks_bad_total{0}, sums_blocks_repaired_total{0};
+    // b200post_generate_proof_sums: digest ranges the scan hashed and compared, found bad, recomputed and scanned
+    std::atomic<uint64_t> prove_sum_blocks_checked_total{0}, prove_sum_blocks_bad_total{0}, prove_sum_blocks_healed_total{0};
 };
 Metrics &metrics();
 void observe_verify_seconds(double s);

@@ -8,10 +8,10 @@
 
 namespace b200post {
 
-void HitBook::add(uint32_t nonce, uint64_t index, const uint8_t *label) {
+void HitBook::add(uint32_t nonce, uint64_t index, const uint8_t *label, bool good) {
     std::vector<KeptHit> &l = lists_[nonce];
     if (born_good_ && l.size() >= k2_) return;   // hits past a nonce's K2-th good one never count
-    KeptHit k{index, {}, born_good_};
+    KeptHit k{index, {}, born_good_ || good};
     if (label) memcpy(k.label, label, 16);
     l.push_back(k);
     full_ += l.size() == k2_;

@@ -26,8 +26,9 @@ public:
     using Lists = std::map<uint32_t, std::vector<KeptHit>>;   // ordered, so ties resolve to the lower nonce
 
     HitBook(uint32_t nonces, uint32_t k2, bool born_good) : nonces_(nonces), k2_(k2), born_good_(born_good) {}
-    // a hit above every earlier hit of its nonce; `label`: its 16 stored bytes, or nullptr
-    void add(uint32_t nonce, uint64_t index, const uint8_t *label);
+    // a hit above every earlier hit of its nonce; `label`: its 16 stored bytes, or nullptr.  good: known to be the
+    // real label already (a checksummed proof's covered hit), even in a book whose hits are born pending
+    void add(uint32_t nonce, uint64_t index, const uint8_t *label, bool good = false);
     void advance(uint64_t labels) { scanned_ += labels; }
     // a recheck's verdict on a hit, if it is still kept: good, or damaged and removed
     void settle(uint32_t nonce, uint64_t index, bool damaged);

@@ -13,6 +13,11 @@
 // kernels also return each hit's stored bytes (StoredHit), and the tentative winner has its first K2 hits recomputed and
 // compared on the device before the scan may stop on it; damaged hits are dropped (DESIGN.md §5).
 //
+// Checksummed data (b200post_generate_proof_sums): the checked scan over a chunk plan of whole digest ranges
+// (sums_plan.h).  Each chunk's covered ranges are hashed on the device after its H2D and compared with their sidecar at
+// collect; a bad range is recomputed into the chunk's device buffer and scanned again, covered hits are folded good and
+// only uncovered ones pending (DESIGN.md §5).
+//
 // Nonce windows (b200post_prove_opts.max_windows): generate() runs passes over the data, each scanning windows_per_pass
 // windows of nonces with their own pows, until a window has a proof; the kernels only ever see pass-relative nonces.
 //
@@ -210,25 +215,66 @@ int Scanner::init(uint32_t provider, const uint8_t challenge[32], uint32_t nonce
 }
 
 template <class Rec>
-void Scanner::launch(cudaStream_t st, const uint4 *labels, uint64_t first, uint32_t count, Rec *hits, uint32_t *n_hits) {
+void Scanner::launch(cudaStream_t st, const uint4 *labels, uint64_t first, uint32_t count, Rec *hits, uint32_t *n_hits, uint2 *cands,
+                     uint32_t cand_cap, uint32_t *n_cands) {
     prove_scan_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, count, reinterpret_cast<const uint4 *>(d_rk_.get()), nonces_ / 16,
-                                                               msb_, d_tables_.get(), hits, hit_cap_, n_hits, d_cands_.get(), cand_cap_,
-                                                               d_ncands_.get());
-    prove_lazy_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, d_cands_.get(), d_ncands_.get(), cand_cap_,
+                                                               msb_, d_tables_.get(), hits, hit_cap_, n_hits, cands, cand_cap, n_cands);
+    prove_lazy_kernel<Rec><<<grid_, 256, AES_SMEM_BYTES, st>>>(labels, first, cands, n_cands, cand_cap,
                                                                reinterpret_cast<const uint4 *>(d_lazy_.get()), lsb_, d_tables_.get(),
                                                                hits, hit_cap_, n_hits);
 }
 
-int Scanner::submit(int b, uint64_t first, uint32_t count) {
+int Scanner::use_sums(SumsCheck *sums, const uint8_t commitment[32], uint64_t N, size_t max_ranges, const volatile int *cancel) {
+    if (!stored_) { set_error("a checksummed scan keeps its hits' stored bytes"); return B200POST_ERR_INVALID_ARGUMENT; }
+    sums_ = sums; N_ = N; cancel_ = cancel;
+    memcpy(commitment_, commitment, 32);
+    CUDA_TRY(cudaSetDevice(dev_));
+    const size_t n = std::max<size_t>(max_ranges, 1);
+    for (int b = 0; b < 2; b++) {
+        CUDA_TRY(h_desc_[b].resize(n));
+        CUDA_TRY(d_desc_[b].resize(n));
+        CUDA_TRY(h_dig_[b].resize(n * 32));
+        CUDA_TRY(d_dig_[b].resize(n * 32));
+        hashed_[b].reserve(n);
+    }
+    heal_cand_cap_ = (uint32_t)((kSumBlockLabels * nonces_) / 128 + 65536);
+    CUDA_TRY(d_heal_hits_.resize((size_t)hit_cap_ * rec_));
+    CUDA_TRY(h_heal_hits_.resize((size_t)hit_cap_ * rec_));
+    CUDA_TRY(d_heal_cands_.resize(heal_cand_cap_));
+    CUDA_TRY(d_heal_n_.resize(2));
+    CUDA_TRY(h_heal_n_.resize(2));
+    CUDA_TRY(d_heal_dig_.resize(32));
+    CUDA_TRY(h_heal_dig_.resize(32));
+    CUDA_TRY(d_heal_desc_.resize(1));
+    CUDA_TRY(h_heal_desc_.resize(1));
+    return B200POST_OK;
+}
+
+int Scanner::submit(int b, uint64_t first, uint32_t count, const SumRange *ranges, size_t n_ranges) {
     CUDA_TRY(cudaMemcpyAsync(d_labels_[b].get(), h_labels_[b].get(), (size_t)count * 16, cudaMemcpyHostToDevice, st_[b].get()));
+    if (sums_) {   // the covered ranges' digests, from the bytes K6a/K6b are about to read
+        first_label_[b] = first; ranges_[b] = ranges; n_ranges_[b] = n_ranges;
+        hashed_[b].clear();
+        for (size_t i = 0; i < n_ranges; i++)
+            if (ranges[i].sum) {
+                h_desc_[b].get()[hashed_[b].size()] = DigestDesc{(ranges[i].first - first) * 16, (uint32_t)(ranges[i].count * 16), 0};
+                hashed_[b].push_back(i);
+            }
+        const uint32_t nh = (uint32_t)hashed_[b].size();
+        if (nh) {
+            CUDA_TRY(cudaMemcpyAsync(d_desc_[b].get(), h_desc_[b].get(), nh * sizeof(DigestDesc), cudaMemcpyHostToDevice, st_[b].get()));
+            CUDA_TRY(launch_range_digests(st_[b].get(), d_labels_[b].get(), d_desc_[b].get(), nh, d_dig_[b].get()));
+            CUDA_TRY(cudaMemcpyAsync(h_dig_[b].get(), d_dig_[b].get(), (size_t)nh * 32, cudaMemcpyDeviceToHost, st_[b].get()));
+        }
+    }
     CUDA_TRY(cudaMemsetAsync(d_nhits_[b].get(), 0, 4, st_[b].get()));
     // the single candidate queue is reused by consecutive chunks: wait for the other stream's lazy pass
     if (pending_[b ^ 1]) CUDA_TRY(cudaStreamWaitEvent(st_[b].get(), ev_[b ^ 1].get(), 0));
     CUDA_TRY(cudaMemsetAsync(d_ncands_.get(), 0, 8, st_[b].get()));
     cudaStream_t st = st_[b].get();
     const uint4 *labels = reinterpret_cast<const uint4 *>(d_labels_[b].get());
-    if (stored_) launch(st, labels, first, count, reinterpret_cast<StoredHit *>(d_hits_[b].get()), d_nhits_[b].get());
-    else launch(st, labels, first, count, reinterpret_cast<Hit *>(d_hits_[b].get()), d_nhits_[b].get());
+    if (stored_) launch(st, labels, first, count, reinterpret_cast<StoredHit *>(d_hits_[b].get()), d_nhits_[b].get(), d_cands_.get(), cand_cap_, d_ncands_.get());
+    else launch(st, labels, first, count, reinterpret_cast<Hit *>(d_hits_[b].get()), d_nhits_[b].get(), d_cands_.get(), cand_cap_, d_ncands_.get());
     g_launches += 2;
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(h_ncands_[b].get(), d_ncands_.get(), 4, cudaMemcpyDeviceToHost, st_[b].get()));
@@ -245,6 +291,7 @@ int Scanner::collect(int b, HitBook *book, std::mutex *fold_mu) {
     pending_[b] = false;
     const uint32_t n = *h_nhits_[b].get();
     if (n > hit_cap_ || *h_ncands_[b].get() > cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
+    if (sums_) return fold_sums(b, n, book, fold_mu);
     if (stored_) fold<StoredHit>(b, n, book, fold_mu);
     else fold<Hit>(b, n, book, fold_mu);
     return B200POST_OK;
@@ -259,6 +306,95 @@ void Scanner::fold(int b, uint32_t n, HitBook *book, std::mutex *fold_mu) {
     if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
     for (const Rec &h : v) book->add(first_ + h.nonce, h.index, stored_bytes(h));
     book->advance(count_[b]);   // chunks are contiguous from the first index: the sum is how far the scan went
+}
+
+// One bad range of chunk b whose stored bytes hash to `stored`: its labels recomputed on this device's engine straight
+// into the chunk's device buffer, then hashed (to classify the damage) and scanned into the heal buffers.  *hits: the
+// range's StoredHit records.  Shards sharing a device serialise on its engine, as rechecks do.
+int Scanner::heal(int b, const SumRange &r, const uint8_t stored[32], std::vector<uint8_t> *hits, bool *sidecar_only) {
+    const uint64_t off = r.first - first_label_[b];
+    uint8_t *dst = d_labels_[b].get() + off * 16;
+    if (int rc = engine_->labels_range(commitment_, N_, r.first, r.count, nullptr, dst, nullptr, nullptr, cancel_)) return rc;
+    CUDA_TRY(cudaSetDevice(dev_));
+    cudaStream_t st = st_[b].get();
+    *h_heal_desc_.get() = DigestDesc{off * 16, (uint32_t)(r.count * 16), 0};
+    CUDA_TRY(cudaMemcpyAsync(d_heal_desc_.get(), h_heal_desc_.get(), sizeof(DigestDesc), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(launch_range_digests(st, d_labels_[b].get(), d_heal_desc_.get(), 1, d_heal_dig_.get()));
+    CUDA_TRY(cudaMemsetAsync(d_heal_n_.get(), 0, 8, st));
+    launch(st, reinterpret_cast<const uint4 *>(dst), r.first, (uint32_t)r.count, reinterpret_cast<StoredHit *>(d_heal_hits_.get()),
+           d_heal_n_.get(), d_heal_cands_.get(), heal_cand_cap_, d_heal_n_.get() + 1);
+    g_launches += 2;
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(h_heal_dig_.get(), d_heal_dig_.get(), 32, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(h_heal_n_.get(), d_heal_n_.get(), 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    const uint32_t n = h_heal_n_.get()[0];
+    if (n > hit_cap_ || h_heal_n_.get()[1] > heal_cand_cap_) { set_error("hit buffer overflow: K1 too large for this chunk size"); return B200POST_ERR_OUT_OF_MEMORY; }
+    CUDA_TRY(cudaMemcpyAsync(h_heal_hits_.get(), d_heal_hits_.get(), (size_t)n * rec_, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    hits->assign(h_heal_hits_.get(), h_heal_hits_.get() + (size_t)n * rec_);
+    // the stored bytes' digest equals the recomputation's: the data is right and the sidecar's digest is wrong
+    *sidecar_only = memcmp(h_heal_dig_.get(), stored, 32) == 0;
+    return B200POST_OK;
+}
+
+// collect of a checksummed chunk: the covered ranges' digests compared with their sidecar's, the bad ones counted
+// against the heal cap and healed, then the fold.  A hit's state comes from its range: covered (the digest matched, or
+// the range was recomputed) is good, uncovered is pending; a bad range's stored hits are replaced by its healed ones.
+int Scanner::fold_sums(int b, uint32_t n, HitBook *book, std::mutex *fold_mu) {
+    const SumRange *r = ranges_[b];
+    const size_t nr = n_ranges_[b];
+    std::vector<uint8_t> bad(nr, 0);
+    std::vector<size_t> bad_list;
+    uint64_t verified = 0, uncovered = 0;
+    for (size_t k = 0; k < hashed_[b].size(); k++) {
+        const size_t i = hashed_[b][k];
+        if (memcmp(h_dig_[b].get() + k * 32, r[i].sum, 32) == 0) verified += r[i].count;
+        else { bad[i] = 1; bad_list.push_back(k); }
+    }
+    for (size_t i = 0; i < nr; i++) if (!r[i].sum) uncovered += r[i].count;
+    sums_->blocks_checked += hashed_[b].size();
+    sums_->labels_verified += verified;
+    sums_->labels_uncovered += uncovered;
+    const StoredHit *rec = reinterpret_cast<const StoredHit *>(h_hits_[b].get());
+    std::vector<StoredHit> v;
+    v.reserve(n);
+    const auto range_of = [&](uint64_t index) {   // the range holding a label of the chunk
+        size_t lo = 0, hi = nr;
+        while (hi - lo > 1) { const size_t m = (lo + hi) / 2; (r[m].first <= index ? lo : hi) = m; }
+        return lo;
+    };
+    for (uint32_t j = 0; j < n; j++) if (!bad[range_of(rec[j].index)]) v.push_back(rec[j]);
+    if (!bad_list.empty()) {
+        {
+            std::lock_guard<std::mutex> g(sums_->mu);
+            for (size_t k : bad_list) {
+                const SumRange &x = r[hashed_[b][k]];
+                sums_->bad.emplace(x.first, SumsCheck::Bad{x.count, false});
+            }
+            if (sums_->bad.size() > sums_->max_heal) {
+                set_error("more than " + std::to_string(sums_->max_heal) + " damaged blocks: repair first (b200postcli -checkSums -repair)");
+                return B200POST_ERR_LABEL_MISMATCH;
+            }
+        }
+        for (size_t k : bad_list) {
+            const SumRange &x = r[hashed_[b][k]];
+            std::vector<uint8_t> healed;
+            bool sidecar_only = false;
+            if (int rc = heal(b, x, h_dig_[b].get() + k * 32, &healed, &sidecar_only)) return rc;
+            const StoredHit *h = reinterpret_cast<const StoredHit *>(healed.data());
+            v.insert(v.end(), h, h + healed.size() / sizeof(StoredHit));
+            std::lock_guard<std::mutex> g(sums_->mu);
+            sums_->bad[x.first].sidecar_only = sidecar_only;
+            sums_->healed.insert(x.first);
+        }
+    }
+    std::sort(v.begin(), v.end(), [](const StoredHit &x, const StoredHit &y) { return x.index != y.index ? x.index < y.index : x.nonce < y.nonce; });
+    std::unique_lock<std::mutex> lk;
+    if (fold_mu) lk = std::unique_lock<std::mutex>(*fold_mu);
+    for (const StoredHit &h : v) book->add(first_ + h.nonce, h.index, stored_bytes(h), r[range_of(h.index)].sum != nullptr);
+    book->advance(count_[b]);
+    return B200POST_OK;
 }
 
 void Scanner::drain() {
@@ -303,6 +439,8 @@ public:
     }
     Scanner &scanner(size_t s) { return shards_[s]->sc; }
     ProveRule &rule() { return rule_; }
+    // the shards stream the plan's chunks (their ranges must be the plan's shards) instead of chunks of `chunk` labels
+    void use_plan(const SumsPlan *plan) { plan_ = plan; }
 
     // runs every shard (the calling thread alone when there is one) and returns the first failing shard's status, in
     // list order, once every thread has joined
@@ -344,6 +482,7 @@ private:
         if (sh.lo == sh.hi) return rc;
         if (cudaSetDevice(sc.device()) != cudaSuccess) { cudaGetLastError(); set_error("cudaSetDevice failed"); return B200POST_ERR_CUDA; }
         int b = 0;
+        size_t k = plan_ ? plan_->shards[s].first : 0;   // the plan's next chunk
         for (uint64_t pos = sh.lo; pos < sh.hi; b ^= 1) {
             if (cancel && *cancel) { sc.drain(); set_error("cancelled"); return B200POST_ERR_CANCELLED; }
             if (abort_) { sc.drain(); return B200POST_OK; }   // another shard failed: its status is the call's
@@ -352,8 +491,13 @@ private:
             if (rc) { sc.drain(); return rc; }
             if (stop) break;
             // fill the staging buffer (a chunk may span files)
-            const uint64_t n = std::min<uint64_t>(chunk, sh.hi - pos);
-            if ((rc = fill(s, pos, n, sc.staging(b))) || (rc = sc.submit(b, base + pos, (uint32_t)n))) { sc.drain(); return rc; }
+            const SumChunk *c = plan_ ? &plan_->chunks[k++] : nullptr;
+            const uint64_t n = c ? c->count : std::min<uint64_t>(chunk, sh.hi - pos);
+            if ((rc = fill(s, pos, n, sc.staging(b))) ||
+                (rc = sc.submit(b, base + pos, (uint32_t)n, c ? &plan_->ranges[c->r0] : nullptr, c ? c->r1 - c->r0 : 0))) {
+                sc.drain();
+                return rc;
+            }
             pos += n;
         }
         for (int k = 0; k < 2; k++) if ((rc = sc.collect(b ^ k, &book, &mu_))) { sc.drain(); return rc; }   // older chunk first
@@ -361,6 +505,7 @@ private:
     }
 
     ProveRule rule_;
+    const SumsPlan *plan_ = nullptr;
     uint8_t commitment_[32] = {0};
     uint64_t N_ = 0;
     const volatile int *cancel_ = nullptr;
@@ -486,10 +631,13 @@ struct ItemProof {
     b200post_proof_out *out = nullptr;
     b200post_proof_metadata *meta_out = nullptr;
     b200post_prove_check *check = nullptr;
+    SumsCheck *sums = nullptr;         // set for a checksummed proof (with check)
     b200post_post_metadata md{};
     uint64_t num_labels = 0, per_file = 0, chunk = 0;
     uint32_t n = 0, windows = 0, per_pass = 0;
     std::vector<std::pair<uint64_t, uint64_t>> ranges;
+    std::vector<PostSums> sidecars;    // checksummed: per file, its usable sidecar (covering nothing without one)
+    SumsPlan plan;                     // checksummed: the chunks and shards over the sidecars' digest ranges
     uint8_t commitment[32] = {0};
     uint32_t a = 0;                    // the next pass starts at window a
     uint64_t scanned = 0;              // over every pass
@@ -529,6 +677,19 @@ int open_item(ItemProof &it, const b200post_prove_opts &o, int n_providers) {
     it.chunk = std::min<uint64_t>(o.chunk_labels, it.num_labels);
     it.ranges = split_shards(it.num_labels, it.chunk, (size_t)n_providers);
     if (it.check) commitment_bytes(md.node_id, md.commitment_atx_id, it.commitment);
+    if (it.sums) {   // a missing or unusable sidecar only leaves its file uncovered
+        const Layout lay(md);
+        std::vector<SumsFile> files;
+        it.sidecars.resize(lay.n_files);
+        for (uint64_t f = 0; f < lay.n_files; f++) {
+            PostSums &ps = it.sidecars[f];
+            if (!load_post_sums(it.data_dir, md, f, lay.labels_in(f), &ps)) ps = PostSums::of(md, f);
+            files.push_back({lay.labels_in(f), ps.covered, reinterpret_cast<const uint8_t *>(ps.digests.data())});
+        }
+        it.plan = plan_sums(files, o.chunk_labels, (size_t)n_providers);
+        it.chunk = it.plan.max_chunk;
+        for (size_t s = 0; s < it.ranges.size(); s++) it.ranges[s] = it.plan.shard_labels(s);
+    }
     return B200POST_OK;
 }
 
@@ -538,11 +699,14 @@ int scan_pass(ItemProof &it, const b200post_post_config &cfg, const uint32_t *pr
     const uint32_t m = it.pass_windows(), first = it.a * it.n;
     // one shard per list entry: its own Scanner (device buffers, double-buffered staging), reader and host thread
     ShardedScan scan(it.ranges, first, it.n, m, cfg.k2, it.check ? it.commitment : nullptr, it.md.scrypt_n, cancel);
+    if (it.sums) scan.use_plan(&it.plan);
     int rc;
-    for (int s = 0; s < n_providers; s++)
-        if ((rc = scan.scanner((size_t)s).init(providers[s], it.challenge, m * it.n, it.pows.data(), cfg.k1, cfg.k2, it.num_labels, it.chunk,
-                                               it.check != nullptr, first)))
+    for (int s = 0; s < n_providers; s++) {
+        Scanner &sc = scan.scanner((size_t)s);
+        if ((rc = sc.init(providers[s], it.challenge, m * it.n, it.pows.data(), cfg.k1, cfg.k2, it.num_labels, it.chunk, it.check != nullptr, first)))
             return rc;
+        if (it.sums && (rc = sc.use_sums(it.sums, it.commitment, it.md.scrypt_n, it.plan.max_ranges, cancel))) return rc;
+    }
     std::vector<std::unique_ptr<PostDataReader>> readers;
     for (int s = 0; s < n_providers; s++) readers.emplace_back(new PostDataReader(it.data_dir, it.per_file));
     rc = scan.run([&](size_t s, uint64_t pos, uint64_t cnt, uint8_t *dst) { return readers[s]->read(pos, cnt, dst); }, it.chunk, 0, cancel);
@@ -725,7 +889,7 @@ int prove_items(std::vector<ItemProof> &items, const b200post_post_config &cfg, 
 
 int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
              const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
-             b200post_prove_check *check, const volatile int *cancel);
+             b200post_prove_check *check, const volatile int *cancel, SumsCheck *sums = nullptr);
 b200post_prove_opts prove_opts(const b200post_prove_opts *opts);
 
 }  // namespace
@@ -773,6 +937,29 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
     return generate(data_dir, challenge, cfg, opts, providers, n_providers, out, meta_out, check, cancel);
 }
 
+int b200post_generate_proof_sums(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                 const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                 const b200post_prove_sums_opts *sopts, b200post_proof_out *out, b200post_proof_metadata *meta_out,
+                                 b200post_prove_check *check, b200post_prove_sums_report *sums, const volatile int *cancel) {
+    if (!data_dir || !challenge || !cfg || !out || !providers || n_providers <= 0 || !check || !sums) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
+    memset(check, 0, sizeof *check);
+    memset(sums, 0, sizeof *sums);
+    SumsCheck sc(sopts && sopts->max_heal_blocks ? sopts->max_heal_blocks : 1024);
+    const int rc = generate(data_dir, challenge, cfg, opts, providers, n_providers, out, meta_out, check, cancel, &sc);
+    const std::string err = rc ? last_error() : std::string();
+    sums->blocks_checked = sc.blocks_checked; sums->labels_verified = sc.labels_verified; sums->labels_uncovered = sc.labels_uncovered;
+    sums->bad_blocks = sc.bad.size(); sums->healed_blocks = sc.healed.size();
+    for (const auto &kv : sc.bad) {   // ascending
+        sums->sidecar_only += kv.second.sidecar_only;
+        if (sums->n_reported < 64) sums->bad[sums->n_reported++] = b200post_sums_block{kv.first, kv.second.count};
+    }
+    metrics().prove_sum_blocks_checked_total += sums->blocks_checked;
+    metrics().prove_sum_blocks_bad_total += sums->bad_blocks;
+    metrics().prove_sum_blocks_healed_total += sums->healed_blocks;
+    if (rc) set_error(err);
+    return rc;
+}
+
 int b200post_generate_proofs(b200post_prove_item *items, size_t n, const b200post_post_config *cfg, const b200post_prove_opts *opts,
                              const uint32_t *providers, int n_providers, uint32_t checked, uint32_t parallel_scans,
                              const volatile int *cancel) {
@@ -808,15 +995,15 @@ b200post_prove_opts prove_opts(const b200post_prove_opts *opts) {
     return o;
 }
 
-// b200post_generate_proof_multi (check == nullptr) and b200post_generate_proof_checked: the one-item case of
-// prove_items.  They differ only in the scan's hit records, whether hits are born pending (the ShardedScan's
-// commitment), the report and the final verifier gate.
+// b200post_generate_proof_multi (check == nullptr), b200post_generate_proof_checked and b200post_generate_proof_sums
+// (check and sums): the one-item case of prove_items.  They differ only in the scan's hit records, whether hits are born
+// pending (the ShardedScan's commitment), the chunk plan and sidecar check (sums), the report and the verifier gate.
 int generate(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg, const b200post_prove_opts *opts,
              const uint32_t *providers, int n_providers, b200post_proof_out *out, b200post_proof_metadata *meta_out,
-             b200post_prove_check *check, const volatile int *cancel) {
+             b200post_prove_check *check, const volatile int *cancel, SumsCheck *sums) {
     std::vector<ItemProof> items(1);
     ItemProof &it = items[0];
-    it.data_dir = data_dir; it.challenge = challenge; it.out = out; it.meta_out = meta_out; it.check = check;
+    it.data_dir = data_dir; it.challenge = challenge; it.out = out; it.meta_out = meta_out; it.check = check; it.sums = sums;
     prove_items(items, *cfg, prove_opts(opts), providers, n_providers, 1, cancel);
     if (it.status) set_error(it.error);
     return it.status;

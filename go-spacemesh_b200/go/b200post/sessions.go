@@ -498,6 +498,74 @@ func GenerateProofCheckedWindows(ctx context.Context, providers []uint32, dataDi
 	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, rep, nil
 }
 
+// SumsBlock is a run of labels [FirstLabel, FirstLabel+Count) that one block checksum covers.
+type SumsBlock struct {
+	FirstLabel, Count uint64
+}
+
+// SumsReport is what GenerateProofSums found in the block checksums (postdata_N.sum): digest ranges read, hashed and
+// compared, labels in ranges that matched and labels read without a usable checksum (all three summed over passes),
+// the distinct bad ranges, those recomputed and scanned from the recomputation, the bad ranges whose stored bytes were
+// right (only the checksum was wrong), and the lowest 64 bad ranges, ascending.
+type SumsReport struct {
+	BlocksChecked, LabelsVerified, LabelsUncovered uint64
+	BadBlocks, HealedBlocks, SidecarOnly           uint64
+	Bad                                            []SumsBlock
+}
+
+// ProveSumsOpts are GenerateProofSums's options: MaxHealBlocks bounds the bad blocks the call may recompute
+// (0 = 1024, 1 GiB of labels); past it the call fails with "more than M damaged blocks: repair first".
+type ProveSumsOpts struct {
+	MaxHealBlocks uint32
+}
+
+// GenerateProofSums is GenerateProofCheckedWindows with the POST's block checksums in the loop
+// (b200post_generate_proof_sums): every covered block the scan reads is hashed on the device and compared with its
+// checksum, so the epoch's proof read is also a full check of the data it reads.  A matching block's hits are usable at
+// once; a damaged block is recomputed and scanned from the recomputation, so over covered data the proof is the
+// undamaged POST's whatever the damage; labels without a usable checksum follow GenerateProofChecked's rule.  The call
+// never writes into dataDir: a report with Bad ranges means the data needs `b200postcli -checkSums -repair`.  The report
+// is returned with the error when the call fails after the scan began (e.g. past MaxHealBlocks).
+func GenerateProofSums(ctx context.Context, providers []uint32, dataDir string, challenge []byte, cfg SetupConfig, nonces uint32,
+	w NonceWindows, opts ProveSumsOpts) (*Proof, *ProveCheck, *SumsReport, error) {
+	if len(providers) == 0 {
+		return nil, nil, nil, ErrNoProvider
+	}
+	dir := C.CString(dataDir)
+	defer C.free(unsafe.Pointer(dir))
+	var c C.b200post_post_config
+	c.labels_per_unit, c.k1, c.k2 = C.uint64_t(cfg.LabelsPerUnit), C.uint32_t(cfg.K1), C.uint32_t(cfg.K2)
+	C.memcpy(unsafe.Pointer(&c.pow_difficulty[0]), unsafe.Pointer(&cfg.PowDifficulty[0]), 32)
+	o := C.b200post_prove_opts{nonces: C.uint32_t(nonces), max_windows: C.uint32_t(w.Max), windows_per_pass: C.uint32_t(w.PerPass)}
+	so := C.b200post_prove_sums_opts{max_heal_blocks: C.uint32_t(opts.MaxHealBlocks)}
+	provs := (*C.uint32_t)(C.CBytes(unsafe.Slice((*byte)(unsafe.Pointer(&providers[0])), 4*len(providers))))
+	defer C.free(unsafe.Pointer(provs))
+	flag, stop := cancelFlag(ctx)
+	defer stop()
+	var out C.b200post_proof_out
+	var chk C.b200post_prove_check
+	var sr C.b200post_prove_sums_report
+	err := statusErr(checked(func() C.int {
+		return C.b200post_generate_proof_sums(dir, (*C.uint8_t)(unsafe.Pointer(&challenge[0])), &c, &o, provs, C.int(len(providers)), &so,
+			&out, nil, &chk, &sr, flag)
+	}))
+	sums := &SumsReport{BlocksChecked: uint64(sr.blocks_checked), LabelsVerified: uint64(sr.labels_verified),
+		LabelsUncovered: uint64(sr.labels_uncovered), BadBlocks: uint64(sr.bad_blocks), HealedBlocks: uint64(sr.healed_blocks),
+		SidecarOnly: uint64(sr.sidecar_only)}
+	for i := 0; i < int(sr.n_reported); i++ {
+		sums.Bad = append(sums.Bad, SumsBlock{FirstLabel: uint64(sr.bad[i].first_label), Count: uint64(sr.bad[i].count)})
+	}
+	if err != nil {
+		return nil, nil, sums, err
+	}
+	rep := &ProveCheck{LabelsRechecked: uint64(chk.labels_rechecked), Damaged: uint64(chk.damaged), ProofVerified: chk.proof_verified != 0,
+		Rounds: uint32(chk.rounds)}
+	for i := 0; i < int(chk.n_reported); i++ {
+		rep.DamagedIndex = append(rep.DamagedIndex, uint64(chk.damaged_index[i]))
+	}
+	return &Proof{Nonce: uint32(out.nonce), Pow: uint64(out.pow), Indices: C.GoBytes(unsafe.Pointer(&out.indices[0]), C.int(out.indices_len))}, rep, sums, nil
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // The initial proof (BuildInitialPost's PostClient.Proof(ctx, nodeID, shared.ZeroChallenge, nil), activation/activation.go:350-403)
 // ---------------------------------------------------------------------------------------------------------

@@ -12,7 +12,7 @@ from dataclasses import dataclass, field
 import numpy as np
 
 from . import B200PostError, ERR_NO_DEVICE, OK, lib, providers as _providers
-from .setup import PostConfig, _PostConfig, _bind as _bind_setup
+from .setup import PostConfig, _PostConfig, _SumsBlock, _bind as _bind_setup
 from .verify import Proof, ProofMetadata, _Meta
 
 POW_PROVE_FN = ctypes.CFUNCTYPE(ctypes.c_int, ctypes.c_void_p, ctypes.c_uint8, ctypes.POINTER(ctypes.c_uint8),
@@ -51,6 +51,31 @@ class ProveCheck:
     rounds: int = 0
 
 
+class _ProveSumsOpts(ctypes.Structure):
+    _fields_ = [("max_heal_blocks", ctypes.c_uint32)]
+
+
+class _SumsReport(ctypes.Structure):
+    _fields_ = [("blocks_checked", ctypes.c_uint64), ("labels_verified", ctypes.c_uint64), ("labels_uncovered", ctypes.c_uint64),
+                ("bad_blocks", ctypes.c_uint64), ("healed_blocks", ctypes.c_uint64), ("sidecar_only", ctypes.c_uint64),
+                ("n_reported", ctypes.c_uint32), ("reserved", ctypes.c_uint32), ("bad", _SumsBlock * 64)]
+
+
+@dataclass
+class SumsReport:
+    """What generate_proof_sums found in the block checksums: digest ranges hashed and compared, labels in ranges that
+    matched, labels read without a usable sidecar (all three summed over passes), the distinct bad ranges, those healed
+    (recomputed and scanned from the recomputation), the bad ranges whose stored bytes were right (only the sidecar's
+    digest was wrong), and the lowest 64 bad ranges as (first label, labels), ascending."""
+    blocks_checked: int
+    labels_verified: int
+    labels_uncovered: int
+    bad_blocks: int
+    healed_blocks: int
+    sidecar_only: int
+    bad: list = field(default_factory=list)
+
+
 class _ProveItem(ctypes.Structure):
     _fields_ = [("data_dir", ctypes.c_char_p), ("challenge", ctypes.c_uint8 * 32), ("status", ctypes.c_int32),
                 ("error", ctypes.c_char * 256), ("proof", _ProofOut), ("meta", _Meta), ("check", _ProveCheck)]
@@ -83,6 +108,10 @@ def _bind():
     L.b200post_generate_proof_checked.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
                                                   ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_ProofOut),
                                                   ctypes.POINTER(_Meta), ctypes.POINTER(_ProveCheck), ctypes.c_void_p]
+    L.b200post_generate_proof_sums.argtypes = [ctypes.c_char_p, ctypes.c_char_p, ctypes.POINTER(_PostConfig), ctypes.POINTER(_ProveOpts),
+                                               ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.POINTER(_ProveSumsOpts),
+                                               ctypes.POINTER(_ProofOut), ctypes.POINTER(_Meta), ctypes.POINTER(_ProveCheck),
+                                               ctypes.POINTER(_SumsReport), ctypes.c_void_p]
     L.b200post_generate_proofs.argtypes = [ctypes.POINTER(_ProveItem), ctypes.c_size_t, ctypes.POINTER(_PostConfig),
                                            ctypes.POINTER(_ProveOpts), ctypes.POINTER(ctypes.c_uint32), ctypes.c_int, ctypes.c_uint32,
                                            ctypes.c_uint32, ctypes.c_void_p]
@@ -187,6 +216,37 @@ def generate_proof_checked(data_dir: str, challenge: bytes, cfg: PostConfig, *, 
     report = ProveCheck(int(chk.labels_rechecked), int(chk.damaged), [int(v) for v in chk.damaged_index[: chk.n_reported]],
                         bool(chk.proof_verified), int(chk.rounds))
     return (*_results(out, meta), report)
+
+
+def generate_proof_sums(data_dir: str, challenge: bytes, cfg: PostConfig, *, providers=(0,), nonces: int = 16,
+                        chunk_labels: int = 0, pow="builtin", cancel=None, max_windows=1, windows_per_pass: int = 1,
+                        max_heal_blocks: int = 0):
+    """generate_proof_checked with the POST's block checksums (postdata_<N>.sum) in the loop
+    (b200post_generate_proof_sums): every covered block the scan reads is hashed on the GPU and compared with its
+    checksum; a matching block's hits are usable at once, a damaged block is recomputed and scanned from the
+    recomputation, and labels without a usable checksum follow generate_proof_checked's rule.  Where every label read is
+    covered the proof is the undamaged POST's.  Nothing in data_dir is written: repair with check_sums(repair=True).
+    max_heal_blocks: bad blocks the call may recompute (0 = 1024); past it the call raises ERR_LABEL_MISMATCH.
+    Returns (Proof, ProofMetadata, ProveCheck, SumsReport).  A raised B200PostError carries the report as `.sums`."""
+    L = _bind()
+    opts, providers = _opts(None, list(providers) if not isinstance(providers, str) else providers, nonces, chunk_labels, pow,
+                            max_windows, windows_per_pass)
+    out, meta, chk, rep, c = _ProofOut(), _Meta(), _ProveCheck(), _SumsReport(), _c_cfg(cfg)
+    sopts = _ProveSumsOpts(max_heal_blocks)
+    cptr = ctypes.addressof(cancel) if cancel is not None else None
+    arr = (ctypes.c_uint32 * max(len(providers), 1))(*providers)
+    rc = L.b200post_generate_proof_sums(data_dir.encode(), challenge, ctypes.byref(c), ctypes.byref(opts), arr if len(providers) else None,
+                                        len(providers), ctypes.byref(sopts), ctypes.byref(out), ctypes.byref(meta), ctypes.byref(chk),
+                                        ctypes.byref(rep), cptr)
+    report = SumsReport(int(rep.blocks_checked), int(rep.labels_verified), int(rep.labels_uncovered), int(rep.bad_blocks),
+                        int(rep.healed_blocks), int(rep.sidecar_only),
+                        [(int(b.first_label), int(b.count)) for b in rep.bad[: rep.n_reported]])
+    if rc != OK:
+        e = B200PostError(rc, L.b200post_last_error().decode(errors="replace"))
+        e.sums = report
+        raise e
+    proof, pm, _ = _results(out, meta)
+    return proof, pm, _report(chk), report
 
 
 def generate_proof(data_dir: str, challenge: bytes, cfg: PostConfig, *, provider: int | None = None, nonces: int = 16,

@@ -9,8 +9,9 @@
  * mainnet Nonces = 288, config/mainnet.go:60-65).  Result = types.Post{Nonce, Indices, Pow}
  * (post_client.go:124-128), exactly what b200post_verifier_verify consumes.
  *
- * The k2pow itself is RandomX (cmd/root.go:254-259) and is NOT implemented: `pow_prove` supplies the pow of a
- * nonce group (e.g. libpost's prover); NULL uses pow = 0, which only a verifier without a pow check accepts.
+ * The k2pow is RandomX (cmd/root.go:254-259): pow_mode BUILTIN (the default) searches it on the device
+ * (b200post_k2pow.h); CALLBACK takes it from `pow_prove` (e.g. libpost's prover); SKIP uses pow = 0, which only a
+ * verifier without a pow check accepts.
  * All conventions are the post-rs Prover8_56 ones from memory: ASSUMED, "parity unpinned" (DESIGN.md §2).
  * Selection rule (deterministic): among nonces that reach K2 hits, the one whose K2-th hit has the lowest
  * label index wins; ties go to the lower nonce; its first K2 hit indices, ascending, are the proof.
@@ -137,6 +138,52 @@ int b200post_generate_proof_checked(const char *data_dir, const uint8_t challeng
                                     const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
                                     b200post_proof_out *out, b200post_proof_metadata *meta_out, b200post_prove_check *check,
                                     const volatile int *cancel);
+
+/* Options of b200post_generate_proof_sums (NULL = the defaults). */
+typedef struct b200post_prove_sums_opts {
+    uint32_t max_heal_blocks;          /* bad blocks the call may recompute; 0 = 1024 (1 GiB of labels)             */
+} b200post_prove_sums_opts;
+
+/* What b200post_generate_proof_sums found in the POST's block checksums (postdata_N.sum, b200post_setup.h). */
+typedef struct b200post_prove_sums_report {
+    uint64_t blocks_checked;           /* digest ranges read, hashed and compared (summed over passes)             */
+    uint64_t labels_verified;          /* labels in ranges whose digest matched (summed over passes)               */
+    uint64_t labels_uncovered;         /* labels read with no usable sidecar: the checked rule (summed over passes) */
+    uint64_t bad_blocks;               /* distinct ranges whose stored digest differed                             */
+    uint64_t healed_blocks;            /* distinct bad ranges recomputed and scanned from the recomputation        */
+    uint64_t sidecar_only;             /* of the bad ranges: the stored bytes were right, the digest wrong          */
+    uint32_t n_reported, reserved;
+    b200post_sums_block bad[64];       /* the lowest n_reported bad ranges, ascending                               */
+} b200post_prove_sums_report;
+
+/* b200post_generate_proof_checked with the POST's block checksums in the loop: each epoch's proof read becomes a check
+ * of every covered label it reads, at no extra read (DESIGN.md §5, "Proving over checksummed data").
+ *   Coverage: a label is covered when a usable sidecar of its file (what b200post_check_sums accepts) describes it.  A
+ *   digest range is one sidecar digest's labels: 2^16 aligned to the file's first label, or the short last range up to
+ *   `covered`.  The scan reads whole ranges per chunk (chunk_labels is an upper bound, raised to 2^16), hashes each
+ *   covered range on the device and compares it with its digest.
+ *     digest matches: every hit in the range is usable at once (sidecars are only made from device-computed labels).
+ *     digest differs (a bad block): the range is recomputed on the scan's device under the metadata's N, hashed again
+ *       and scanned from the recomputation; the stored bytes' hits there are discarded.  The recomputed digest equals
+ *       the stored one: only the sidecar is wrong (sidecar_only); it equals the sidecar's: the data is damaged.
+ *     uncovered (past `covered`, or a file without a usable sidecar): the checked call's rule, hits rechecked.
+ *   The proof is the selection rule over those usable hits, with the checked call's stop rule, windows, shards and
+ *   verifier gate.  So when every label read is covered, (nonce, indices, pow) are byte-identical to
+ *   b200post_generate_proof_multi's over the undamaged POST whatever the damage, device list, chunk size or windows;
+ *   without any usable sidecar they and the status are b200post_generate_proof_checked's.  On clean covered data
+ *   check->labels_rechecked is 0.
+ *   Read-only: the call writes nothing into data_dir; repair stays b200post_check_sums with repair = 1.
+ *   Heal cap: more than sopts->max_heal_blocks distinct bad ranges met returns B200POST_ERR_LABEL_MISMATCH ("more than
+ *   M damaged blocks: repair first") with `sums` filled and no proof.  As with a read error, a shard can meet bad blocks
+ *   past the point where one device would already have stopped, so a device list can reach the cap where one device
+ *   does not.
+ * Errors and their order are the checked call's (arguments, `sums` NULL included; metadata and an invalid scrypt N:
+ * B200POST_ERR_IO; pow mode; NO_DEVICE / UNSUPPORTED for the CPU id; CANCELLED).  A missing or unusable sidecar is
+ * never an error.  check and sums are cleared past the argument checks; sums is filled whatever the outcome. */
+int b200post_generate_proof_sums(const char *data_dir, const uint8_t challenge[32], const b200post_post_config *cfg,
+                                 const b200post_prove_opts *opts, const uint32_t *providers, int n_providers,
+                                 const b200post_prove_sums_opts *sopts, b200post_proof_out *out, b200post_proof_metadata *meta_out,
+                                 b200post_prove_check *check, b200post_prove_sums_report *sums, const volatile int *cancel);
 
 /* One identity's proof in b200post_generate_proofs. */
 typedef struct b200post_prove_item {
