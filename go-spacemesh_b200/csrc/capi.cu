@@ -68,7 +68,7 @@ int b200post_set_option(const char *key, int64_t value) {
     if (!key) return B200POST_ERR_INVALID_ARGUMENT;
     Options &o = options();
     const std::string k(key);
-    if (k == "romix_variant" && value >= 0 && value <= 4) { o.romix_variant = value; return B200POST_OK; }
+    if (k == "romix_variant" && value >= 0 && value <= 5) { o.romix_variant = value; return B200POST_OK; }
     if (k == "rotate_mask" && value >= 0 && value <= 1 && romix_mask_supported((int)value)) { o.rotate_mask = value; return B200POST_OK; }
     if (k == "tpb" && (value == 64 || value == 128 || value == 256 || value == 512)) { o.tpb = value; return B200POST_OK; }
     if (k == "dr_unroll" && (value == 1 || value == 4)) { o.dr_unroll = value; return B200POST_OK; }

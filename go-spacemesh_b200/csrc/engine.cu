@@ -75,7 +75,8 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
     Options &o = options();
     const int variant = (int)o.romix_variant.load(), mw = (int)o.rotate_mask.load();
     int tpb = (int)o.tpb.load();
-    if (variant != ROMIX_PIPELINED && tpb != 128 && tpb != 256) tpb = 128;   // the classic kernels are built for 128/256 only
+    const bool two_pads = variant == ROMIX_PIPELINED || variant == ROMIX_PHASED;   // two scratchpads per slot
+    if (!two_pads && tpb != 128 && tpb != 256) tpb = 128;   // the classic kernels are built for 128/256 only
     const int dr = (int)o.dr_unroll.load();
     if (!stream_.get()) {
         CUDA_TRY(stream_.create(cudaStreamNonBlocking));
@@ -86,7 +87,7 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
         CUDA_TRY(d_running_.resize(1));
         CUDA_TRY(h_running_.resize(1));
     }
-    const size_t pads = variant == ROMIX_PIPELINED ? 2 : 1;   // scratchpads per slot
+    const size_t pads = two_pads ? 2 : 1;   // scratchpads per slot
     const size_t per_slot = 128 * (size_t)N * pads;
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
@@ -108,7 +109,7 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
     // 80 GB H100 holds ~36 k slots at N = 8192, while 132 SMs x 512 threads would take 67 k, and a 512-thread grid of
     // 36 k slots leaves half of the SMs idle.  Smaller CTAs (down to 64 threads) then spread the layer over every SM;
     // the size that puts the most slots on the device wins.
-    if (variant == ROMIX_PIPELINED) {
+    if (two_pads) {
         for (int t = tpb / 2; t >= 64; t /= 2) {
             const int c = ctas_for(t);
             if ((uint64_t)c * t > (uint64_t)ctas * tpb) { ctas = c; tpb = t; }
@@ -124,9 +125,12 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
     }
     if (wave != wave_slots_) spec_.valid = false;   // a pre-filled layer has the old layer's shape
     wave_slots_ = (uint32_t)wave;
+    // a phased layer gives each slot two labels of the layer (its two scratchpads)
+    const uint64_t layer = variant == ROMIX_PHASED ? 2 * wave : wave;
+    layer_labels_ = (uint32_t)layer;
 
-    const uint32_t need = (uint32_t)std::min<uint64_t>(wave, round_up((uint32_t)std::min<uint64_t>(want_slots, wave), 32));
-    const size_t need_v = per_slot * (size_t)need;
+    const uint32_t need = (uint32_t)std::min<uint64_t>(layer, round_up((uint32_t)std::min<uint64_t>(want_slots, layer), 32));
+    const size_t need_v = per_slot * (size_t)std::min<uint64_t>(need, wave);
     if (need_v > v_bytes_ || 128 * (size_t)N * 32 > v_align_) {
         CUDA_TRY(cudaStreamSynchronize(stream_.get()));
         spec_.valid = false;
@@ -182,7 +186,7 @@ int DeviceEngine::retire(const Job &job, int b) {
 
 int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj) {
     Layer &l = layer_[b];
-    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(wave_slots_, alloc_slots_);
+    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(layer_labels_, alloc_slots_);
     *lj = LabelJob{d_range_commit_.get(), 0, nullptr, job.start + off, n_valid, nullptr};
     if (job.gather) {
         // the staging buffers of this parity are free once the previous layer's inputs have left them
@@ -212,7 +216,7 @@ int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_
 
 int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj) {
     Layer &l = layer_[b];
-    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(wave_slots_, alloc_slots_);
+    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(layer_labels_, alloc_slots_);
     const uint32_t n_slots = round_up(n_valid, 32);
     if (job.expect_host) {
         // K3c: the expected slice goes H2D on the copy stream (pinned staging, double-buffered by parity; retire(b) has
@@ -255,7 +259,7 @@ int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n
 }
 
 int DeviceEngine::run_job(const Job &job) {
-    const uint64_t S = std::min<uint64_t>(wave_slots_, alloc_slots_);
+    const uint64_t S = std::min<uint64_t>(layer_labels_, alloc_slots_);
     const uint64_t M = (job.total + S - 1) / S;
     int rc_ = B200POST_OK, status = B200POST_OK;
     auto layer_count = [&](uint64_t m) { return (uint32_t)std::min<uint64_t>(S, job.total - m * S); };
@@ -263,10 +267,10 @@ int DeviceEngine::run_job(const Job &job) {
 
     // small jobs (a proof's K2 labels, one VRF-nonce label, ...): the low-latency kernel, one launch
     const int64_t lowlat_max = options().lowlat_max_labels.load();
-    const bool lowlat = variant_ == ROMIX_PIPELINED && M == 1 && lowlat_max > 0 && job.total <= (uint64_t)lowlat_max &&
+    const bool lowlat = (variant_ == ROMIX_PIPELINED || variant_ == ROMIX_PHASED) && M == 1 && lowlat_max > 0 && job.total <= (uint64_t)lowlat_max &&
                         job.total <= (uint64_t)prop_.multiProcessorCount * 4 * 32;
     if (lowlat || variant_ != ROMIX_PIPELINED) {
-        // one ROMix launch per layer: the low-latency kernel (a single layer) or a classic variant
+        // one ROMix launch per layer: the low-latency kernel (a single layer), the phased kernel or a classic variant
         spec_.valid = false;
         for (uint64_t m = 0; m < M; m++) {
             if (job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; break; }
@@ -285,6 +289,7 @@ int DeviceEngine::run_job(const Job &job) {
                 CUDA_TRY(launch_romix_lowlat(mw_, rp, romix_lowlat_warps(n_valid, prop_.multiProcessorCount), st));
             } else {
                 rp.n_slots = round_up(n_valid, 32); rp.flags = (uint32_t)options().debug_skip_phase.load();
+                rp.pair_offset = wave_slots_;
                 CUDA_TRY(launch_romix(variant_, mw_, tpb_, rp, st));
             }
             CUDA_TRY(cudaEventRecord(l.ev_k2b.get(), st));

@@ -18,7 +18,7 @@
 namespace b200post {
 
 struct Options {
-    std::atomic<int64_t> romix_variant{ROMIX_PIPELINED};
+    std::atomic<int64_t> romix_variant{ROMIX_PHASED};
     std::atomic<int64_t> rotate_mask{0};
     std::atomic<int64_t> tpb{512};             // CTA size; the pipelined kernel takes smaller CTAs when HBM cannot give every SM one of this size
     std::atomic<int64_t> dr_unroll{4};         // pipelined kernel: ChaCha double-rounds unrolled (4) or rolled (1)
@@ -148,8 +148,9 @@ private:
     DeviceBuffer<uint8_t> V_raw_;
     uint4 *V_ = nullptr;                   // aligned view into V_raw_
     size_t v_bytes_ = 0, v_align_ = 0;
-    uint32_t alloc_slots_ = 0;             // capacity of the per-slot buffers of layer_
-    uint32_t wave_slots_ = 0;              // slots per layer for the current (N, options)
+    uint32_t alloc_slots_ = 0;             // capacity of the per-slot buffers of layer_, in labels
+    uint32_t wave_slots_ = 0;              // resident slots (ROMix threads with their scratch) for the current (N, options)
+    uint32_t layer_labels_ = 0;            // labels per layer: wave_slots_, or twice that for ROMIX_PHASED
     Layer layer_[2];                       // per-layer state, double-buffered by layer parity
     DeviceBuffer<uint32_t> d_range_commit_;   // the commitment of the current call (32 bytes)
     DeviceBuffer<uint8_t> d_ctab_;            // indexed gather: call-level commitment table

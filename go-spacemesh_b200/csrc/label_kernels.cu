@@ -389,6 +389,135 @@ __global__ void __launch_bounds__(TPB) romix_pipe_kernel(const PipeParams p) {
 }
 
 // =================================================================================================
+// K2f: phased ROMix.  Every thread runs TWO labels of the same layer, A = slot t and B = slot t + S
+// (S = p.pair_offset, the engine's resident slot count), with the slot's two scratchpads: first N fill steps of both, then N
+// mix steps of both.  So a whole launch first only writes the scratchpads and then only reads them,
+// and HBM stops turning its bus around between reads and writes in every step (DESIGN.md §4).
+// In the mix loop each label's dependent row read is requested with cp.async while the other label's
+// BlockMix runs, the same window romix_pipe_kernel gives its mix read.  A warp of a partial layer whose
+// B slots lie past n_slots runs A alone (fill, then mix); a layer of at most S labels has no B at all, so
+// it keeps one label per thread and as many threads as the pipelined kernel would give it.  One launch is a whole layer: no state crosses
+// launches.
+// =================================================================================================
+template <int MW, int TPB>
+__global__ void __launch_bounds__(TPB) romix_phased_kernel(const RomixParams p) {
+    constexpr int DR = 4;
+    extern __shared__ __align__(128) uint8_t smem_raw[];
+    const uint32_t T = p.pair_offset;
+    const uint32_t slot = blockIdx.x * TPB + threadIdx.x;
+    if (slot >= T || slot >= p.n_slots) return;     // both are multiples of 32: whole warps leave together
+    const bool has_b = slot + T < p.n_slots;        // warp-uniform
+    const uint32_t lane = threadIdx.x & 31, warp_in_cta = threadIdx.x >> 5;
+    const uint32_t N = p.N, mask = N - 1;
+    const uint32_t tile_a = smem_u32(smem_raw) + warp_in_cta * 8192, tile_b = tile_a + 4096;
+    const uint32_t own_a = tile_a + lane * 128, own_b = tile_b + lane * 128;
+    const uint32_t swz = lane & 7, tr_row = lane >> 3, tr_c = lane & 7;
+    const uint32_t tile_a_tr = tile_a + tr_row * 128 + (tr_c << 4), tile_b_tr = tile_b + tr_row * 128 + (tr_c << 4);
+    const size_t warp = slot >> 5;
+    // this lane's base in the warp's two scratchpad regions as {lo, hi} (see romix_pipe_kernel): `hi` is constant
+    // within a region
+    const uint64_t va64 = (uint64_t)(p.V + (warp * 2) * (size_t)N * 256 + lane);
+    const uint64_t vb64 = (uint64_t)(p.V + (warp * 2 + 1) * (size_t)N * 256 + lane);
+    const uint32_t va_lo = (uint32_t)va64, va_hi = (uint32_t)(va64 >> 32);
+    const uint32_t vb_lo = (uint32_t)vb64, vb_hi = (uint32_t)(vb64 >> 32);
+    uint32_t src_lane[8];
+#pragma unroll
+    for (int k = 0; k < 8; k++) src_lane[k] = k * 4 + tr_row;
+
+    uint32_t lo_a[16], hi_a[16], lo_b[16], hi_b[16];
+#pragma unroll
+    for (int k = 0; k < 8; k++) set_chunk(lo_a, hi_a, k, p.X[(size_t)k * p.x_stride + slot]);
+    if (has_b) {
+#pragma unroll
+        for (int k = 0; k < 8; k++) set_chunk(lo_b, hi_b, k, p.X[(size_t)k * p.x_stride + slot + T]);
+    }
+
+    // own row -> tile (swizzled); after a __syncwarp, tile -> HBM row at {cur, hi} as 8 x 512 contiguous bytes
+#define ROW_TO_TILE(own, lo, hi) \
+    _Pragma("unroll") for (int k = 0; k < 8; k++) sts128(own + ((k ^ swz) << 4), ROW_CHUNK(lo, hi, k));
+#define TILE_TO_HBM_K(tile_tr, cur, vhi, k) st_stream_lohi<(k) * 512>(cur, vhi, lds128(tile_tr + (k) * 512));
+#define TILE_TO_HBM(tile_tr, cur, vhi)                                                                          \
+    TILE_TO_HBM_K(tile_tr, cur, vhi, 0) TILE_TO_HBM_K(tile_tr, cur, vhi, 1) TILE_TO_HBM_K(tile_tr, cur, vhi, 2) \
+    TILE_TO_HBM_K(tile_tr, cur, vhi, 3) TILE_TO_HBM_K(tile_tr, cur, vhi, 4) TILE_TO_HBM_K(tile_tr, cur, vhi, 5) \
+    TILE_TO_HBM_K(tile_tr, cur, vhi, 6) TILE_TO_HBM_K(tile_tr, cur, vhi, 7)
+    // request row V[Integerify(hi)] of every lane's label into the tile: 8 x (4 rows x 128 B) per warp
+#define ROW_REQUEST_K(tile_tr, j, vlo, vhi, k) \
+    cp_async16_lohi<(k) * 512>(tile_tr + (k) * 512, mad_u32(__shfl_sync(0xffffffffu, j, src_lane[k]), 4096u, vlo), vhi);
+#define ROW_REQUEST(tile_tr, hi, vlo, vhi)                                                                             \
+    {                                                                                                                  \
+        const uint32_t j = hi[0] & mask;                                                                               \
+        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 0) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 1) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 2) \
+        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 3) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 4) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 5) \
+        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 6) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 7)                                  \
+        cp_async_commit();                                                                                             \
+    }
+    // the lane's landed row out of the tile, then X <- BlockMix(X ^ row)
+#define MIX_FROM_TILE(own, lo, hi)                                                                       \
+    {                                                                                                    \
+        uint32_t vlo[16], vhi[16];                                                                       \
+        _Pragma("unroll") for (int k = 0; k < 8; k++) set_chunk(vlo, vhi, k, lds128(own + ((k ^ swz) << 4))); \
+        __syncwarp();                                                                                    \
+        blockmix_r1_xor<MW, DR>(lo, hi, vlo, vhi);                                                       \
+    }
+
+    uint32_t va_cur = va_lo, vb_cur = vb_lo;   // low word of row i's address; +4096 per step
+    if (has_b) {
+        for (uint32_t i = 0; i < N; i++) {
+            ROW_TO_TILE(own_a, lo_a, hi_a)
+            ROW_TO_TILE(own_b, lo_b, hi_b)
+            __syncwarp();
+            TILE_TO_HBM(tile_a_tr, va_cur, va_hi)
+            TILE_TO_HBM(tile_b_tr, vb_cur, vb_hi)
+            __syncwarp();
+            va_cur = mad_u32(1u, 4096u, va_cur); vb_cur = mad_u32(1u, 4096u, vb_cur);
+            blockmix_r1_x2<MW, DR>(lo_a, hi_a, lo_b, hi_b);
+        }
+        ROW_REQUEST(tile_b_tr, hi_b, vb_lo, vb_hi)
+        for (uint32_t i = 0; i < N; i++) {
+            ROW_REQUEST(tile_a_tr, hi_a, va_lo, va_hi)
+            asm volatile("cp.async.wait_group 1;" ::: "memory");   // B's row has landed; A's is in flight
+            __syncwarp();
+            MIX_FROM_TILE(own_b, lo_b, hi_b)
+            if (i + 1 < N) {
+                ROW_REQUEST(tile_b_tr, hi_b, vb_lo, vb_hi)
+                asm volatile("cp.async.wait_group 1;" ::: "memory");
+            } else {
+                cp_async_wait_all();
+            }
+            __syncwarp();
+            MIX_FROM_TILE(own_a, lo_a, hi_a)
+        }
+    } else {
+        for (uint32_t i = 0; i < N; i++) {
+            ROW_TO_TILE(own_a, lo_a, hi_a)
+            __syncwarp();
+            TILE_TO_HBM(tile_a_tr, va_cur, va_hi)
+            __syncwarp();
+            va_cur = mad_u32(1u, 4096u, va_cur);
+            blockmix_r1<MW, DR>(lo_a, hi_a);
+        }
+        for (uint32_t i = 0; i < N; i++) {
+            ROW_REQUEST(tile_a_tr, hi_a, va_lo, va_hi)
+            cp_async_wait_all();
+            __syncwarp();
+            MIX_FROM_TILE(own_a, lo_a, hi_a)
+        }
+    }
+#undef ROW_TO_TILE
+#undef TILE_TO_HBM_K
+#undef TILE_TO_HBM
+#undef ROW_REQUEST_K
+#undef ROW_REQUEST
+#undef MIX_FROM_TILE
+#pragma unroll
+    for (int k = 0; k < 8; k++) p.X[(size_t)k * p.x_stride + slot] = ROW_CHUNK(lo_a, hi_a, k);
+    if (has_b) {
+#pragma unroll
+        for (int k = 0; k < 8; k++) p.X[(size_t)k * p.x_stride + slot + T] = ROW_CHUNK(lo_b, hi_b, k);
+    }
+}
+
+// =================================================================================================
 // K3: PBKDF2 final + label output (TMA bulk store) + VRF candidate per CTA
 // =================================================================================================
 constexpr int FINAL_TPB = 128;
@@ -653,7 +782,7 @@ size_t romix_smem_bytes(int variant, int tpb) {
     const size_t warps = (size_t)tpb / 32;
     if (variant == ROMIX_COALESCED) return warps * 4096;
     if (variant == ROMIX_BULK) return warps * 8192 + warps * 8;
-    if (variant == ROMIX_PIPELINED) return warps * 8192;
+    if (variant == ROMIX_PIPELINED || variant == ROMIX_PHASED) return warps * 8192;
     return 0;
 }
 
@@ -664,6 +793,7 @@ const char *romix_variant_name(int variant) {
         case ROMIX_BULK: return "bulk";
         case ROMIX_NOMEM: return "nomem";
         case ROMIX_PIPELINED: return "pipelined";
+        case ROMIX_PHASED: return "phased";
     }
     return "?";
 }
@@ -728,6 +858,25 @@ static pipe_fn pick_pipe(int mw, int tpb, int dr_unroll) {
     return nullptr;
 }
 
+template <int MW>
+static romix_fn pick_phased_tpb(int tpb) {
+    switch (tpb) {
+        case 64: return romix_phased_kernel<MW, 64>;
+        case 128: return romix_phased_kernel<MW, 128>;
+        case 256: return romix_phased_kernel<MW, 256>;
+        case 512: return romix_phased_kernel<MW, 512>;
+    }
+    return nullptr;
+}
+static romix_fn pick_phased(int mw, int tpb) {
+    switch (mw) {
+#define X(m) case m: return pick_phased_tpb<m>(tpb);
+        B200POST_MW_LIST(X)
+#undef X
+    }
+    return nullptr;
+}
+
 bool romix_mask_supported(int mw) {
     switch (mw) {
 #define X(m) case m: return true;
@@ -747,7 +896,7 @@ int romix_max_ctas_per_sm(int variant, int rot_mask, int tpb, int dr_unroll) {
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, tpb, smem) != cudaSuccess) return 0;
         return n;
     }
-    romix_fn fn = pick(variant, rot_mask, tpb);
+    romix_fn fn = variant == ROMIX_PHASED ? pick_phased(rot_mask, tpb) : pick(variant, rot_mask, tpb);
     if (!fn) return 0;
     if (smem > 48 * 1024) cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, fn, tpb, smem) != cudaSuccess) return 0;
@@ -756,14 +905,17 @@ int romix_max_ctas_per_sm(int variant, int rot_mask, int tpb, int dr_unroll) {
 
 cudaError_t launch_romix(int variant, int rot_mask, int tpb, const RomixParams &p, cudaStream_t s) {
     if (p.n_slots == 0) return cudaSuccess;
-    romix_fn fn = pick(variant, rot_mask, tpb);
+    const bool phased = variant == ROMIX_PHASED;
+    romix_fn fn = phased ? pick_phased(rot_mask, tpb) : pick(variant, rot_mask, tpb);
     if (!fn) return cudaErrorInvalidValue;
     const size_t smem = romix_smem_bytes(variant, tpb);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
     }
-    fn<<<(p.n_slots + tpb - 1) / tpb, tpb, smem, s>>>(p);
+    if (phased && (p.pair_offset % 32 || 2 * (uint64_t)p.pair_offset < p.n_slots)) return cudaErrorInvalidValue;
+    const uint32_t threads = phased && p.pair_offset < p.n_slots ? p.pair_offset : p.n_slots;
+    fn<<<(threads + tpb - 1) / tpb, tpb, smem, s>>>(p);
     return cudaGetLastError();
 }
 

@@ -29,6 +29,7 @@ enum RomixVariant : int {
     ROMIX_BULK = 2,     // rows moved by the TMA unit: cp.async.bulk global<->shared + mbarrier
     ROMIX_NOMEM = 3,    // ALU ceiling probe: no scratchpad traffic (results are NOT labels)
     ROMIX_PIPELINED = 4,// two labels per thread: layer m fills while layer m-1 mixes (cp.async prefetch)
+    ROMIX_PHASED = 5,   // two labels of one layer per thread: both fill, then both mix (scratch writes, then reads)
 };
 
 struct RomixParams {
@@ -37,7 +38,9 @@ struct RomixParams {
     uint32_t x_stride;   // slots in the wave buffer (multiple of 32)
     uint32_t N;          // scrypt N (power of two, >= 2)
     uint32_t n_slots;    // active slots this wave (multiple of 32)
-    uint32_t flags;      // diagnostics: bit0 skip fill loop, bit1 skip mix loop (0 in production)
+    uint32_t flags;      // diagnostics: bit0 skip fill loop, bit1 skip mix loop (0 in production; not read by ROMIX_PHASED)
+    uint32_t pair_offset;// ROMIX_PHASED only (multiple of 32, >= n_slots / 2): the launch has min(n_slots, pair_offset)
+                         // threads, and thread t runs slot t and, if it exists, slot t + pair_offset
 };
 
 struct PipeParams {

@@ -133,6 +133,18 @@ PD_HD void blockmix_r1_dual(uint32_t (&lo_f)[16], uint32_t (&hi_f)[16], uint32_t
     chacha20_8_x2<ROT, DR_UNROLL>(hi_f, hi_m);
 }
 
+// BlockMix of two independent labels (a, b) in one instruction stream: the fill step of the phased ROMix kernel,
+// where every thread writes the scratchpads of two labels of the same layer together.
+template <int ROT, int DR_UNROLL>
+PD_HD void blockmix_r1_x2(uint32_t (&lo_a)[16], uint32_t (&hi_a)[16], uint32_t (&lo_b)[16], uint32_t (&hi_b)[16]) {
+#pragma unroll
+    for (int i = 0; i < 16; i++) { lo_a[i] ^= hi_a[i]; lo_b[i] ^= hi_b[i]; }
+    chacha20_8_x2<ROT, DR_UNROLL>(lo_a, lo_b);
+#pragma unroll
+    for (int i = 0; i < 16; i++) { hi_a[i] ^= lo_a[i]; hi_b[i] ^= lo_b[i]; }
+    chacha20_8_x2<ROT, DR_UNROLL>(hi_a, hi_b);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Keccak-f[1600] (the Keccak submission §1.2; lane (x, y) at s[x + 5y]) and the label's two PBKDF2 passes.
 // 13 permutations per label against 32768 ChaCha cores: ~0.5 % of the work, so the round loop stays rolled.
