@@ -11,6 +11,7 @@
 #include "engine.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -57,8 +58,8 @@ int DeviceEngine::Layer::allocate(uint32_t slots) {
     CUDA_TRY(d_exp.resize((size_t)slots * 16));
     CUDA_TRY(h_exp.resize((size_t)slots * 16));
     CUDA_TRY(d_bits.resize(slots / 32));
-    CUDA_TRY(d_cnt.resize(1));
-    CUDA_TRY(h_cnt.resize(1));
+    CUDA_TRY(d_cnt.resize(slots / 32));   // a compare job's count in word 0; rider compare chunks' at slot / 32
+    CUDA_TRY(h_cnt.resize(slots / 32));
     CUDA_TRY(ev_done.create(cudaEventDisableTiming));
     CUDA_TRY(ev_k3.create(cudaEventDisableTiming));
     CUDA_TRY(ev_in.create(cudaEventDisableTiming));
@@ -67,6 +68,7 @@ int DeviceEngine::Layer::allocate(uint32_t slots) {
     CUDA_TRY(ev_k2b.create(cudaEventDefault));
     in_pending = k2_pending = false;
     pend.live = false;
+    pend.riders.clear();
     return B200POST_OK;
 }
 
@@ -170,27 +172,67 @@ int DeviceEngine::retire(const Job &job, int b) {
     Layer &l = layer_[b];
     if (!l.pend.live) return B200POST_OK;
     CUDA_TRY(cudaEventSynchronize(l.ev_done.get()));
-    if (job.out_host) memcpy(job.out_host + l.pend.off * 16, l.h_out.get(), (size_t)l.pend.n * 16);
-    if (job.cmp && *l.h_cnt.get()) {
-        // rare path: the layer has mismatches; fetch its bitmap and decode positions (ascending: layers retire in order)
-        std::vector<uint32_t> bits(round_up(l.pend.n, 32) / 32);
-        CUDA_TRY(cudaMemcpy(bits.data(), l.d_bits.get(), bits.size() * 4, cudaMemcpyDeviceToHost));
-        job.cmp->mismatches += *l.h_cnt.get();
-        for (size_t w = 0; w < bits.size() && job.cmp->first.size() < CompareResult::kMaxReported; w++)
-            for (uint32_t v = bits[w]; v && job.cmp->first.size() < CompareResult::kMaxReported; v &= v - 1)
-                job.cmp->first.push_back(l.pend.off + 32 * w + (uint64_t)__builtin_ctz(v));
+    const LayerPlan &p = l.pend.plan;
+    if (job.out_host) memcpy(job.out_host + p.range_off * 16, l.h_out.get(), (size_t)p.n_range * 16);
+    // compare results: the layer's (or a rider chunk's) mismatch count, then, only when it is non-zero, its bitmap,
+    // decoded into positions of `cmp`'s job from item `first` on (ascending: layers retire in order)
+    auto take_mismatches = [&](CompareResult *cmp, uint32_t count, uint32_t word0, uint32_t n, uint64_t first) -> int {
+        if (!count) return B200POST_OK;
+        std::vector<uint32_t> bits(round_up(n, 32) / 32);
+        CUDA_TRY(cudaMemcpy(bits.data(), l.d_bits.get() + word0, bits.size() * 4, cudaMemcpyDeviceToHost));
+        cmp->mismatches += count;
+        for (size_t w = 0; w < bits.size() && cmp->first.size() < CompareResult::kMaxReported; w++)
+            for (uint32_t v = bits[w]; v && cmp->first.size() < CompareResult::kMaxReported; v &= v - 1)
+                cmp->first.push_back(first + 32 * w + (uint64_t)__builtin_ctz(v));
+        return B200POST_OK;
+    };
+    if (job.cmp)
+        if (int rc = take_mismatches(job.cmp, *l.h_cnt.get(), 0, p.n_range, p.range_off)) return rc;
+    for (size_t k = 0; k < p.chunks.size(); k++) {
+        const RiderChunk &c = p.chunks[k];
+        const Job &rj = *l.pend.riders[k]->job;
+        if (rj.out_host) memcpy(rj.out_host + c.item_off * 16, l.h_out.get() + (size_t)c.slot * 16, (size_t)c.n * 16);
+        if (rj.cmp)
+            if (int rc = take_mismatches(rj.cmp, l.h_cnt.get()[c.slot / 32], c.slot / 32, c.n, c.item_off)) return rc;
     }
     l.pend.live = false;
+    if (!p.chunks.empty()) {
+        // a rider whose every item has retired is done: it leaves the queue, and its caller returns
+        std::lock_guard<std::mutex> lk(rider_mu_);
+        for (size_t k = 0; k < p.chunks.size(); k++) {
+            Rider *r = l.pend.riders[k];
+            r->retired += p.chunks[k].n;
+            if (r->retired == r->load.items) {
+                r->done = true;
+                riders_.erase(std::find(riders_.begin(), riders_.end(), r));
+            }
+        }
+        rider_cv_.notify_all();
+    }
+    l.pend.riders.clear();
     return B200POST_OK;
 }
 
-int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj) {
+void DeviceEngine::next_layer(const Job &job, uint64_t range_off, uint64_t S, bool host, Layer &l) {
+    l.chunk_rider.clear();
+    if (!host) { l.plan = plan_layer((uint32_t)S, range_off, job.total, {}); return; }
+    std::lock_guard<std::mutex> lk(rider_mu_);
+    std::vector<RiderLoad *> queue;
+    for (Rider *r : riders_) queue.push_back(&r->load);
+    l.plan = plan_layer((uint32_t)S, range_off, job.total, queue);
+    for (const RiderChunk &c : l.plan.chunks) l.chunk_rider.push_back(riders_[c.rider]);
+}
+
+int DeviceEngine::stage_layer(const Job &job, int b, LabelJob *lj) {
     Layer &l = layer_[b];
-    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(layer_labels_, alloc_slots_);
+    const LayerPlan &p = l.plan;
+    const uint64_t off = p.range_off;
+    const uint32_t n_valid = p.n_range;
     *lj = LabelJob{d_range_commit_.get(), 0, nullptr, job.start + off, n_valid, nullptr};
+    const bool riders = !p.chunks.empty();
+    // the staging buffers of this parity are free once the previous layer's inputs have left them
+    if ((job.gather || riders) && l.in_pending) { CUDA_TRY(cudaEventSynchronize(l.ev_in.get())); l.in_pending = false; }
     if (job.gather) {
-        // the staging buffers of this parity are free once the previous layer's inputs have left them
-        if (l.in_pending) { CUDA_TRY(cudaEventSynchronize(l.ev_in.get())); l.in_pending = false; }
         memcpy(l.h_idx.get(), job.indices + off, (size_t)n_valid * 8);
         CUDA_TRY(cudaMemcpyAsync(l.d_idx.get(), l.h_idx.get(), (size_t)n_valid * 8, cudaMemcpyHostToDevice, stream_.get()));
         lj->indices = l.d_idx.get();
@@ -206,96 +248,175 @@ int DeviceEngine::stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_
             lj->commit = reinterpret_cast<const uint32_t *>(l.d_commit.get());
             lj->commit_stride = 8;
         }   // else one commitment for every item (compare jobs): only the indices travel
+    }
+    // rider segment [seg, n_slots): every slot gets its own commitment row and index at its layer position, whatever form
+    // the rider's call had; the slots that round a chunk up to whole warps get index 0 under a zero commitment
+    const uint32_t seg = p.range_slots, n_seg = p.n_slots - seg;
+    if (riders) {
+        bool any_cmp = false;
+        for (size_t k = 0; k < p.chunks.size(); k++) {
+            const RiderChunk &c = p.chunks[k];
+            const Job &rj = *l.chunk_rider[k]->job;
+            for (uint32_t i = 0; i < c.n; i++) {
+                l.h_idx.get()[c.slot + i] = rj.indices[c.item_off + i];
+                memcpy(l.h_commit.get() + (size_t)(c.slot + i) * 32, rj.row(c.item_off + i), 32);
+            }
+            const uint32_t pad = round_up(c.n, 32) - c.n;
+            memset(l.h_idx.get() + c.slot + c.n, 0, (size_t)pad * 8);
+            memset(l.h_commit.get() + (size_t)(c.slot + c.n) * 32, 0, (size_t)pad * 32);
+            if (rj.expect_host) {
+                memcpy(l.h_exp.get() + (size_t)c.slot * 16, rj.expect_host + c.item_off * 16, (size_t)c.n * 16);
+                any_cmp = true;
+            }
+        }
+        CUDA_TRY(cudaMemcpyAsync(l.d_idx.get() + seg, l.h_idx.get() + seg, (size_t)n_seg * 8, cudaMemcpyHostToDevice, stream_.get()));
+        CUDA_TRY(cudaMemcpyAsync(l.d_commit.get() + (size_t)seg * 32, l.h_commit.get() + (size_t)seg * 32, (size_t)n_seg * 32,
+                                 cudaMemcpyHostToDevice, stream_.get()));
+        if (any_cmp)
+            CUDA_TRY(cudaMemcpyAsync(l.d_exp.get() + (size_t)seg * 16, l.h_exp.get() + (size_t)seg * 16, (size_t)n_seg * 16,
+                                     cudaMemcpyHostToDevice, stream_.get()));
+    }
+    if (job.gather || riders) {
         CUDA_TRY(cudaEventRecord(l.ev_in.get(), stream_.get()));
         l.in_pending = true;
     }
-    CUDA_TRY(launch_pbkdf2_expand(*lj, l.X.get(), alloc_slots_, round_up(n_valid, 32), stream_.get()));
+    CUDA_TRY(launch_pbkdf2_expand(*lj, l.X.get(), alloc_slots_, seg, stream_.get()));
     g_launches += 1;
+    if (riders) {
+        // K1 of the rider segment: the same kernel on the X columns from `seg` on
+        const LabelJob rl{reinterpret_cast<const uint32_t *>(l.d_commit.get()) + 8 * (size_t)seg, 8, l.d_idx.get() + seg, 0, n_seg, nullptr};
+        CUDA_TRY(launch_pbkdf2_expand(rl, l.X.get() + seg, alloc_slots_, n_seg, stream_.get()));
+        g_launches += 1;
+    }
     return B200POST_OK;
 }
 
-int DeviceEngine::finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj) {
+int DeviceEngine::finish_layer(const Job &job, int b, const LabelJob &lj) {
     Layer &l = layer_[b];
-    const uint64_t off = layer * (uint64_t)std::min<uint64_t>(layer_labels_, alloc_slots_);
-    const uint32_t n_slots = round_up(n_valid, 32);
+    const LayerPlan &p = l.plan;
+    const uint64_t off = p.range_off;
+    const uint32_t n_valid = p.n_range, n_slots = p.range_slots;
+    cudaStream_t st = stream_.get();
+    // the range segment (or the gather's items): K3 as without riders, so the VRF scan and cta_cand see range slots only
     if (job.expect_host) {
         // K3c: the expected slice goes H2D on the copy stream (pinned staging, double-buffered by parity; retire(b) has
         // seen the previous copy out of h_exp finish), and K3c waits for it by event
         memcpy(l.h_exp.get(), job.expect_host + off * 16, (size_t)n_valid * 16);
         CUDA_TRY(cudaMemcpyAsync(l.d_exp.get(), l.h_exp.get(), (size_t)n_valid * 16, cudaMemcpyHostToDevice, copy_stream_.get()));
         CUDA_TRY(cudaEventRecord(l.ev_exp.get(), copy_stream_.get()));
-        CUDA_TRY(cudaStreamWaitEvent(stream_.get(), l.ev_exp.get(), 0));
-        CUDA_TRY(cudaMemsetAsync(l.d_cnt.get(), 0, 4, stream_.get()));
+        CUDA_TRY(cudaStreamWaitEvent(st, l.ev_exp.get(), 0));
+        CUDA_TRY(cudaMemsetAsync(l.d_cnt.get(), 0, 4, st));
         CUDA_TRY(launch_pbkdf2_final_compare(lj, l.X.get(), alloc_slots_, n_slots, l.d_exp.get(), l.d_bits.get(), l.d_cnt.get(),
-                                           job.d_diff, d_cta_cand_.get(), stream_.get()));
+                                           job.d_diff, d_cta_cand_.get(), st));
     } else if (job.out_hi_dev) {
         // K3w: both halves of every label32 stay in HBM (gathers of VRF-nonce checks)
-        CUDA_TRY(launch_pbkdf2_final_wide(lj, l.X.get(), alloc_slots_, n_slots, job.out_dev + off * 16, job.out_hi_dev + off * 16,
-                                          stream_.get()));
+        CUDA_TRY(launch_pbkdf2_final_wide(lj, l.X.get(), alloc_slots_, n_slots, job.out_dev + off * 16, job.out_hi_dev + off * 16, st));
     } else {
         uint8_t *d_out = job.out_dev ? job.out_dev + off * 16 : l.d_out.get();
-        CUDA_TRY(launch_pbkdf2_final(lj, l.X.get(), alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_.get(), stream_.get()));
+        CUDA_TRY(launch_pbkdf2_final(lj, l.X.get(), alloc_slots_, n_slots, d_out, job.d_diff, d_cta_cand_.get(), st));
     }
     g_launches += 1;
     if (job.d_diff) {
-        CUDA_TRY(launch_vrf_merge(d_cta_cand_.get(), pbkdf2_final_ctas(n_slots), d_running_.get(), stream_.get()));
+        CUDA_TRY(launch_vrf_merge(d_cta_cand_.get(), pbkdf2_final_ctas(n_slots), d_running_.get(), st));
         g_launches += 1;
     }
-    if (job.out_host || job.expect_host) {
+    // the rider chunks: each one's K3 / K3w / K3c on its X columns, into the rider's own destination (a host
+    // destination through d_out at the chunk's slots; a compare chunk's bitmap words and count at slot / 32)
+    uint32_t copy_slots = job.out_host ? n_valid : 0;   // d_out slots the D2H takes
+    bool rider_cmp = false;
+    for (size_t k = 0; k < p.chunks.size(); k++) {
+        const RiderChunk &c = p.chunks[k];
+        const Job &rj = *l.chunk_rider[k]->job;
+        const LabelJob cj{reinterpret_cast<const uint32_t *>(l.d_commit.get()) + 8 * (size_t)c.slot, 8, l.d_idx.get() + c.slot, 0, c.n, nullptr};
+        const uint4 *Xc = l.X.get() + c.slot;
+        if (rj.expect_host) {
+            CUDA_TRY(cudaMemsetAsync(l.d_cnt.get() + c.slot / 32, 0, 4, st));
+            CUDA_TRY(launch_pbkdf2_final_compare(cj, Xc, alloc_slots_, c.n, l.d_exp.get() + (size_t)c.slot * 16, l.d_bits.get() + c.slot / 32,
+                                               l.d_cnt.get() + c.slot / 32, nullptr, nullptr, st));
+            rider_cmp = true;
+        } else if (rj.out_hi_dev) {
+            CUDA_TRY(launch_pbkdf2_final_wide(cj, Xc, alloc_slots_, c.n, rj.out_dev + c.item_off * 16, rj.out_hi_dev + c.item_off * 16, st));
+        } else if (rj.out_dev) {
+            CUDA_TRY(launch_pbkdf2_final(cj, Xc, alloc_slots_, c.n, rj.out_dev + c.item_off * 16, nullptr, nullptr, st));
+        } else {
+            CUDA_TRY(launch_pbkdf2_final(cj, Xc, alloc_slots_, c.n, l.d_out.get() + (size_t)c.slot * 16, nullptr, nullptr, st));
+            if (rj.out_host) copy_slots = c.slot + c.n;
+        }
+        g_launches += 1;
+    }
+    if (copy_slots || job.expect_host || rider_cmp) {
         // the copy runs on its own stream: the next layers' kernels do not queue behind PCIe.  A compare job brings
-        // back only its 4-byte count; the bitmap follows in retire() when it is non-zero.
-        CUDA_TRY(cudaEventRecord(l.ev_k3.get(), stream_.get()));
+        // back only its 4-byte count (rider chunks: one per chunk, at slot / 32); the bitmap follows in retire() when it
+        // is non-zero.
+        CUDA_TRY(cudaEventRecord(l.ev_k3.get(), st));
         CUDA_TRY(cudaStreamWaitEvent(copy_stream_.get(), l.ev_k3.get(), 0));
-        if (job.expect_host)
-            CUDA_TRY(cudaMemcpyAsync(l.h_cnt.get(), l.d_cnt.get(), 4, cudaMemcpyDeviceToHost, copy_stream_.get()));
-        else
-            CUDA_TRY(cudaMemcpyAsync(l.h_out.get(), l.d_out.get(), (size_t)n_valid * 16, cudaMemcpyDeviceToHost, copy_stream_.get()));
+        if (job.expect_host || rider_cmp)
+            CUDA_TRY(cudaMemcpyAsync(l.h_cnt.get(), l.d_cnt.get(), job.expect_host ? 4 : (size_t)p.n_slots / 32 * 4, cudaMemcpyDeviceToHost,
+                                     copy_stream_.get()));
+        if (copy_slots)
+            CUDA_TRY(cudaMemcpyAsync(l.h_out.get(), l.d_out.get(), (size_t)copy_slots * 16, cudaMemcpyDeviceToHost, copy_stream_.get()));
         CUDA_TRY(cudaEventRecord(l.ev_done.get(), copy_stream_.get()));
     } else {
-        CUDA_TRY(cudaEventRecord(l.ev_done.get(), stream_.get()));
+        CUDA_TRY(cudaEventRecord(l.ev_done.get(), st));
     }
-    l.pend = Layer::Pending{off, n_valid, true};
+    l.pend.plan = p;
+    l.pend.riders = l.chunk_rider;
+    l.pend.live = true;
     return B200POST_OK;
+}
+
+// labels a layer's launches compute: the range segment's and the rider chunks'
+static double layer_labels(const LayerPlan &p) {
+    double n = p.n_range;
+    for (const RiderChunk &c : p.chunks) n += c.n;
+    return n;
 }
 
 int DeviceEngine::run_job(const Job &job) {
     const uint64_t S = std::min<uint64_t>(layer_labels_, alloc_slots_);
-    const uint64_t M = (job.total + S - 1) / S;
+    const uint64_t M = (job.total + S - 1) / S;   // layers without riders
     int rc_ = B200POST_OK, status = B200POST_OK;
-    auto layer_count = [&](uint64_t m) { return (uint32_t)std::min<uint64_t>(S, job.total - m * S); };
     cudaStream_t st = stream_.get();
 
     // small jobs (a proof's K2 labels, one VRF-nonce label, ...): the low-latency kernel, one launch
     const int64_t lowlat_max = options().lowlat_max_labels.load();
     const bool lowlat = (variant_ == ROMIX_PIPELINED || variant_ == ROMIX_PHASED) && M == 1 && lowlat_max > 0 && job.total <= (uint64_t)lowlat_max &&
                         job.total <= (uint64_t)prop_.multiProcessorCount * 4 * 32;
+    // a range job that launches layers hosts riders (compare jobs do not)
+    const bool host = !job.gather && !job.expect_host && !lowlat && rider_cap((uint32_t)S) > 0;
+    if (host) {
+        { std::lock_guard<std::mutex> lk(rider_mu_); hosting_ = true; host_N_ = job.N; }
+        rider_cv_.notify_all();   // gathers waiting for the engine may ride now
+    }
+    uint64_t range_off = 0;   // labels (of a gather: items) of the job in the layers staged so far
     if (lowlat || variant_ != ROMIX_PIPELINED) {
         // one ROMix launch per layer: the low-latency kernel (a single layer), the phased kernel or a classic variant
         spec_.valid = false;
-        for (uint64_t m = 0; m < M; m++) {
+        for (uint64_t m = 0; range_off < job.total; m++) {
             if (job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; break; }
             const int b = (int)(m & 1);
             Layer &l = layer_[b];
             if ((rc_ = retire(job, b))) return rc_;
             harvest(b);
-            const uint32_t n_valid = layer_count(m);
+            next_layer(job, range_off, S, host, l);
+            range_off += l.plan.n_range;
             LabelJob lj;
-            if ((rc_ = stage_layer(job, m, b, n_valid, &lj))) return rc_;
+            if ((rc_ = stage_layer(job, b, &lj))) return rc_;
             RomixParams rp;
             rp.V = V_; rp.X = l.X.get(); rp.x_stride = alloc_slots_; rp.N = (uint32_t)job.N;
             CUDA_TRY(cudaEventRecord(l.ev_k2a.get(), st));
             if (lowlat) {
-                rp.n_slots = n_valid; rp.flags = 0;
-                CUDA_TRY(launch_romix_lowlat(mw_, rp, romix_lowlat_warps(n_valid, prop_.multiProcessorCount), st));
+                rp.n_slots = l.plan.n_range; rp.flags = 0;
+                CUDA_TRY(launch_romix_lowlat(mw_, rp, romix_lowlat_warps(l.plan.n_range, prop_.multiProcessorCount), st));
             } else {
-                rp.n_slots = round_up(n_valid, 32); rp.flags = (uint32_t)options().debug_skip_phase.load();
+                rp.n_slots = l.plan.n_slots; rp.flags = (uint32_t)options().debug_skip_phase.load();
                 rp.pair_offset = wave_slots_;
                 CUDA_TRY(launch_romix(variant_, mw_, tpb_, rp, st));
             }
             CUDA_TRY(cudaEventRecord(l.ev_k2b.get(), st));
-            l.k2_pending = true; l.k2_labels = n_valid;
+            l.k2_pending = true; l.k2_labels = layer_labels(l.plan);
             g_launches += 1;
-            if ((rc_ = finish_layer(job, m, b, n_valid, lj))) return rc_;
+            if ((rc_ = finish_layer(job, b, lj))) return rc_;
         }
     } else {
         // consume a matching speculation: layer 0 of this call was filled by the previous call's last launch
@@ -306,33 +427,41 @@ int DeviceEngine::run_job(const Job &job) {
         const bool speculate = !job.gather && options().speculate_next.load() != 0 && M >= 4 && job.start + job.total + S > job.start + job.total;
         auto par = [&](uint64_t m) { return (int)((m + (uint64_t)poff) & 1); };
         LabelJob lj[2];
-        uint32_t nv[2] = {0, 0};
-        bool spec_filled = false;
-        for (uint64_t m = 0; m <= M; m++) {
-            if (m < M && job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; break; }
+        bool pending_mix = false;   // the other parity holds a filled layer that this launch mixes
+        int spec_parity = -1;       // parity of the speculatively filled layer
+        // Each launch fills layer m (staged here) and mixes layer m-1.  Riders go only into the layers this call stages:
+        // a resumed layer 0 and the speculative layer are the range job's alone.  A cancelled job still mixes and
+        // finishes the layer it has filled, so that the riders in it complete.
+        for (uint64_t m = 0;; m++) {
+            bool more = status == B200POST_OK && range_off < job.total;
+            if (more && job.cancel && *job.cancel) { status = B200POST_ERR_CANCELLED; more = false; }
+            if (!more && !pending_mix) break;
             const int b = par(m);
             Layer &l = layer_[b];
             harvest(b);
             bool fill = false;
             uint32_t n_fill = 0;
-            if (m < M) {
-                nv[b] = layer_count(m);
+            if (more) {
                 if (m == 0 && resume) {
-                    lj[b] = LabelJob{d_range_commit_.get(), 0, nullptr, job.start, nv[b], nullptr};   // already filled: X holds its mid-state
+                    next_layer(job, 0, S, false, l);
+                    lj[b] = LabelJob{d_range_commit_.get(), 0, nullptr, job.start, l.plan.n_range, nullptr};   // already filled: X holds its mid-state
                 } else {
-                    if ((rc_ = stage_layer(job, m, b, nv[b], &lj[b]))) return rc_;
-                    fill = true; n_fill = round_up(nv[b], 32);
+                    next_layer(job, range_off, S, host, l);
+                    if ((rc_ = stage_layer(job, b, &lj[b]))) return rc_;
+                    fill = true; n_fill = l.plan.n_slots;
                 }
+                range_off += l.plan.n_range;
             } else if (speculate && status == B200POST_OK) {
                 // one layer past the end of this call: the next initialize() batch, if it comes
                 LabelJob next;
                 Job after = job;                       // the range that would follow this call: [start + total, ...)
                 after.start = job.start + job.total;
-                if ((rc_ = stage_layer(after, 0, b, (uint32_t)S, &next))) return rc_;
-                fill = true; n_fill = (uint32_t)S; spec_filled = true;
+                next_layer(after, 0, S, false, l);     // S labels: speculate needs M >= 4
+                if ((rc_ = stage_layer(after, b, &next))) return rc_;
+                fill = true; n_fill = l.plan.n_slots; spec_parity = b;
             }
-            const uint32_t n_mix = m >= 1 ? round_up(nv[b ^ 1], 32) : 0;
-            if (n_fill == 0 && n_mix == 0) continue;   // resumed call: nothing to launch for m = 0
+            const uint32_t n_mix = pending_mix ? layer_[b ^ 1].plan.n_slots : 0;
+            if (n_fill == 0 && n_mix == 0) { pending_mix = more; continue; }   // resumed call: nothing to launch for m = 0
             PipeParams pp;
             pp.V = V_; pp.x_stride = alloc_slots_; pp.N = (uint32_t)job.N;
             pp.Xfill = l.X.get(); pp.Xmix = layer_[b ^ 1].X.get();
@@ -344,7 +473,7 @@ int DeviceEngine::run_job(const Job &job) {
             static const char *trace_path = getenv("B200POST_CTA_TRACE");
             DeviceBuffer<unsigned long long> d_trace;
             const uint32_t n_cta = (std::max(pp.n_fill, pp.n_mix) + tpb_ - 1) / tpb_;
-            if (trace_path && m >= 1 && m + 1 == M) {
+            if (trace_path && m >= 1 && fill && more && range_off == job.total) {
                 CUDA_TRY(d_trace.resize((size_t)n_cta * 3));
                 CUDA_TRY(cudaMemsetAsync(d_trace.get(), 0, (size_t)n_cta * 24, st));
                 pp.cta_trace = d_trace.get();
@@ -353,7 +482,7 @@ int DeviceEngine::run_job(const Job &job) {
             CUDA_TRY(launch_romix_pipe(mw_, tpb_, dr_unroll_, pp, st));
             CUDA_TRY(cudaEventRecord(l.ev_k2b.get(), st));
             l.k2_pending = true;
-            l.k2_labels = 0.5 * ((fill ? (m < M ? nv[b] : (uint32_t)S) : 0) + (m >= 1 ? nv[b ^ 1] : 0));
+            l.k2_labels = 0.5 * ((fill ? layer_labels(l.plan) : 0) + (pending_mix ? layer_labels(layer_[b ^ 1].plan) : 0));
             g_launches += 1;
             if (d_trace.get()) {
                 std::vector<unsigned long long> h((size_t)n_cta * 3);
@@ -364,16 +493,17 @@ int DeviceEngine::run_job(const Job &job) {
                     fclose(f);
                 }
             }
-            if (m >= 1) {
+            if (pending_mix) {
                 // layer m-3 used the output buffers of this parity.  Waiting for it HERE, after launch m is queued,
                 // keeps one whole launch ahead of the host: a slow wake-up, host copy or PCIe transfer does not
                 // leave the GPU idle between layers.
                 if ((rc_ = retire(job, b ^ 1))) return rc_;
-                if ((rc_ = finish_layer(job, m - 1, b ^ 1, nv[b ^ 1], lj[b ^ 1]))) return rc_;
+                if ((rc_ = finish_layer(job, b ^ 1, lj[b ^ 1]))) return rc_;
             }
+            pending_mix = more;
         }
-        if (spec_filled && status == B200POST_OK) {
-            spec_.valid = true; spec_.N = job.N; spec_.next_start = job.start + job.total; spec_.parity = par(M);
+        if (spec_parity >= 0 && status == B200POST_OK) {
+            spec_.valid = true; spec_.N = job.N; spec_.next_start = job.start + job.total; spec_.parity = spec_parity;
             memcpy(spec_.commitment, cur_commitment_, 32);
         }
     }
@@ -386,8 +516,101 @@ int DeviceEngine::run_job(const Job &job) {
     return status;
 }
 
+void DeviceEngine::end_hosting(int status) {
+    std::lock_guard<std::mutex> lk(rider_mu_);
+    if (!hosting_) return;
+    hosting_ = false;
+    const bool failed = status != B200POST_OK && status != B200POST_ERR_CANCELLED;
+    const std::string err = last_error();
+    for (Rider *r : riders_) {
+        if (failed && r->retired < r->load.placed) {
+            // it had labels in a layer that did not retire: the host job's error is its error
+            r->rc = status; r->err = err; r->done = true;
+        } else {
+            r->load.placed = r->retired;
+            r->released = true;
+        }
+    }
+    riders_.clear();
+    rider_cv_.notify_all();
+}
+
+bool DeviceEngine::ride(Job &job, const std::function<int()> &setup, int *rc) {
+    Rider r;
+    r.load.items = job.total;
+    r.job = &job;
+    const auto t0 = std::chrono::steady_clock::now();
+    {
+        std::unique_lock<std::mutex> lk(rider_mu_);
+        if (!hosting_ || host_N_ != job.N) return false;
+        if (job.cmp) *job.cmp = CompareResult{};
+        riders_.push_back(&r);
+        rider_cv_.wait(lk, [&] { return r.done || r.released; });
+    }
+    const uint64_t rode = r.retired;
+    if (rode == 0 && r.released) return false;   // the range job ended before any layer took it: call() goes on
+    Metrics &mx = metrics();
+    if (r.done) {
+        *rc = r.rc;
+        if (r.rc != B200POST_OK) { set_error(r.err); return true; }
+        mx.gather_calls_total++;
+    } else {
+        // released by a range job that ended first: items [rode, total) run as an ordinary call
+        Job rest = job;
+        rest.total = job.total - rode;
+        rest.indices += rode;
+        if (rest.commitments) rest.commitments += rode * 32;
+        if (rest.commit_index) rest.commit_index += rode;
+        if (rest.out_host) rest.out_host += rode * 16;
+        if (rest.out_dev) rest.out_dev += rode * 16;
+        if (rest.out_hi_dev) rest.out_hi_dev += rode * 16;
+        if (rest.expect_host) rest.expect_host += rode * 16;
+        CompareResult tail;
+        if (job.cmp) rest.cmp = &tail;
+        *rc = call(rest, setup);
+        if (job.cmp) {
+            job.cmp->mismatches += tail.mismatches;
+            for (uint64_t pos : tail.first)
+                if (job.cmp->first.size() < CompareResult::kMaxReported) job.cmp->first.push_back(pos + rode);
+        }
+        if (*rc != B200POST_OK) return true;
+    }
+    if (!job.expect_host) mx.labels_gather_total += rode;
+    mx.rider_calls_total++;
+    mx.rider_labels_total += rode;
+    observe_rider_wait_seconds(std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count());
+    return true;
+}
+
+DeviceEngine::Hold::Hold(DeviceEngine &e, bool locked) : e_(e) { if (!locked) e_.mu_.lock(); }
+
+DeviceEngine::Hold::~Hold() {
+    e_.mu_.unlock();
+    { std::lock_guard<std::mutex> rl(e_.rider_mu_); e_.release_gen_++; }
+    e_.rider_cv_.notify_all();
+}
+
 int DeviceEngine::call(Job &job, const std::function<int()> &setup) {
-    std::lock_guard<std::mutex> lk(mu_);
+    if (!job.gather || job.total == 0 || (job.cancel && *job.cancel)) {
+        Hold hold(*this);
+        return run_call(job, setup);
+    }
+    // A gather waits for the engine or for a range job it can ride, whichever comes first: one that was already waiting
+    // when the range job took the engine rides it too.
+    for (;;) {
+        int rc = B200POST_OK;
+        if (ride(job, setup, &rc)) return rc;
+        uint64_t seen;
+        { std::lock_guard<std::mutex> rl(rider_mu_); seen = release_gen_; }
+        if (mu_.try_lock()) break;
+        std::unique_lock<std::mutex> rl(rider_mu_);
+        rider_cv_.wait(rl, [&] { return release_gen_ != seen || (hosting_ && host_N_ == job.N); });
+    }
+    Hold hold(*this, true);
+    return run_call(job, setup);
+}
+
+int DeviceEngine::run_call(Job &job, const std::function<int()> &setup) {
     CUDA_TRY(cudaSetDevice(dev_));
     if (job.vrf) *job.vrf = VrfResult{};
     if (job.cmp) *job.cmp = CompareResult{};
@@ -399,7 +622,8 @@ int DeviceEngine::call(Job &job, const std::function<int()> &setup) {
     if ((rc = setup())) return rc;
     // A cancelled job has drained what it started: like a finished one it is timed and counted, without its labels.
     const int status = run_job(job);
-    if (status != B200POST_OK && status != B200POST_ERR_CANCELLED) { quiesce(); return status; }
+    if (status != B200POST_OK && status != B200POST_ERR_CANCELLED) { quiesce(); end_hosting(status); return status; }
+    end_hosting(status);
     if (status == B200POST_OK && job.vrf && job.d_diff) {
         CUDA_TRY(cudaMemcpyAsync(h_running_.get(), d_running_.get(), sizeof(VrfCandidate), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
@@ -478,8 +702,10 @@ int DeviceEngine::labels_gather_indexed(size_t n_items, size_t n_commit, const u
                                         const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev,
                                         uint8_t *out_hi_dev) {
     if (out_hi_dev && (!out_dev || out_host)) { set_error("out_hi_dev needs out_dev (and no out_host)"); return B200POST_ERR_INVALID_ARGUMENT; }
+    for (size_t i = 0; commit_index && i < n_items; i++)
+        if (commit_index[i] >= n_commit) { set_error("commitment row index past the commitment table"); return B200POST_ERR_INVALID_ARGUMENT; }
     Job job;
-    job.gather = true; job.commit_index = commit_index; job.indices = indices; job.total = n_items; job.N = N;
+    job.gather = true; job.commit_table = commitments; job.commit_index = commit_index; job.indices = indices; job.total = n_items; job.N = N;
     job.out_host = out_host; job.out_dev = out_dev; job.out_hi_dev = out_hi_dev;
     return call(job, [&]() -> int {
         CUDA_TRY(d_ctab_.grow(n_commit * 32));
@@ -492,7 +718,8 @@ int DeviceEngine::labels_compare_indexed(const uint8_t commitment[32], size_t n_
                                          const uint8_t *expect_host, CompareResult *cmp, const volatile int *cancel) {
     if (!commitment || !indices || !expect_host || !cmp) { set_error("invalid argument"); return B200POST_ERR_INVALID_ARGUMENT; }
     Job job;
-    job.gather = true; job.indices = indices; job.total = n_items; job.N = N; job.expect_host = expect_host; job.cmp = cmp;
+    job.gather = true; job.commit_table = commitment; job.indices = indices; job.total = n_items; job.N = N; job.expect_host = expect_host;
+    job.cmp = cmp;
     job.cancel = cancel;
     return call(job, [&] { return upload_commitment(commitment); });
 }
@@ -504,20 +731,20 @@ void DeviceEngine::quiesce() {
     if (stream_.get()) cudaStreamSynchronize(stream_.get());
     if (copy_stream_.get()) cudaStreamSynchronize(copy_stream_.get());
     cudaGetLastError();
-    for (Layer &l : layer_) { l.pend.live = false; l.k2_pending = false; l.in_pending = false; }
+    for (Layer &l : layer_) { l.pend.live = false; l.pend.riders.clear(); l.k2_pending = false; l.in_pending = false; }
     spec_.valid = false;
     set_error(keep);
 }
 
 uint32_t DeviceEngine::wave_slots(uint64_t N) {
-    std::lock_guard<std::mutex> lk(mu_);
+    Hold lk(*this);
     if (cudaSetDevice(dev_) != cudaSuccess) return 0;
     if (ensure(N, 32) != B200POST_OK) return 0;
     return wave_slots_;
 }
 
 int DeviceEngine::timer_mark(int which) {
-    std::lock_guard<std::mutex> lk(mu_);
+    Hold lk(*this);
     CUDA_TRY(cudaSetDevice(dev_));
     if (which < 0 || which > 1) return B200POST_ERR_INVALID_ARGUMENT;
     if (!stream_.get()) { int rc = ensure(2, 32); if (rc) return rc; }
@@ -527,7 +754,7 @@ int DeviceEngine::timer_mark(int which) {
 }
 
 double DeviceEngine::timer_elapsed_ms() {
-    std::lock_guard<std::mutex> lk(mu_);
+    Hold lk(*this);
     if (!ev_timer_[0].get() || !ev_timer_[1].get() || cudaSetDevice(dev_) != cudaSuccess) return -1.0;
     float ms = 0;
     if (cudaEventSynchronize(ev_timer_[1].get()) != cudaSuccess || cudaEventElapsedTime(&ms, ev_timer_[0].get(), ev_timer_[1].get()) != cudaSuccess) return -1.0;
@@ -535,12 +762,12 @@ double DeviceEngine::timer_elapsed_ms() {
 }
 
 double DeviceEngine::last_call_ms() {
-    std::lock_guard<std::mutex> lk(mu_);
+    Hold lk(*this);
     return last_call_ms_;
 }
 
 void DeviceEngine::romix_time(double *ms_total, uint64_t *launches, double *labels, bool reset) {
-    std::lock_guard<std::mutex> lk(mu_);
+    Hold lk(*this);
     if (ms_total) *ms_total = romix_ms_;
     if (launches) *launches = romix_launches_;
     if (labels) *labels = romix_labels_;

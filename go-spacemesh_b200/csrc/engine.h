@@ -6,7 +6,9 @@
 #include <cuda_runtime.h>
 
 #include <atomic>
+#include <condition_variable>
 #include <cstdint>
+#include <deque>
 #include <functional>
 #include <mutex>
 #include <string>
@@ -14,6 +16,7 @@
 
 #include "label_kernels.cuh"
 #include "cuda_util.h"
+#include "rider_plan.h"
 
 namespace b200post {
 
@@ -63,7 +66,15 @@ public:
                       uint8_t *out_dev = nullptr);
     // same with the commitments given once (n_commit x 32 bytes) and a per-item row index into them: the verify
     // path recomputes ~37 labels per identity, so the commitment H2D shrinks by that factor.  out_hi_dev (optional, only
-    // with out_dev): device buffer of n_items*16 bytes that gets bytes 16-31 of every label32 (K3w instead of K3)
+    // with out_dev): device buffer of n_items*16 bytes that gets bytes 16-31 of every label32 (K3w instead of K3).
+    // A row index past n_commit is B200POST_ERR_INVALID_ARGUMENT.
+    //
+    // Riders: a gather-class call (labels_gather, labels_gather_indexed, labels_compare_indexed) that arrives while a
+    // range job of the same N runs on this engine does not wait for that job to end.  It queues as a rider, the range
+    // job packs queued riders into the free slots of its next layers (FIFO, at most half of each layer, rider_plan.h),
+    // and the call returns once its last chunk has retired.  Riders still queued when the range job ends run as ordinary
+    // calls; a CUDA error in a shared layer fails every rider in it with the host job's code and text.  A rider does not
+    // look at its cancel flag once queued.
     int labels_gather_indexed(size_t n_items, size_t n_commit, const uint8_t *commitments, const uint32_t *commit_index,
                               const uint64_t *indices, uint64_t N, uint8_t *out_host, uint8_t *out_dev,
                               uint8_t *out_hi_dev = nullptr);
@@ -90,6 +101,8 @@ private:
     struct Job {
         bool gather = false;
         const uint8_t *commitments = nullptr;   // gather: n x 32 (host)
+        const uint8_t *commit_table = nullptr;  // indexed gather: the call's n_commit x 32 rows; compare-indexed: its one
+                                                // commitment (host; riders stage from it)
         const uint64_t *indices = nullptr;      // gather: n (host)
         const uint32_t *commit_index = nullptr; // indexed gather: per-item row of the call-level commitment table
                                                 // (gather with neither: every item uses the call's one commitment)
@@ -101,6 +114,20 @@ private:
         uint8_t *out_hi_dev = nullptr;          // gather: bytes 16-31 of each label32 (device, with out_dev; K3w)
         const uint32_t *d_diff = nullptr;
         const volatile int *cancel = nullptr;
+        // the commitment of item i of a gather-class job
+        const uint8_t *row(uint64_t i) const {
+            return commit_index ? commit_table + 32 * (size_t)commit_index[i] : commitments ? commitments + 32 * i : commit_table;
+        }
+    };
+    // A gather-class call queued on a running range job (see labels_gather_indexed).  The caller owns it and blocks
+    // until `done` (result in rc / err) or `released` (the range job ended first: items [retired, items) are left).
+    struct Rider {
+        RiderLoad load;
+        uint64_t retired = 0;            // items whose layers have retired
+        const Job *job = nullptr;
+        bool done = false, released = false;
+        int rc = 0;
+        std::string err;
     };
     // Everything one layer parity owns: its slot buffers, events and in-flight bookkeeping.
     struct Layer {
@@ -123,18 +150,38 @@ private:
         Event ev_k2a, ev_k2b; // bracket the ROMix launch (timed)
         bool in_pending = false, k2_pending = false;
         double k2_labels = 0;
-        struct Pending { uint64_t off; uint32_t n; bool live; } pend{0, 0, false};
+        // the layer being staged: its segments (range labels or a gather's items, then rider chunks) and each chunk's rider
+        LayerPlan plan;
+        std::vector<Rider *> chunk_rider;
+        // the finished layer retire() waits for (the pipelined loop stages this parity again before retiring it)
+        struct Pending { LayerPlan plan; std::vector<Rider *> riders; bool live = false; } pend;
         int allocate(uint32_t slots);   // (re)creates every buffer and event for `slots` slots
     };
-    // the shared body of the label calls: lock, scratch, `setup` (per-call uploads), the timed job, metrics
+    // mu_, held for the scope (locked = already taken by try_lock); its release wakes gathers waiting in call()
+    struct Hold {
+        explicit Hold(DeviceEngine &e, bool locked = false);
+        ~Hold();
+        DeviceEngine &e_;
+    };
+    // the label calls: a gather-class call rides a range job when it can (ride()), else it holds the engine for run_call()
     int call(Job &job, const std::function<int()> &setup);
+    // the shared body of the label calls, mu_ held: scratch, `setup` (per-call uploads), the timed job, metrics
+    int run_call(Job &job, const std::function<int()> &setup);
+    // true when the call rode a range job (*rc: its result, leftovers included); false: not now
+    bool ride(Job &job, const std::function<int()> &setup, int *rc);
+    // the range job in run_job has ended with `status`: fail the riders of its failed layers, release the rest
+    void end_hosting(int status);
+    // l.plan / l.chunk_rider = the next layer of `job` from its item range_off on: at most S of its labels, plus the
+    // queued riders when the job hosts them
+    void next_layer(const Job &job, uint64_t range_off, uint64_t S, bool host, Layer &l);
     int ensure(uint64_t N, uint64_t want_slots);   // (re)allocates scratch; sets wave_slots_
     int run_job(const Job &job);
     int range_call(Job &job, const uint8_t commitment[32], const uint8_t *vrf_difficulty);
     int upload_commitment(const uint8_t commitment[32]);
     // b = buffer parity of the layer (layer index + parity offset of the call)
-    int stage_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, LabelJob *lj);          // inputs + K1
-    int finish_layer(const Job &job, uint64_t layer, int b, uint32_t n_valid, const LabelJob &lj);   // K3 (+K4) + D2H + event
+    // l.plan says which labels: the range segment (or a gather's items) and the rider chunks
+    int stage_layer(const Job &job, int b, LabelJob *lj);          // inputs + K1
+    int finish_layer(const Job &job, int b, const LabelJob &lj);   // K3 (+K4) + D2H + event
     int retire(const Job &job, int buf);
     void harvest(int buf);
     void quiesce();   // after an error: drain the stream, drop in-flight bookkeeping
@@ -142,6 +189,13 @@ private:
     int dev_;
     cudaDeviceProp prop_{};
     std::mutex mu_;
+    // riders: queued gathers and whether a range job (of scrypt-N host_N_) takes them now
+    std::mutex rider_mu_;
+    std::condition_variable rider_cv_;
+    std::deque<Rider *> riders_;
+    bool hosting_ = false;
+    uint64_t host_N_ = 0;
+    uint64_t release_gen_ = 0;             // releases of mu_ so far
     Stream stream_;
     Stream copy_stream_;                   // D2H of finished labels, off the kernels' stream
     // scratch

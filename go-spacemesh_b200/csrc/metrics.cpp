@@ -20,6 +20,15 @@ void observe_verify_seconds(double s) {
     m.verify_seconds_sum_us += (uint64_t)(s * 1e6);
 }
 
+void observe_rider_wait_seconds(double s) {
+    Metrics &m = metrics();
+    double bound = 0.001;
+    for (int k = 0; k < 15; k++, bound *= 2)
+        if (s <= bound) m.rider_wait_bucket[k]++;
+    m.rider_wait_bucket[15]++;   // +Inf
+    m.rider_wait_sum_us += (uint64_t)(s * 1e6);
+}
+
 }  // namespace b200post
 
 using namespace b200post;
@@ -63,6 +72,18 @@ extern "C" size_t b200post_metrics_text(char *buf, size_t cap) {
     line("b200post_prove_sum_blocks_checked_total", "label blocks the proving scan hashed and compared with their checksums (checksummed proofs)", "counter", m.prove_sum_blocks_checked_total);
     line("b200post_prove_sum_blocks_bad_total", "label blocks of checksummed proofs whose stored digest differed from their checksum", "counter", m.prove_sum_blocks_bad_total);
     line("b200post_prove_sum_blocks_healed_total", "bad label blocks a checksummed proof recomputed and scanned from the recomputation", "counter", m.prove_sum_blocks_healed_total);
+    line("b200post_engine_rider_calls_total", "gather calls that rode a running range job's ROMix layers instead of waiting for it", "counter", m.rider_calls_total);
+    line("b200post_engine_rider_labels_total", "labels of rider calls computed in a range job's layers", "counter", m.rider_labels_total);
+    o += "# HELP b200post_engine_rider_wait_seconds rider calls from enqueue to done\n# TYPE b200post_engine_rider_wait_seconds histogram\n";
+    bound = 0.001;
+    for (int k = 0; k < 15; k++, bound *= 2) {
+        char le[32];
+        snprintf(le, sizeof le, "%g", bound);
+        o += std::string("b200post_engine_rider_wait_seconds_bucket{le=\"") + le + "\"} " + std::to_string(m.rider_wait_bucket[k].load()) + "\n";
+    }
+    o += "b200post_engine_rider_wait_seconds_bucket{le=\"+Inf\"} " + std::to_string(m.rider_wait_bucket[15].load()) + "\n";
+    o += "b200post_engine_rider_wait_seconds_sum " + std::to_string(m.rider_wait_sum_us.load() / 1e6) + "\n";
+    o += "b200post_engine_rider_wait_seconds_count " + std::to_string(m.rider_wait_bucket[15].load()) + "\n";
     if (buf && cap) {
         const size_t n = o.size() < cap - 1 ? o.size() : cap - 1;
         memcpy(buf, o.data(), n);

@@ -27,8 +27,14 @@ struct Metrics {
     std::atomic<uint64_t> sums_blocks_checked_total{0}, sums_blocks_bad_total{0}, sums_blocks_repaired_total{0};
     // b200post_generate_proof_sums: digest ranges the scan hashed and compared, found bad, recomputed and scanned
     std::atomic<uint64_t> prove_sum_blocks_checked_total{0}, prove_sum_blocks_bad_total{0}, prove_sum_blocks_healed_total{0};
+    // gathers that rode a range job's layers (DeviceEngine riders): calls, labels computed in shared layers, and the
+    // calls' wait from enqueue to done, a cumulative histogram with upper bounds 1 ms x 2^k (k = 0..14), last = +Inf
+    std::atomic<uint64_t> rider_calls_total{0}, rider_labels_total{0};
+    std::atomic<uint64_t> rider_wait_bucket[16];
+    std::atomic<uint64_t> rider_wait_sum_us{0};
 };
 Metrics &metrics();
 void observe_verify_seconds(double s);
+void observe_rider_wait_seconds(double s);
 
 }  // namespace b200post

@@ -180,7 +180,8 @@ int b200post_wave_slots(uint32_t provider, uint64_t n, uint64_t *slots);
 
 /* Observability: the engine's counters in the Prometheus text exposition format (the reference's metrics for this
  * path: activation/metrics/metrics.go:40-52 post_verification_waiting_total / post_verification_seconds,
- * metrics/public/public.go:19-21).  Writes at most cap-1 bytes + NUL; returns the full length needed. */
+ * metrics/public/public.go:19-21), plus the label engine's riders (gathers that ran in a concurrent init call's
+ * layers: calls, labels, wait histogram).  Writes at most cap-1 bytes + NUL; returns the full length needed. */
 size_t b200post_metrics_text(char *buf, size_t cap);
 
 /* Frees scratch and streams of every device (optional; also runs at library unload). */
