@@ -398,10 +398,29 @@ __global__ void __launch_bounds__(TPB) romix_pipe_kernel(const PipeParams p) {
 // B slots lie past n_slots runs A alone (fill, then mix); a layer of at most S labels has no B at all, so
 // it keeps one label per thread and as many threads as the pipelined kernel would give it.  One launch is a whole layer: no state crosses
 // launches.
+// The step loops hold little besides the BlockMix arithmetic, because the ALU pipe sets the fill phase's pace:
+//  - fill: the lanes write their rows into the warp's 4 KiB tile, whose byte order is the scratchpad row's, and lane 0
+//    sends the tile to HBM with one TMA bulk store.  Tiles are double-buffered per label (single at 512 threads, where
+//    two would not fit in shared memory), so a step waits only on the store issued two steps earlier.
+//  - mix: the 32 row indices pass through shared memory instead of 8 shuffles: each lane stores its j, then reads the
+//    8 it needs for its transposed cp.async requests (4 whole 128-B lines each) with two 16-byte loads.
+// Shared memory per warp: PHASED_BUFS(TPB) x (tile A, tile B), then 2 x 128 B of row indices.
 // =================================================================================================
+#define PHASED_BUFS(tpb) ((tpb) <= 256 ? 2u : 1u)
+#define PHASED_WARP_SMEM(tpb) (PHASED_BUFS(tpb) * 8192u + 256u)
+
+__device__ __forceinline__ void sts32(uint32_t a, uint32_t v) { asm volatile("st.shared.u32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+// bulk_s2g to the 64-bit address {lo, hi}, issued by the lanes with `issue` set, without a branch around it
+__device__ __forceinline__ void bulk_s2g_lohi_if(bool issue, uint32_t lo, uint32_t hi, uint32_t src_smem, uint32_t bytes) {
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 a;\n\tsetp.ne.u32 p, %4, 0;\n\tmov.b64 a, {%0, %1};\n\t"
+                 "@p cp.async.bulk.global.shared::cta.bulk_group [a], [%2], %3;\n\t}"
+                 ::"r"(lo), "r"(hi), "r"(src_smem), "r"(bytes), "r"((uint32_t)issue) : "memory");
+}
+
 template <int MW, int TPB>
 __global__ void __launch_bounds__(TPB) romix_phased_kernel(const RomixParams p) {
     constexpr int DR = 4;
+    constexpr uint32_t BUFS = PHASED_BUFS(TPB);
     extern __shared__ __align__(128) uint8_t smem_raw[];
     const uint32_t T = p.pair_offset;
     const uint32_t slot = blockIdx.x * TPB + threadIdx.x;
@@ -409,20 +428,23 @@ __global__ void __launch_bounds__(TPB) romix_phased_kernel(const RomixParams p) 
     const bool has_b = slot + T < p.n_slots;        // warp-uniform
     const uint32_t lane = threadIdx.x & 31, warp_in_cta = threadIdx.x >> 5;
     const uint32_t N = p.N, mask = N - 1;
-    const uint32_t tile_a = smem_u32(smem_raw) + warp_in_cta * 8192, tile_b = tile_a + 4096;
+    const uint32_t tile_a = smem_u32(smem_raw) + warp_in_cta * PHASED_WARP_SMEM(TPB), tile_b = tile_a + 4096;
+    const uint32_t idx_a = tile_a + BUFS * 8192, idx_b = idx_a + 128;
     const uint32_t own_a = tile_a + lane * 128, own_b = tile_b + lane * 128;
     const uint32_t swz = lane & 7, tr_row = lane >> 3, tr_c = lane & 7;
     const uint32_t tile_a_tr = tile_a + tr_row * 128 + (tr_c << 4), tile_b_tr = tile_b + tr_row * 128 + (tr_c << 4);
+    // lane s's row index sits at word (s & 3) * 8 + (s >> 2); lane t's k-th transposed request needs lane 4k + (t >> 3),
+    // so its 8 indices are the words tr_row * 8 .. tr_row * 8 + 7
+    const uint32_t idx_put = ((lane & 3) * 8 + (lane >> 2)) * 4, idx_get = tr_row * 32;
     const size_t warp = slot >> 5;
+    uint4 *const va = p.V + (warp * 2) * (size_t)N * 256, *const vb = va + (size_t)N * 256;   // row i at + i * 256
     // this lane's base in the warp's two scratchpad regions as {lo, hi} (see romix_pipe_kernel): `hi` is constant
     // within a region
-    const uint64_t va64 = (uint64_t)(p.V + (warp * 2) * (size_t)N * 256 + lane);
-    const uint64_t vb64 = (uint64_t)(p.V + (warp * 2 + 1) * (size_t)N * 256 + lane);
+    const uint64_t va64 = (uint64_t)(va + lane), vb64 = (uint64_t)(vb + lane);
     const uint32_t va_lo = (uint32_t)va64, va_hi = (uint32_t)(va64 >> 32);
     const uint32_t vb_lo = (uint32_t)vb64, vb_hi = (uint32_t)(vb64 >> 32);
-    uint32_t src_lane[8];
-#pragma unroll
-    for (int k = 0; k < 8; k++) src_lane[k] = k * 4 + tr_row;
+    const bool issuer = lane == 0;
+    uint32_t ra = (uint32_t)(uint64_t)va, rb = (uint32_t)(uint64_t)vb;   // low word of row i's address; +4096 per step
 
     uint32_t lo_a[16], hi_a[16], lo_b[16], hi_b[16];
 #pragma unroll
@@ -432,24 +454,28 @@ __global__ void __launch_bounds__(TPB) romix_phased_kernel(const RomixParams p) 
         for (int k = 0; k < 8; k++) set_chunk(lo_b, hi_b, k, p.X[(size_t)k * p.x_stride + slot + T]);
     }
 
-    // own row -> tile (swizzled); after a __syncwarp, tile -> HBM row at {cur, hi} as 8 x 512 contiguous bytes
+    // before a tile is rewritten, the bulk store that last read it has read it (the issuing lane waits; the
+    // __syncwarp after the wait holds the others back)
+#define TILE_FREE()                                                    \
+    {                                                                  \
+        if (BUFS == 2) bulk_wait_read<1>(); else bulk_wait_read<0>(); \
+        __syncwarp();                                                  \
+    }
+    // own row -> tile (swizzled: chunk k at position k ^ (lane & 7), which is where the scratchpad row keeps it)
 #define ROW_TO_TILE(own, lo, hi) \
     _Pragma("unroll") for (int k = 0; k < 8; k++) sts128(own + ((k ^ swz) << 4), ROW_CHUNK(lo, hi, k));
-#define TILE_TO_HBM_K(tile_tr, cur, vhi, k) st_stream_lohi<(k) * 512>(cur, vhi, lds128(tile_tr + (k) * 512));
-#define TILE_TO_HBM(tile_tr, cur, vhi)                                                                          \
-    TILE_TO_HBM_K(tile_tr, cur, vhi, 0) TILE_TO_HBM_K(tile_tr, cur, vhi, 1) TILE_TO_HBM_K(tile_tr, cur, vhi, 2) \
-    TILE_TO_HBM_K(tile_tr, cur, vhi, 3) TILE_TO_HBM_K(tile_tr, cur, vhi, 4) TILE_TO_HBM_K(tile_tr, cur, vhi, 5) \
-    TILE_TO_HBM_K(tile_tr, cur, vhi, 6) TILE_TO_HBM_K(tile_tr, cur, vhi, 7)
     // request row V[Integerify(hi)] of every lane's label into the tile: 8 x (4 rows x 128 B) per warp
-#define ROW_REQUEST_K(tile_tr, j, vlo, vhi, k) \
-    cp_async16_lohi<(k) * 512>(tile_tr + (k) * 512, mad_u32(__shfl_sync(0xffffffffu, j, src_lane[k]), 4096u, vlo), vhi);
-#define ROW_REQUEST(tile_tr, hi, vlo, vhi)                                                                             \
-    {                                                                                                                  \
-        const uint32_t j = hi[0] & mask;                                                                               \
-        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 0) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 1) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 2) \
-        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 3) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 4) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 5) \
-        ROW_REQUEST_K(tile_tr, j, vlo, vhi, 6) ROW_REQUEST_K(tile_tr, j, vlo, vhi, 7)                                  \
-        cp_async_commit();                                                                                             \
+#define ROW_REQUEST_K(tile_tr, jv, vlo, vhi, k) cp_async16_lohi<(k) * 512>(tile_tr + (k) * 512, mad_u32(jv, 4096u, vlo), vhi);
+#define ROW_REQUEST(tile_tr, idx, hi, vlo, vhi)                                                                    \
+    {                                                                                                              \
+        sts32(idx + idx_put, hi[0] & mask);                                                                        \
+        __syncwarp();                                                                                              \
+        const uint4 j0 = lds128(idx + idx_get), j1 = lds128(idx + idx_get + 16);                                   \
+        ROW_REQUEST_K(tile_tr, j0.x, vlo, vhi, 0) ROW_REQUEST_K(tile_tr, j0.y, vlo, vhi, 1)                        \
+        ROW_REQUEST_K(tile_tr, j0.z, vlo, vhi, 2) ROW_REQUEST_K(tile_tr, j0.w, vlo, vhi, 3)                        \
+        ROW_REQUEST_K(tile_tr, j1.x, vlo, vhi, 4) ROW_REQUEST_K(tile_tr, j1.y, vlo, vhi, 5)                        \
+        ROW_REQUEST_K(tile_tr, j1.z, vlo, vhi, 6) ROW_REQUEST_K(tile_tr, j1.w, vlo, vhi, 7)                        \
+        cp_async_commit();                                                                                         \
     }
     // the lane's landed row out of the tile, then X <- BlockMix(X ^ row)
 #define MIX_FROM_TILE(own, lo, hi)                                                                       \
@@ -460,52 +486,69 @@ __global__ void __launch_bounds__(TPB) romix_phased_kernel(const RomixParams p) 
         blockmix_r1_xor<MW, DR>(lo, hi, vlo, vhi);                                                       \
     }
 
-    uint32_t va_cur = va_lo, vb_cur = vb_lo;   // low word of row i's address; +4096 per step
+    uint32_t buf = 0;   // byte offset of this step's tile pair: 0 or 8192
     if (has_b) {
         for (uint32_t i = 0; i < N; i++) {
-            ROW_TO_TILE(own_a, lo_a, hi_a)
-            ROW_TO_TILE(own_b, lo_b, hi_b)
+            TILE_FREE()
+            ROW_TO_TILE(own_a + buf, lo_a, hi_a)
+            ROW_TO_TILE(own_b + buf, lo_b, hi_b)
+            fence_proxy_async_smem();
             __syncwarp();
-            TILE_TO_HBM(tile_a_tr, va_cur, va_hi)
-            TILE_TO_HBM(tile_b_tr, vb_cur, vb_hi)
-            __syncwarp();
-            va_cur = mad_u32(1u, 4096u, va_cur); vb_cur = mad_u32(1u, 4096u, vb_cur);
+            bulk_s2g_lohi_if(issuer, ra, va_hi, tile_a + buf, 4096);
+            bulk_s2g_lohi_if(issuer, rb, vb_hi, tile_b + buf, 4096);
+            bulk_commit();
+            ra = mad_u32(1u, 4096u, ra); rb = mad_u32(1u, 4096u, rb);
+            buf ^= (BUFS - 1) * 8192;
             blockmix_r1_x2<MW, DR>(lo_a, hi_a, lo_b, hi_b);
-        }
-        ROW_REQUEST(tile_b_tr, hi_b, vb_lo, vb_hi)
-        for (uint32_t i = 0; i < N; i++) {
-            ROW_REQUEST(tile_a_tr, hi_a, va_lo, va_hi)
-            asm volatile("cp.async.wait_group 1;" ::: "memory");   // B's row has landed; A's is in flight
-            __syncwarp();
-            MIX_FROM_TILE(own_b, lo_b, hi_b)
-            if (i + 1 < N) {
-                ROW_REQUEST(tile_b_tr, hi_b, vb_lo, vb_hi)
-                asm volatile("cp.async.wait_group 1;" ::: "memory");
-            } else {
-                cp_async_wait_all();
-            }
-            __syncwarp();
-            MIX_FROM_TILE(own_a, lo_a, hi_a)
         }
     } else {
         for (uint32_t i = 0; i < N; i++) {
-            ROW_TO_TILE(own_a, lo_a, hi_a)
+            TILE_FREE()
+            ROW_TO_TILE(own_a + buf, lo_a, hi_a)
+            fence_proxy_async_smem();
             __syncwarp();
-            TILE_TO_HBM(tile_a_tr, va_cur, va_hi)
-            __syncwarp();
-            va_cur = mad_u32(1u, 4096u, va_cur);
+            bulk_s2g_lohi_if(issuer, ra, va_hi, tile_a + buf, 4096);
+            bulk_commit();
+            ra = mad_u32(1u, 4096u, ra);
+            buf ^= (BUFS - 1) * 8192;
             blockmix_r1<MW, DR>(lo_a, hi_a);
         }
+    }
+    // every row is in HBM before any lane requests one, and no store still reads a tile the requests land in
+    bulk_wait_all<0>();
+    __syncwarp();
+#ifndef B200POST_PHASED_FILL_ONLY   // a scratch build of tools/romix_phase_split.py times the fill phase alone
+    if (has_b) {
+        ROW_REQUEST(tile_b_tr, idx_b, hi_b, vb_lo, vb_hi)
+        for (uint32_t i = 0; i + 1 < N; i++) {
+            ROW_REQUEST(tile_a_tr, idx_a, hi_a, va_lo, va_hi)
+            asm volatile("cp.async.wait_group 1;" ::: "memory");   // B's row has landed; A's is in flight
+            __syncwarp();
+            MIX_FROM_TILE(own_b, lo_b, hi_b)
+            ROW_REQUEST(tile_b_tr, idx_b, hi_b, vb_lo, vb_hi)
+            asm volatile("cp.async.wait_group 1;" ::: "memory");
+            __syncwarp();
+            MIX_FROM_TILE(own_a, lo_a, hi_a)
+        }
+        // the last step: no further request of B
+        ROW_REQUEST(tile_a_tr, idx_a, hi_a, va_lo, va_hi)
+        asm volatile("cp.async.wait_group 1;" ::: "memory");
+        __syncwarp();
+        MIX_FROM_TILE(own_b, lo_b, hi_b)
+        cp_async_wait_all();
+        __syncwarp();
+        MIX_FROM_TILE(own_a, lo_a, hi_a)
+    } else {
         for (uint32_t i = 0; i < N; i++) {
-            ROW_REQUEST(tile_a_tr, hi_a, va_lo, va_hi)
+            ROW_REQUEST(tile_a_tr, idx_a, hi_a, va_lo, va_hi)
             cp_async_wait_all();
             __syncwarp();
             MIX_FROM_TILE(own_a, lo_a, hi_a)
         }
     }
+#endif
+#undef TILE_FREE
 #undef ROW_TO_TILE
-#undef TILE_TO_HBM_K
-#undef TILE_TO_HBM
 #undef ROW_REQUEST_K
 #undef ROW_REQUEST
 #undef MIX_FROM_TILE
@@ -782,7 +825,8 @@ size_t romix_smem_bytes(int variant, int tpb) {
     const size_t warps = (size_t)tpb / 32;
     if (variant == ROMIX_COALESCED) return warps * 4096;
     if (variant == ROMIX_BULK) return warps * 8192 + warps * 8;
-    if (variant == ROMIX_PIPELINED || variant == ROMIX_PHASED) return warps * 8192;
+    if (variant == ROMIX_PIPELINED) return warps * 8192;
+    if (variant == ROMIX_PHASED) return warps * PHASED_WARP_SMEM(tpb);
     return 0;
 }
 
