@@ -93,7 +93,14 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
     const size_t per_slot = 128 * (size_t)N * pads;
     size_t free_b = 0, total_b = 0;
     CUDA_TRY(cudaMemGetInfo(&free_b, &total_b));
-    size_t budget = (size_t)((double)(free_b + v_bytes_) * 0.95);   // 0.95: headroom for the k2pow engine's dataset and scratchpads (~14 GiB) when it allocates after this one
+    // V is aligned to the largest per-warp region it can be used with (N * 4 KiB, <= 4 GiB), so that no region straddles
+    // a 4 GiB boundary: the kernels do 32-bit address arithmetic inside one.  The allocation carries that alignment as a
+    // pad, which the budget pays for: 95 % of the HBM that is free or held by V (its pad included), less the pad of a V
+    // for this N.  So the layer does not depend on what V held before, and V plus its pad fits in the share.
+    const size_t align = std::min<size_t>(128 * (size_t)N * 32, (size_t)1 << 32);
+    const size_t held = V_ ? v_bytes_ + v_align_ : 0;
+    const size_t share = (size_t)((double)(free_b + held) * 0.95);   // 0.95: headroom for the k2pow engine's dataset and scratchpads (~14 GiB) when it allocates after this one
+    size_t budget = share > align ? share - align : 0;
     const int64_t cap_mib = o.max_scratch_mib.load();
     if (cap_mib > 0) budget = std::min(budget, (size_t)cap_mib << 20);
     const size_t sms = (size_t)prop_.multiProcessorCount;
@@ -137,9 +144,6 @@ int DeviceEngine::ensure(uint64_t N, uint64_t want_slots) {
         CUDA_TRY(cudaStreamSynchronize(stream_.get()));
         spec_.valid = false;
         V_raw_.reset(); V_ = nullptr; v_bytes_ = 0;
-        // align to the largest per-warp region this allocation can be used with (N * 4 KiB, <= 4 GiB) so
-        // that no region straddles a 4 GiB boundary: the kernels do 32-bit address arithmetic inside one
-        const size_t align = std::min<size_t>(128 * (size_t)N * 32, (size_t)1 << 32);
         CUDA_TRY(V_raw_.resize(need_v + align));
         V_ = reinterpret_cast<uint4 *>(((uintptr_t)V_raw_.get() + align - 1) / align * align);
         v_bytes_ = need_v;

@@ -309,7 +309,8 @@ def test_small_scratch_budget_still_correct(b2, orc):
 
 def test_largest_supported_n(b2, orc):
     """N = 2^20 (128 MiB per scratchpad) is the documented cap: two labels through the low-latency kernel (one launch).
-    test_gpu_romix_matrix.py runs the pipelined and classic kernels over several layers at this N."""
+    test_gpu_romix_matrix.py runs the pipelined and classic kernels over several layers at this N, and
+    test_gpu_romix_phased_matrix.py the phased kernel (test_large_n_ladder, test_largest_layer_uncapped)."""
     c = hashlib.sha256(b"big-n").digest()
     b2.romix_time(reset=True)
     got, _ = b2.labels_range(c, 1 << 20, 7, 2)

@@ -230,7 +230,9 @@ def test_low_latency_slot_mapping(b2, opts, lowlat_items, sms, mw, n):
 def test_largest_n_over_several_layers(b2, orc, opts):
     """N = 2^20: each warp's scratch region is exactly 4 GiB and V is aligned to 4 GiB, which the pipelined kernel's
     32-bit {lo, hi} address arithmetic relies on.  Two pipelined instances over more than one layer and one classic
-    variant agree byte for byte, and a sample (layer seams, ragged tail, random) agrees with the oracle."""
+    variant agree byte for byte, and a sample (layer seams, ragged tail, random) agrees with the oracle.  The phased kernel
+    (the default) at this N, where its B regions start in the next 4 GiB window, is tested by
+    test_gpu_romix_phased_matrix.py::test_large_n_ladder."""
     n = 1 << 20
     c = hashlib.sha256(b"largest-n-layers").digest()
     start = 2**40 - 3

@@ -1,5 +1,5 @@
 """CPU tier: the phased ROMix instances compiled into label_kernels.cu's launch table are exactly the ones
-test_gpu_romix_phased.py runs against the oracle."""
+test_gpu_romix_phased.py and test_gpu_romix_phased_matrix.py run against the oracle."""
 import importlib.util
 import re
 from pathlib import Path
@@ -13,15 +13,21 @@ def _body(signature):
     return SRC[i: SRC.index("\n}\n", i)]
 
 
-def test_phased_instances_are_all_in_the_matrix():
-    spec = importlib.util.spec_from_file_location("romix_phased", Path(__file__).with_name("test_gpu_romix_phased.py"))
+def _matrix(module):
+    spec = importlib.util.spec_from_file_location(module, Path(__file__).with_name(module + ".py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)
+    return mod.PHASED_MATRIX
+
+
+def test_phased_instances_are_all_in_the_matrix():
     cases = re.findall(r"case (\d+): return romix_phased_kernel<MW, (\d+)>;", _body("static romix_fn pick_phased_tpb("))
     assert cases and all(t == t2 for t, t2 in cases)
     masks = {int(x) for x in re.findall(r"X\((\d+)\)", re.search(r"#define B200POST_MW_LIST\(X\)(.*)", SRC).group(1))}
     compiled = {(mw, int(t)) for mw in masks for t, _ in cases}
-    assert len(mod.PHASED_MATRIX) == len(set(mod.PHASED_MATRIX))
-    assert set(mod.PHASED_MATRIX) == compiled
+    for module in ("test_gpu_romix_phased", "test_gpu_romix_phased_matrix"):
+        matrix = _matrix(module)
+        assert len(matrix) == len(set(matrix)), module
+        assert set(matrix) == compiled, module
     # the phased kernel is only reached through its own table: the classic table (pick) does not list it
     assert "ROMIX_PHASED" not in _body("static romix_fn pick(")
